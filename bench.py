@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- prompts/sec classified by the B200 signal-extraction path (BASELINE.json metric).
+"""bench.py -- prompts/sec classified by the H100 (sm_90a) signal-extraction path (BASELINE.json metric).
 
 A "step" = one pass of the hot path (encoder forward + sequence head) over one batch of synthetic prompts.
 Workload at every N: BASELINE.json configs[1] per GPU -- ModernBERT-base intent classifier (L22 H768 I1152
@@ -9,7 +9,7 @@ batch; no data-path collective: prompts are independent, SURVEY.md 8e).
   value  : kernel-only throughput, ids resident in HBM, CUDA-event timed on the launching stream
   e2e    : the same metric through the C-ABI host-buffer call (sr_classify_ids): pinned-host -> device copy of
            the ids and device -> host read of probabilities/classes inside the timed region
-  roofline: dominant kernel = the tcgen05 GEMM launch with the most time; algorithmic FLOPs / CUDA-event time
+  roofline: dominant kernel = the wgmma GEMM launch with the most time; algorithmic FLOPs / CUDA-event time
   cpu_baseline / --impl reference: the oracle restatement of the reference's candle CPU path (torch fp32 CPU,
            one prompt per call = the reference's operating mode) on the box's host cores.
   text_e2e : 256 UTF-8 texts through the reference-facing TEXT call (`classify_batch` of libonnx_semantic_router: the
@@ -19,6 +19,11 @@ Other workloads (`--workload`, not the headline): `cache-1m-768-b1024` / `cache-
 semantic-cache cosine top-8 over 1 M x 768 fp16 rows; under torchrun the rows are sharded over the ranks, every rank
 scans its shard for the whole query batch and ONE NCCL all-gather of 8-byte {score, id} entries + a device merge give
 every rank the global result (checked against the unsharded scan).
+
+--dump-outputs DIR: after the timed steps, the arrays the timed path's caller receives from its last step are written as
+DIR/<name>.npy (float32): logits, probs, cls and conf of the sequence head, and a fixed seeded sample of 256 rows of the
+final hidden state; for cache workloads the top-k ids and scores.  Inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -102,7 +107,7 @@ def config_of(workload, wl, world):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -301,6 +306,30 @@ def peaks():
         return {}
 
 
+def dev_array(ptr, shape, typestr):
+    """Host copy of a device array the library owns (pointer from sr_dev_*), through __cuda_array_interface__."""
+    import torch
+
+    class _Dev:
+        __cuda_array_interface__ = {"data": (int(ptr), False), "shape": tuple(shape), "typestr": typestr, "version": 3}
+    if not ptr:
+        raise RuntimeError("device result pointer is null")
+    return torch.as_tensor(_Dev(), device="cuda").cpu().numpy()
+
+
+def dump_outputs(out_dir, arrays):
+    """DIR/<name>.npy in float32 (float64 where float32 cannot hold the values exactly); 64 MB at most in all."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64 if a.dtype.kind in "iu" and a.size and np.abs(a).max() >= 2 ** 24 else np.float32)
+        total += a.nbytes
+        if total > 64 << 20:
+            raise RuntimeError(f"--dump-outputs: more than 64 MB at {name}")
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def text_e2e_classify(wl, wdir, local_rank, steps):
     """256 texts -> `classify_batch` of libonnx_semantic_router (the reference's only true batch text entry,
     onnx-binding/semantic-router.go:119): tokenizer + H2D + forward + head + D2H inside the timed call."""
@@ -457,38 +486,34 @@ def main_cache(args, wl, rank, world, local_rank):
         pk = peaks()
         rows_local = hi - lo
         if B > 4:
-            peak = pk.get("bf16_tflops") or 1600.0
-            src = "measured (MEASURED_PEAKS.json bf16_tflops: kernel timed alone)" if pk.get("bf16_tflops") else "fallback (B200_PROFILING.md)"
+            peak = pk.get("bf16_tflops") or 989.0
+            src = "measured (MEASURED_PEAKS.json bf16_tflops: kernel timed alone)" if pk.get("bf16_tflops") else "H100 SXM data sheet, dense FP16 (not reached)"
             ach = 2.0 * B * rows_local * D / (scan_ms_max * 1e-3) / 1e12
-            roof = {"bound": "tensor", "kernel": "gemm_kernel<256,EPI_TOPK> (+ select_stage2)", "achieved": ach, "peak": peak,
+            roof = {"bound": "tensor", "kernel": "gemm_kernel<EPI_TOPK> (+ select_stage2)", "achieved": ach, "peak": peak,
                     "unit": "TFLOP/s", "frac": ach / peak, "traffic": None, "peak_source": src,
                     "flops_per_launch": 2.0 * B * rows_local * D, "ms_per_launch": scan_ms_max,
                     "algorithmic_bytes_per_launch": rows_local * D * 2 + B * D * 2 + B * K * 8}
         else:
-            peak = pk.get("hbm_gbs") or 6400.0
-            src = "measured (MEASURED_PEAKS.json hbm_gbs)" if pk.get("hbm_gbs") else "fallback (B200_PROFILING.md)"
+            peak = pk.get("hbm_gbs") or 3350.0
+            src = "measured (MEASURED_PEAKS.json hbm_gbs)" if pk.get("hbm_gbs") else "H100 SXM data sheet, HBM3 (not reached)"
             ach = (rows_local * D * 2 + B * D * 2 + B * K * 8) / (scan_ms_max * 1e-3) / 1e9
             roof = {"bound": "hbm", "kernel": "scores_small_kernel (+ select_stage1/2)", "achieved": ach, "peak": peak,
                     "unit": "GB/s", "frac": ach / peak, "traffic": None, "peak_source": src,
                     "bytes_per_launch": rows_local * D * 2 + B * D * 2 + B * K * 8, "ms_per_launch": scan_ms_max}
-        try:   # the committed ncu capture is of the UNSHARDED store (1 M rows on one GPU): no figure for a shard
-            if world == 1 and wl["rows"] == 1_000_000:
-                roof["traffic"] = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))["dram_bytes_per_launch"].get(
-                    "cache_topk_b1024" if B > 4 else "cache_scores_b1")
-        except Exception:
-            pass
         line = {
             "metric": "cache lookups/sec (cosine top-k over the store)", "value": value, "unit": "queries/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(3, args.warmup), "ms_per_step": ms_max / args.steps,
             "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
             "config": dict(config_of(args.workload, wl, world),
-                           l2_policy=f"the store shard ({rows_local * D * 2 / 1e6:.0f} MB) is streamed every step and exceeds the 126 MB L2" if rows_local * D * 2 > 126e6 else "store shard fits L2 (quick-check workload)"),
+                           l2_policy=f"the store shard ({rows_local * D * 2 / 1e6:.0f} MB) is streamed every step and exceeds the 50 MB L2" if rows_local * D * 2 > 50e6 else "store shard fits L2 (quick-check workload)"),
             "e2e": {"value": e2e_value, "unit": "queries/s", "h2d_bytes_per_step": int(B * D * 4), "d2h_bytes_per_step": int(B * K * 8)},
             "gpu_launches": int(launches), "clocks": clocks, "roofline": roof,
             "exchange": {"collective": "all_gather_into_tensor (NCCL)" if world > 1 else None, "bytes_per_rank": B * K * 8 if world > 1 else 0,
                          "scan_ms": scan_ms_max, "step_ms": ms_max / args.steps},
             "check": check,
         }
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"topk_idx": out[0], "topk_score": out[1]})
         if world == 1 and not args.no_cpu_baseline:
             v, n, dt, nt = cpu_cache_queries_per_s(store, q, args.cpu_budget_s)
             line["cpu_baseline"] = {"value": v, "unit": "queries/s", "cores": nt, "kind": "port",
@@ -510,6 +535,8 @@ def main():
     ap.add_argument("--no-text-e2e", action="store_true")
     ap.add_argument("--qps", type=float, default=100000.0, help="stream workloads: offered load of the whole job (BASELINE cfg 5: 100 k)")
     ap.add_argument("--duration", type=float, default=3.0, help="stream workloads: seconds of arrivals per phase")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", "0"))
@@ -599,6 +626,14 @@ def main():
     ms = ev0.elapsed_time(ev1)
     launches = L.sr_launch_count() - launches0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:   # the device results of the last timed step, before anything else runs
+        Cn_ = wl["classes"]
+        hid = dev_array(L.sr_dev_hidden(h), (T, cfg.hidden_size), "<f4")
+        rows = np.sort(np.random.default_rng(0).choice(T, size=min(256, T), replace=False))
+        dump_outputs(args.dump_outputs, {
+            "logits": dev_array(L.sr_dev_logits(h), (B, Cn_), "<f4"), "probs": dev_array(L.sr_dev_probs(h), (B, Cn_), "<f4"),
+            "cls": dev_array(L.sr_dev_cls(h), (B,), "<i4"), "conf": dev_array(L.sr_dev_conf(h), (B,), "<f4"),
+            "hidden_sample_rows": rows, "hidden_sample": hid[rows]})
     t = torch.tensor([ms], device="cuda", dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -652,20 +687,12 @@ def main():
         peak_tf = pk.get("bf16_tflops_sustained")
         peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained: kernel timed inside a long step)"
         if not peak_tf:
-            peak_tf, peak_src = 1400.0, "fallback (B200_PROFILING.md sustained ~1.4 PFLOP/s)"
+            peak_tf, peak_src = 989.0, "H100 SXM data sheet, dense FP16 (not reached)"
         H, I = cfg.hidden_size, cfg.intermediate_size
         gemm_flops = {2: 2 * T * 3 * H * H, 4: 2 * T * H * H, 5: 2 * T * 2 * I * H, 6: 2 * T * H * I}
         per_launch = {k: (prof_ms[k] / prof_n[k]) if prof_n[k] else None for k in gemm_flops}
         dom = max((k for k in gemm_flops if per_launch[k]), key=lambda k: prof_ms[k])
         achieved = gemm_flops[dom] / (per_launch[dom] * 1e-3) / 1e12
-        traffic = None   # dram__bytes_read.sum + dram__bytes_write.sum of that kernel from the committed ncu capture
-        for tf_name in ("r2_traffic.json", "r1_traffic.json"):
-            try:
-                traffic = json.load(open(os.path.join(ROOT, "profiles", tf_name)))["dram_bytes_per_launch"].get(PC_NAMES[dom])
-                if traffic:
-                    break
-            except Exception:
-                pass
         step_flops = algorithmic_flops_per_token(cfg, S) * T
         breakdown = {PC_NAMES[i]: {"ms_per_step": prof_ms[i] / prof_steps, "launches": prof_n[i] // max(1, prof_steps)}
                      for i in range(8)}
@@ -675,14 +702,14 @@ def main():
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16",
             "data": "synthetic",
             "config": dict(config_of(args.workload, wl, world),
-                           l2_policy="activations per step (>1 GB) exceed the 126 MB L2; no explicit flush"),
+                           l2_policy="activations per step (>1 GB) exceed the 50 MB L2; no explicit flush"),
             "e2e": {"value": e2e_value, "unit": "prompts/s", "h2d_bytes_per_step": int(h2d),
                     "d2h_bytes_per_step": int(d2h)},
             "text_e2e": text,
             "gpu_launches": int(launches),
             "clocks": clocks,
-            "roofline": {"bound": "tensor", "kernel": "gemm_kernel<256," + PC_NAMES[dom] + ">", "achieved": achieved,
-                         "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf, "traffic": traffic,
+            "roofline": {"bound": "tensor", "kernel": "gemm_kernel (" + PC_NAMES[dom] + ")", "achieved": achieved,
+                         "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf, "traffic": None,
                          "peak_source": peak_src, "flops_per_launch": gemm_flops[dom],
                          "ms_per_launch": per_launch[dom]},
             "step_tflops": step_flops / (ms_max / args.steps * 1e-3) / 1e12,

@@ -1,8 +1,8 @@
 /* candle_semantic_router.h -- the drop-in C ABI of libcandle_semantic_router for the signal-extraction path.
  *
  * Every declaration below is the C side of an `extern` in the cgo preamble of
- *   /root/reference/candle-binding/semantic-router.go:27-453            (cited as GO:<line>)
- *   /root/reference/src/semantic-router/pkg/classification/unified_classifier.go:5-82   (cited as UC:<line>)
+ *   candle-binding/semantic-router.go:27-453            (cited as GO:<line>)
+ *   src/semantic-router/pkg/classification/unified_classifier.go:5-82   (cited as UC:<line>)
  * with the struct layouts the GO side declares (SURVEY.md section 8b: "the Go cgo preamble is the contract",
  * not candle-binding/src/ffi/types.rs).  The reference implementation of each symbol is the Rust `#[no_mangle]`
  * function named in the comment (candle-binding/src/ffi/<file>:<line>).
@@ -10,9 +10,9 @@
  * Ownership: inputs are borrowed for the call; arrays/strings in results are malloc'd by the library and
  * released through the matching free_* (all of them are free(3)).  Errors: init_* -> false; classify_* ->
  * class = -1, confidence = 0; EmbeddingResult.error = true; similarity -1.0; int-returning calls -> -1.
- * There is NO CPU path: `use_cpu` is accepted and ignored (logged once); init fails without an sm_100 GPU.
+ * There is NO CPU path: `use_cpu` is accepted and ignored (logged once); init fails without an sm_90 (H100) GPU.
  *
- * "LIVE" = implemented on the B200 engine (BERT / MiniLM / ModernBERT / mmBERT sequence and token classifiers,
+ * "LIVE" = implemented on the CUDA engine (BERT / MiniLM / ModernBERT / mmBERT sequence and token classifiers,
  * embeddings, similarity, batch + unified entries, hallucination detector and NLI).  "STUB" = out of the hot-path scope
  * (SURVEY.md section 2 rows 7-8: Qwen3 / Gemma / multimodal / Qwen3Guard / MLP selector / DeBERTa); exported so the Go
  * package still links, returns the documented failure value.

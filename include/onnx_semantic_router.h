@@ -1,10 +1,10 @@
-/* Drop-in C ABI #2: the symbol table /root/reference/onnx-binding/semantic-router.go binds
+/* Drop-in C ABI #2: the symbol table onnx-binding/semantic-router.go binds
  * (`#cgo LDFLAGS: ... -lonnx_semantic_router`, OX:11).  It reuses candle-binding symbol NAMES with other SIGNATURES
  * (named classifier slots, no model-type argument on the embedding calls, result structs that carry label, full
  * probabilities and timing), so it is a separate library -- libonnx_semantic_router.so -- linked from the same
  * engine objects as libcandle_semantic_router.so.  It is also the reference's only ABI with a true batched classify.
  *
- *   OX:<n>  = /root/reference/onnx-binding/semantic-router.go line <n> (the C preamble that Go compiles against)
+ *   OX:<n>  = onnx-binding/semantic-router.go line <n> (the C preamble that Go compiles against)
  *   RS: ... = the Rust (ONNX Runtime) implementation this entry replaces
  *
  * Model directories: where the reference opens <dir>/model.onnx, this library opens <dir>/model.safetensors (the HF

@@ -1,4 +1,4 @@
-/* sr_b200.h -- additive "side door" C ABI of the B200 signal-extraction library.
+/* sr_b200.h -- additive "side door" C ABI of the H100 (sm_90a) signal-extraction library.
  *
  * NOT part of the reference's Go surface: these entry points take pre-tokenised ids (the reference's text ABI
  * tokenises inside the call, SURVEY.md section 8b "Side-door for measurement") so that parity tests and the
@@ -7,7 +7,7 @@
  *
  * Conventions: plain C, no torch types; `ids` / `cu_seqlens` are int32; sequences are packed back to back,
  * cu_seqlens has batch+1 entries (cu[0] = 0, cu[batch] = total tokens).  Return 0 on success, -1 on error
- * (message on stderr and via sr_last_error()).  There is no CPU fallback: loading fails without an sm_100 GPU.
+ * (message on stderr and via sr_last_error()).  There is no CPU fallback: loading fails without an sm_90 GPU.
  */
 #ifndef SR_B200_H
 #define SR_B200_H
@@ -48,7 +48,7 @@ SR_API int sr_head_num_classes(const sr_model* m, int head);
 SR_API int sr_model_set_head_flavor(sr_model* m, int flavor);
 /* Encoder arithmetic of a ModernBERT / mmBERT model.  0 (default): the production path -- fp16 operands on the tensor cores,
  * fp32 accumulation, residual stream and statistics (logits of the x8-scaled synthetic heads within ~3e-4 RELATIVE of the
- * fp32 reference).  1: the "precise" path -- every GEMM operand as an fp16 hi + lo pair (three tcgen05 passes in one GEMM of
+ * fp32 reference).  1: the "precise" path -- every GEMM operand as an fp16 hi + lo pair (three wgmma passes in one GEMM of
  * triple depth, fp32-equivalent products), fp32 LayerNorm / RoPE / GeGLU / attention in between: logits and embeddings
  * within the 1e-3 ABSOLUTE bound of BASELINE's north star, at about five times the cost.  Parity mode, not a serving mode.
  * Returns -1 for other architectures. */
@@ -89,7 +89,7 @@ SR_API int sr_classify_multi_ids(sr_model* m, const int* heads, int n_heads, con
  * of task t: the SAME base tensors in every directory (checked bit for bit), `X.lora_A.weight` / `X.lora_B.weight` next to
  * the adapted `X.weight`s, its own classifier head, lora_config.json {"rank", "alpha"}.  ONE copy of the base is loaded;
  * a batch then runs ONCE through the encoder as n_tasks copies of its rows, every copy with its own task's rank-r term added
- * inside the projection GEMMs' accumulators (a K extension of the tcgen05 mainloop), instead of n_tasks forwards over
+ * inside the projection GEMMs' accumulators (a K extension of the wgmma mainloop), instead of n_tasks forwards over
  * n_tasks merged models.  token_level[t]: 1 token head, 0 sequence head, -1 from config.json.
  * mode SR_LORA_LOWRANK: as described (one copy of the base: the memory form).  mode SR_LORA_GROUPED: every task's adapters are
  * folded into its own copy of the projection weights at load, the copies are stacked, and each 256-row block of a projection

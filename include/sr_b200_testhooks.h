@@ -43,12 +43,11 @@ SR_API int sr_test_gemm_resid_hl(const void* a_f16, const void* w_f16, void* hi_
 SR_API int sr_test_hl_to_f32(const void* hi_f16, const void* lo_f16, const float* pivot, int t, int hdim, float* x);
 SR_API int sr_test_attention(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int max_len,
                       int num_heads, int window);
+/* the production attention kernel (wgmma): global-layer entry (any window) and sliding-window entry (window >= 1) */
 SR_API int sr_test_attention_tc(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int total_tokens,
                                 int max_len, int num_heads, int window);
 SR_API int sr_test_attention_win(const void* qkv_f16, void* out_f16, const int32_t* d_cu_seqlens, int batch, int total_tokens,
                                  int max_len, int num_heads, int window);
-/* debug: CTA-0 event timeline of the next tcgen05 attention launches into a device buffer of 3 x 4096 int64 (NULL = off) */
-SR_API int sr_test_attention_trace(void* dev_buf_3x4096_i64);
 SR_API int sr_test_layernorm(const float* x, int t, int h, const float* w, const float* b, float eps, float* y32,
                       void* y16);
 

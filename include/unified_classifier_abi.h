@@ -1,5 +1,5 @@
 /* unified_classifier_abi.h -- the cgo preamble of
- *   /root/reference/src/semantic-router/pkg/classification/unified_classifier.go:5-82   (cited as UC:<line>)
+ *   src/semantic-router/pkg/classification/unified_classifier.go:5-82   (cited as UC:<line>)
  * The router's classification package declares these seven entries itself and links them from WHICHEVER binding the
  * build selects: libcandle_semantic_router (unified_classifier_cgo_candle.go:9) or, under `-tags=onnx`,
  * libonnx_semantic_router (unified_classifier_cgo_onnx.go:9).  Both libraries of this repository therefore export them

@@ -2,7 +2,7 @@
 
 Restates, in numpy fp32:
   * embeddingDotProduct + scanLinearForSimilarity + threshold test
-    (/root/reference/src/semantic-router/pkg/cache/inmemory_cache_search.go:14-20,65-89,176):
+    (src/semantic-router/pkg/cache/inmemory_cache_search.go:14-20,65-89,176):
     sequential f32 dot product, best updated on strict `>` (first max wins), nil/expired skipped,
     hit iff best >= threshold.
   * calculate_similarity_batch top-k (candle-binding/src/ffi/embedding.rs:1640-1681):

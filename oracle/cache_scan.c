@@ -1,6 +1,6 @@
 /* C restatement of the reference's Go linear cache scan (TEST INFRASTRUCTURE / CPU BASELINE ONLY).
  *
- * Follows /root/reference/src/semantic-router/pkg/cache/inmemory_cache_search.go:
+ * Follows src/semantic-router/pkg/cache/inmemory_cache_search.go:
  *   embeddingDotProduct       :14-20  -- sequential scalar f32 FMA-free dot product
  *   scanLinearForSimilarity   :65-89  -- bestIndex=-1; update when bestIndex==-1 || dot > best
  * No expiry/nil handling here (all rows valid) -- that is covered by cache_oracle.scan_linear.

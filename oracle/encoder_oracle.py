@@ -21,12 +21,12 @@ so it cannot be run.  What pins this restatement instead:
     reference_long_prompts.json and replayed by tests/test_reference_long_prompts.py (CPU: token counts; GPU: the classifiers).
     It pins the tokenisation / truncation contract, not logits: for the arithmetic the status above stands.
 
-Third-party arithmetic the reference delegates to (not vendored in /root/reference):
+Third-party arithmetic the reference delegates to (not vendored in the reference checkout):
 candle-core / candle-nn / candle-transformers 0.9.2-alpha.1 (candle-binding/Cargo.lock:356-453).
 `BertModel` below restates candle-transformers `models/bert.rs` semantics (post-LN BERT,
 erf-GELU, additive f32::MIN mask).
 
-All citations are relative to /root/reference/candle-binding/src/ unless noted.
+All citations are relative to candle-binding/src/ unless noted.
 """
 from __future__ import annotations
 

@@ -121,7 +121,7 @@ def _attach_hooks(L):
         return
     H = hooks()
     for name in ("sr_test_gemm", "sr_test_gemm_fold", "sr_test_attention", "sr_test_attention_tc", "sr_test_attention_win",
-                 "sr_test_attention_trace", "sr_test_layernorm", "sr_test_bio_decode", "sr_test_hallucination_spans"):
+                 "sr_test_layernorm", "sr_test_bio_decode", "sr_test_hallucination_spans"):
         setattr(L, name, getattr(H, name))
 
 

@@ -2,7 +2,7 @@
 
 The reference keeps every entry's embedding in a Go slice and scans it with a scalar loop under a read lock
 (src/semantic-router/pkg/cache/inmemory_cache_search.go:65-89).  This backend keeps the embeddings in HBM (one fp16 row per
-entry, row i == entries[i]) and asks the B200 library for the best row (`sr_cache_topk`, k = 1: descending score, lowest row
+entry, row i == entries[i]) and asks the CUDA library for the best row (`sr_cache_topk`, k = 1: descending score, lowest row
 first on ties == "first maximum wins"), while everything that is NOT arithmetic stays host bookkeeping with the reference's
 semantics: pending entries (present, not searchable), per-entry and global TTL with the sliding window on a hit, lazy expiry
 at lookup time, O(k) cleanup, FIFO / LRU / LFU eviction with "swap with the last entry".  Every slice mutation has its device

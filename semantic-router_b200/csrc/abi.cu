@@ -1,5 +1,5 @@
 // Drop-in C ABI (include/candle_semantic_router.h): the symbol table candle-binding/semantic-router.go links,
-// implemented over the B200 engine.  Replaces candle-binding/src/ffi/{init,classify,embedding,similarity,
+// implemented over the CUDA engine.  Replaces candle-binding/src/ffi/{init,classify,embedding,similarity,
 // tokenization,memory}.rs.  One global slot per reference OnceLock (ffi/init.rs:19-60,431-456); every result
 // buffer is malloc'd here and released by the matching free_* (free(3)).
 #include "../../include/candle_semantic_router.h"

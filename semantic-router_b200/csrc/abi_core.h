@@ -147,7 +147,7 @@ std::vector<int> env_devices() {
 void note_use_cpu(bool use_cpu) {
   static std::once_flag once;
   if (use_cpu) std::call_once(once, [] {
-    fprintf(stderr, "[srb200] use_cpu=true ignored: this library has no CPU path (runs on sm_100a only)\n");
+    fprintf(stderr, "[srb200] use_cpu=true ignored: this library has no CPU path (runs on sm_90a only)\n");
   });
 }
 bool file_exists(const std::string& p) {

@@ -577,20 +577,18 @@ int sr_test_attention(const void* qkv, void* out, const int32_t* cu, int batch, 
   return attention_fwd(nullptr, static_cast<const __half*>(qkv), static_cast<__half*>(out), cu, batch, max_len,
                        num_heads, 64, window);
 }
+// the production attention kernel (attention_wgmma.cu) through the two entry shapes the engine uses: global layers
+// (window 0) and sliding-window layers
 int sr_test_attention_tc(const void* qkv, void* out, const int32_t* cu, int batch, int total_tokens, int max_len,
                          int num_heads, int window) {
-  return attention_tc_fwd(nullptr, static_cast<const __half*>(qkv), static_cast<__half*>(out), cu, batch, total_tokens,
-                          max_len, num_heads, 64, window);
+  (void)total_tokens;
+  return attention_wgmma_fwd(nullptr, static_cast<const __half*>(qkv), static_cast<__half*>(out), cu, batch, max_len,
+                             num_heads, 64, window);
 }
 int sr_test_attention_win(const void* qkv, void* out, const int32_t* cu, int batch, int total_tokens, int max_len,
                           int num_heads, int window) {
-  return attention_win_fwd(nullptr, static_cast<const __half*>(qkv), static_cast<__half*>(out), cu, batch, total_tokens,
-                           max_len, num_heads, 64, window);
-}
-int sr_test_attention_trace(void* dev_buf_3x4096_i64) {
-  attention_tc_set_trace(static_cast<long long*>(dev_buf_3x4096_i64));
-  attention_win_set_trace(static_cast<long long*>(dev_buf_3x4096_i64));
-  return 0;
+  if (window <= 0) return -1;   // the sliding-window entry needs a window
+  return sr_test_attention_tc(qkv, out, cu, batch, total_tokens, max_len, num_heads, window);
 }
 int sr_test_layernorm(const float* x, int t, int hdim, const float* w, const float* b, float eps, float* y32, void* y16) {
   return layernorm_rows(nullptr, x, t, hdim, w, b, eps, y32, static_cast<__half*>(y16));

@@ -2,14 +2,14 @@
 //
 // Replaces ModernBertAttention::compute_standard_attention + the materialised [B,12,S,S] score tensor and
 // [S,S] local mask of the reference
-// (/root/reference/candle-binding/src/model_architectures/traditional/candle_models/modernbert.rs:121-213,
+// (candle-binding/src/model_architectures/traditional/candle_models/modernbert.rs:121-213,
 //  355-393) and candle BertSelfAttention.  The padding mask ((1-mask)*f32::MIN) and the sliding-window
 // mask (-inf where |i-j| > local_attention/2) are predicates here, never tensors: sequences are packed
 // (cu_seqlens) so padded keys do not exist, and local layers only visit the key blocks inside the window.
 //
-// v1 data path: cp.async double-buffered K/V tiles in XOR-swizzled shared memory, ldmatrix fragments,
-// mma.sync.m16n8k16 (legacy tensor path -- attention is ~7.6 % of the model FLOPs; the GEMMs, 92 %, are
-// tcgen05).  One CTA = 64 query rows of one (sequence, head); 4 warps x 16 rows.
+// Data path: cp.async double-buffered K/V tiles in XOR-swizzled shared memory, ldmatrix fragments,
+// mma.sync.m16n8k16.  The engine runs attention_wgmma.cu; this kernel is its independent comparator in the tests.
+// One CTA = 64 query rows of one (sequence, head); 4 warps x 16 rows.
 #include "kernels.h"
 
 #include "common.cuh"

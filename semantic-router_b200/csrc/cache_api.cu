@@ -1,5 +1,5 @@
 // sr_cache_* : device-resident semantic cache (include/sr_b200.h).  Mirrors the in-memory backend's lookup
-// (/root/reference/src/semantic-router/pkg/cache/inmemory_cache.go:192-234, inmemory_cache_search.go:65-89):
+// (src/semantic-router/pkg/cache/inmemory_cache.go:192-234, inmemory_cache_search.go:65-89):
 // entries are appended, may be invalidated (expired / evicted), and are scanned exhaustively.
 #include <algorithm>
 #include <cstring>

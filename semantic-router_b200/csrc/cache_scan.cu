@@ -2,11 +2,11 @@
 // vectors, then per-query top-k with the reference tie rule.
 //
 // Replaces the Go scalar loop `embeddingDotProduct` + `scanLinearForSimilarity`
-// (/root/reference/src/semantic-router/pkg/cache/inmemory_cache_search.go:14-20,65-89; first max wins) and
+// (src/semantic-router/pkg/cache/inmemory_cache_search.go:14-20,65-89; first max wins) and
 // the stable-sort top-k of `calculate_similarity_batch`
-// (/root/reference/candle-binding/src/ffi/embedding.rs:1640-1681; lower index first on ties).
+// (candle-binding/src/ffi/embedding.rs:1640-1681; lower index first on ties).
 //
-// v1 pipeline: scores[B, chunk] = Q . C^T on the tcgen05 GEMM (fp16 operands, fp32 accumulate, fp32 store;
+// v1 pipeline: scores[B, chunk] = Q . C^T on the wgmma GEMM (fp16 operands, fp32 accumulate, fp32 store;
 // HBM-bound for small B, tensor-bound for B >= ~256), then a two-stage selection:
 //   stage 1: one CTA per (query, 8192-score segment): each warp takes the top-k of its 1024 register-resident scores with
 //            warp shuffles, warp 0 merges the eight lists

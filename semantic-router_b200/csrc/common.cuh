@@ -1,5 +1,5 @@
-// Common device helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM PTX wrappers,
-// warp reductions, vector loads.  Everything here is raw inline PTX for sm_100a -- no CUTLASS/CuTe.
+// Common device helpers for the sm_90a kernels: mbarrier, TMA, warp reductions, vector loads, device math.
+// Everything here is raw inline PTX or CUDA C++ -- no CUTLASS/CuTe.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -162,162 +162,6 @@ __device__ __forceinline__ void sts16(uint8_t* p, uint32_t a, uint32_t b, uint32
 
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 (fp16/bf16 operands, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same with the A operand read from TMEM (lane = row, 32-bit column c holds K elements 2c (low half), 2c+1 (high)).
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Make all previously issued MMAs of this thread arrive on an mbarrier when they complete.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// ---- CTA-pair (cluster of 2, cta_group::2) variants ------------------------------------------------
-// One UMMA spans both SMs of a TPC: M = 256 (each CTA holds 128 rows of A and of D), each CTA stages only its half of
-// the B tile, so shared-memory traffic per flop drops by a third against the 1-CTA 128 x 256 tile.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same shared-memory location in CTA `rank` of this cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load into this CTA's shared memory whose bytes are credited to an mbarrier of the pair's leader CTA
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint32_t leader_bar_addr,
-                                                 int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(leader_bar_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {  // same warp of both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the mbarrier at this offset in every CTA of `cta_mask` once the issued MMAs have completed
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-// TMEM -> registers: this thread's lane (row), 32 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM: this thread's lane (row), 32 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-      "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-      "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major, 128B-swizzled operand tile descriptor (rows x 64 fp16; 8-row groups 1024 B apart).
-//   start address >> 4 [0,14) | LBO (ignored for swizzled K-major, =1) [16,30) | SBO = 1024 B >> 4 [32,46)
-//   | version = 1 [46,48) | layout = SWIZZLE_128B (2) [61,64)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Instruction descriptor, kind::f16: C=F32 (bit 4), A/B format (0 = F16, 1 = BF16) at [7,10)/[10,13),
-// both operands K-major (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n, int ab_fmt = 0) {
-  return (1u << 4) | (static_cast<uint32_t>(ab_fmt) << 7) | (static_cast<uint32_t>(ab_fmt) << 10) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-// ------------------------------------------------------------------------------------------
 // explicit shared-memory vector accesses (avoid generic ST/LD through a converted pointer)
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
@@ -349,10 +193,9 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 // 2^x on the FMA pipe (x <= 0 here; clamped at -125): round-to-nearest integer part through the magic-number add, 2^f on
-// f in [-0.5, 0.5] by a degree-3 polynomial, exponent spliced in with an integer add.  Max relative error 8.4e-5 (minimax fit, tools/micro/ex2_bench.cu checks it) -- a
-// sixth of the fp16 rounding (4.9e-4) the probability gets before the PV MMA.  Blackwell's MUFU still does 16 exp2 per
-// clock per SM while the tensor pipe doubled: the softmax of an attention tile is bounded by that unit, so one score in
-// kPolyOneIn takes this route and the MUFU and FMA pipes work side by side (tools/micro/ex2_bench.cu measures the mix).
+// f in [-0.5, 0.5] by a degree-3 polynomial, exponent spliced in with an integer add.  Max relative error 8.4e-5 (minimax
+// fit, tests/test_device_math_constants.py checks it) -- a sixth of the fp16 rounding (4.9e-4) a softmax probability gets before
+// the PV MMA.  An alternative to the MUFU exp2 for kernels whose softmax is bounded by that unit.
 __device__ __forceinline__ float ex2_poly(float x) {
   x = fmaxf(x, -125.0f);
   const float t = x + 12582912.0f;                    // 1.5 * 2^23
@@ -362,18 +205,9 @@ __device__ __forceinline__ float ex2_poly(float x) {
   p = fmaf(p, f, 0.999919593334198f);
   return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
 }
-// kPolyOneIn = 0: every exponential on the MUFU; 4 / 2: one score in four / two on the FMA pipe (kSlot = column mod 4)
-template <int kPolyOneIn, int kSlot>
-__device__ __forceinline__ float exp2_sel(float x) {
-  if constexpr (kPolyOneIn == 4) return kSlot == 0 ? ex2_poly(x) : ex2(x);
-  else if constexpr (kPolyOneIn == 2) return (kSlot & 1) == 0 ? ex2_poly(x) : ex2(x);
-  else return ex2(x);
-}
-// three-input maximum: one FMNMX3 on sm_100a (halves the instruction count of a row-maximum pass)
+// three-input maximum
 __device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
+  return fmaxf(fmaxf(a, b), c);
 }
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);

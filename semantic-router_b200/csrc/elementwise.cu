@@ -2,7 +2,7 @@
 // L2 normalisation, sequence / token classification heads.  One warp per row, float4 coalesced loads,
 // warp-shuffle reductions, fp32 statistics throughout.
 //
-// Reference semantics (paths relative to /root/reference/candle-binding/src/):
+// Reference semantics (paths relative to candle-binding/src/):
 //   embeddings      model_architectures/traditional/candle_models/modernbert.rs:466 (tok_embeddings -> norm)
 //   LayerNorm       candle_nn::LayerNorm (remove_mean, biased variance, eps inside the sqrt)
 //   mean pooling    model_architectures/traditional/modernbert.rs:1146-1169, embedding/pooling.rs:57-85

@@ -407,9 +407,9 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
   if (device < 0 || device >= ndev) { *err = "invalid device index " + std::to_string(device); return nullptr; }
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     *err = std::string("device ") + prop.name + " is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) +
-           "; this library is built for sm_100a only";
+           "; this library is built for sm_90a only";
     return nullptr;
   }
   if (cudaSetDevice(device) != cudaSuccess) { *err = "cudaSetDevice failed"; return nullptr; }
@@ -972,15 +972,6 @@ int workspace_reserve(Model& m, int tokens, int seqs, size_t out_elems) {
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
-// SRB_ATTN_WIN=0 keeps the mma.sync kernel on the sliding-window layers (A/B measurements)
-static bool attn_win_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("SRB_ATTN_WIN");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-
 // SRB_RESID_HL=0 keeps the fp32 residual stream + fp16 copy on the LayerNorm-fold path (A/B measurements)
 static bool resid_hl_enabled() {
   static const bool on = [] {
@@ -1086,14 +1077,8 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       g.rope_sin = local ? m.rope_sin_l : m.rope_sin_g;
       if (lora_ext(g, ll.qkv, folded, PC_GEMM_QKV)) return -1;
       { ProfScope ps(m, PC_GEMM_QKV); if (run_proj(g)) return -1; }
-      { ProfScope ps(m, PC_ATTN); // global layers: tcgen05 kernel; sliding-window layers: the mma.sync kernel is still faster there (it visits 192
-        // keys per 64-row tile where the 128-row tcgen05 tile must visit 256) -- see DESIGN.md section 3
-        const int win = c.local_attention / 2;
-        int rc;
-        if (!local) rc = attention_tc_fwd(s, w.qkv, w.ctx, d_cu, B, T, max_len, c.heads, 64, 0);
-        else if (win <= 64 && attn_win_enabled()) rc = attention_win_fwd(s, w.qkv, w.ctx, d_cu, B, T, max_len, c.heads, 64, win);
-        else rc = attention_fwd(s, w.qkv, w.ctx, d_cu, B, max_len, c.heads, 64, win);
-        if (rc) return -1; }
+      { ProfScope ps(m, PC_ATTN);   // sliding-window layers visit only the key blocks inside the window
+        if (attention_wgmma_fwd(s, w.qkv, w.ctx, d_cu, B, max_len, c.heads, 64, local ? c.local_attention / 2 : 0)) return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = H; g.A = w.ctx; g.W = lw.wo; g.out = w.x; g.ldo = H;
       g.epi = EPI_RESID; g.resid = w.x; g.ldr = H;
@@ -1136,7 +1121,7 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       g.epi = EPI_F16; g.bias = lw.bqkv;
       if (lora_ext(g, ll.qkv, false, PC_GEMM_QKV)) return -1;
       { ProfScope ps(m, PC_GEMM_QKV); if (run_proj(g)) return -1; }
-      { ProfScope ps(m, PC_ATTN); if (attention_tc_fwd(s, w.qkv, w.ctx, d_cu, B, T, max_len, c.heads, 64, 0, m.cur_kv_lens)) return -1; }
+      { ProfScope ps(m, PC_ATTN); if (attention_wgmma_fwd(s, w.qkv, w.ctx, d_cu, B, max_len, c.heads, 64, 0, m.cur_kv_lens)) return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = Hq; g.A = w.ctx; g.W = lw.wo; g.out = w.x; g.ldo = H;
       g.epi = EPI_RESID; g.resid = w.x; g.ldr = H; g.bias = lw.bo;
@@ -1198,7 +1183,7 @@ int head_tokens(Model& m, int head, int B, int T, int row0) {
   const float* x = w.x + off;
   if (c.arch == ARCH_MODERNBERT) {
     if (hd.has_dense) {
-      // final_norm -> fp16, head.dense on the tcgen05 GEMM, then gelu/LN/classifier per token
+      // final_norm -> fp16, head.dense on the wgmma GEMM, then gelu/LN/classifier per token
       if (layernorm_rows(m.stream, x, T, c.H, m.final_norm_w, nullptr, c.ln_eps, nullptr, w.h + off)) return -1;
       GemmDesc g;
       g.M = T; g.a_rows = w.cap_tokens - row0; g.N = c.H; g.K = c.H; g.A = w.h + off; g.W = hd.dense_w16; g.out = w.ctx + off; g.ldo = c.H;

@@ -60,7 +60,7 @@ struct Head {
   int num_classes = 0;
   bool has_dense = false;          // ModernBERT head.dense / BERT pooler
   float* dense_w32 = nullptr;      // [H,H] fp32 (sequence heads)
-  __half* dense_w16 = nullptr;     // [H,H] fp16 (token heads: dense runs on the tcgen05 GEMM)
+  __half* dense_w16 = nullptr;     // [H,H] fp16 (token heads: dense runs on the wgmma GEMM)
   float* dense_b = nullptr;
   float* norm_w = nullptr;
   float* cls_w = nullptr;

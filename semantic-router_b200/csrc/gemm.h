@@ -1,4 +1,4 @@
-// Host interface of the tcgen05 GEMM (see gemm_tcgen05.cu).
+// Host interface of the wgmma GEMM (see gemm_wgmma.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

@@ -9,28 +9,20 @@ namespace srb {
 
 // kernel-launch accounting (engine.cu): every launcher below bumps it; bench.py reports it as gpu_launches
 void note_launch(int n = 1);
-// SRB_PDL=1 turns programmatic dependent launch on for the tcgen05 kernels (measured neutral: default off)
+// SRB_PDL=1 turns programmatic dependent launch on for the GEMM kernels (default off)
 bool pdl_enabled();
 long long launches_total();
 
-// ---- attention.cu (mma.sync flash attention: v1 kernel, kept as the comparator for the tcgen05 kernel's tests)
+// ---- attention.cu (mma.sync flash attention: the comparator of attention_wgmma.cu in the tests)
 int attention_fwd(cudaStream_t stream, const __half* qkv, __half* out, const int* cu_seqlens, int batch,
                   int max_len, int num_heads, int head_dim, int window);
 
-// ---- attention_tc.cu (tcgen05 / TMEM / TMA flash attention; the production path)
+// ---- attention_wgmma.cu (wgmma flash attention, head dim 64, optional sliding window |i - j| <= window; every layer)
 // kv_lens [batch] (optional, global attention only): keys >= kv_lens[b] of sequence b are masked for EVERY query row while
 // all rows stay queries -- right-padded sequences whose pads are queries, as candle's BertModel sees them under a
 // fixed-padding tokenizer (core/similarity.rs:189-222)
-int attention_tc_fwd(cudaStream_t stream, const __half* qkv, __half* out, const int* cu_seqlens, int batch,
-                     int total_tokens, int max_len, int num_heads, int head_dim, int window, const int* kv_lens = nullptr);
-// One-shot tcgen05 attention for sliding-window layers (window <= 64): a 128-row query tile sees <= 256 keys, so the
-// tile is a single score block (no online softmax).  attention_win.cu.
-int attention_win_fwd(cudaStream_t stream, const __half* qkv, __half* out, const int* cu_seqlens, int batch,
-                      int total_tokens, int max_len, int num_heads, int head_dim, int window);
-
-// debug: device buffer of 3 x 4096 int64 receiving CTA 0's event timeline (nullptr disables)
-void attention_tc_set_trace(long long* dev_buf);
-void attention_win_set_trace(long long* dev_buf);
+int attention_wgmma_fwd(cudaStream_t stream, const __half* qkv, __half* out, const int* cu_seqlens, int batch,
+                        int max_len, int num_heads, int head_dim, int window, const int* kv_lens = nullptr);
 
 // ---- elementwise.cu
 // pos[t] = t - cu_seqlens[seq(t)]

@@ -1,5 +1,5 @@
 // Drop-in C ABI #2 (include/onnx_semantic_router.h): the symbol table onnx-binding/semantic-router.go links
-// (-lonnx_semantic_router), implemented over the same B200 engine as abi.cu.  Replaces
+// (-lonnx_semantic_router), implemented over the same CUDA engine as abi.cu.  Replaces
 // onnx-binding/src/ffi/{classification,embedding,memory,multimodal}.rs and the ONNX Runtime sessions behind them
 // (model_architectures/classification/mmbert_classifier.rs, embedding/mmbert_embedding.rs).
 //

@@ -8,7 +8,7 @@
 //   x = hi + lo        hi = fp16(x), lo = fp16(x - hi)      (|x - hi - lo| <= 2^-22 |x|; lo may be subnormal: still exact enough)
 //   A W^T ~= A_hi W_hi^T + A_lo W_hi^T + A_hi W_lo^T         the dropped A_lo W_lo^T term is 2^-22 relative
 //
-// and runs it as ONE tcgen05 GEMM of three times the depth: A' = [A_hi | A_lo | A_hi] (K' = 3K), W' = [W_hi | W_hi | W_lo].
+// and runs it as ONE wgmma GEMM of three times the depth: A' = [A_hi | A_lo | A_hi] (K' = 3K), W' = [W_hi | W_hi | W_lo].
 // fp16 x fp16 products are exact in fp32 and the accumulator is the fp32 TMEM one, so the result carries fp32-accumulation
 // error only.  Everything between the GEMMs is plain fp32 (LayerNorm, RoPE, GeGLU with erff, softmax attention on the CUDA
 // cores with expf): nothing is rounded to fp16 except through the split.  ~5x the time of the production path; selected

@@ -2,8 +2,8 @@
 // pipelines the reference's models use -- ids, token strings and BYTE offsets into the original text.
 //
 // Replaces the third-party `tokenizers 0.21.4` crate behind
-//   /root/reference/candle-binding/src/core/tokenization.rs:196,218-247,343-395 (UnifiedTokenizer)
-//   /root/reference/candle-binding/src/core/similarity.rs:190-205 (BertSimilarity::get_embedding)
+//   candle-binding/src/core/tokenization.rs:196,218-247,343-395 (UnifiedTokenizer)
+//   candle-binding/src/core/similarity.rs:190-205 (BertSimilarity::get_embedding)
 // Supported components: normalizers BertNormalizer / NFC / NFD / NFKC+NFKD (canonical part only) / Lowercase /
 // StripAccents / Replace(String) / Prepend / Strip / Sequence; pre-tokenizers BertPreTokenizer / Whitespace /
 // WhitespaceSplit / ByteLevel (GPT-2 regex) / Split(String pattern) / Metaspace / Punctuation / Digits / Sequence;

@@ -121,7 +121,7 @@ def test_fails_loudly_without_gpu_or_model(lib):
 
 def test_adapter_probe_and_shared_loader_without_gpu(lib, tmp_path):
     """sr_checkpoint_has_adapters is host code (safetensors header): 1 / 0 / -1; the shared-LoRA loader refuses checkpoints over
-    different bases or without adapters BEFORE it touches a device, and without an sm_100 device it fails loudly like every
+    different bases or without adapters BEFORE it touches a device, and without an sm_90 device it fails loudly like every
     other load (no CPU path)."""
     import numpy as np
     import semantic_router_b200 as pkg

@@ -9,7 +9,7 @@ Tolerances (BASELINE.json north_star: "class indices bit-exact, logits and embed
     classifier is scaled x8 (SURVEY 8d) so logits reach ~13 and an absolute 1e-3 would be 7.7e-5 relative,
     below what fp16 operands (2^-11) can give; the encoder GEMMs run fp16 x fp16 -> fp32 as the north star
     prescribes.  Token-level probabilities (no pooling to average the drift): 3e-3 absolute.
-Measured values are printed (pytest -s) and recorded in DESIGN.md."""
+Measured values are printed (pytest -s)."""
 import os
 import tempfile
 
@@ -232,7 +232,7 @@ def test_modernbert_long_context_embeddings(srlib, cuda):
 def test_minilm_heads_of_32(srlib, cuda):
     """all-MiniLM-L6/L12 shape (SURVEY appendix B: H = 384, 12 heads x 32, FFN 1536), the reference's default similarity
     / cache model: the heads are zero-padded to 64 at load time and run on the head_dim-64 kernels.  Classification and
-    the similarity embedding against the oracle, small ragged batch and a batch large enough for the CTA-pair GEMMs."""
+    the similarity embedding against the oracle, small ragged batch and a batch large enough to give every GEMM worker several tiles."""
     cfg = eo.BertConfig(vocab_size=1000, hidden_size=384, num_attention_heads=12, intermediate_size=1536, num_hidden_layers=3)
     w = synth.make_bert_weights(cfg, 14, seed=13)
     rng = np.random.default_rng(13)
@@ -242,7 +242,7 @@ def test_minilm_heads_of_32(srlib, cuda):
         m = srlib.Model(d, device=0)
         out = m.classify_ids(seqs, pooler_mode=0)
         emb = m.embed_ids(seqs)
-        big = seqs + synth.make_ids(rng, [256] * 12, cfg.vocab_size)        # 3 582 tokens: pair tiles
+        big = seqs + synth.make_ids(rng, [256] * 12, cfg.vocab_size)        # 3 582 tokens: several tiles per worker
         out_big = m.classify_ids(big, pooler_mode=0)
         m.close()
     wt = _t(w)

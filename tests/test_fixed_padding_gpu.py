@@ -1,7 +1,7 @@
 """BertSimilarity under a tokenizer.json that carries fixed-length padding (core/similarity.rs:189-222): the reference clones
 the tokenizer as loaded, so "padding": {"strategy": {"Fixed": n}} -- the sentence-transformers MiniLM files ship it -- makes it
 encode every text to n positions, run the encoder over the pad positions as QUERIES (they are only masked as keys) and divide
-the UNMASKED token sum by the number of real tokens.  Reproduced on the device (sr_embed_ids_padded: kv_lens in the tcgen05
+the UNMASKED token sum by the number of real tokens.  Reproduced on the device (sr_embed_ids_padded: kv_lens in the
 attention, divisor lengths in the pooling) and through the text ABI (init_similarity_model / get_text_embedding /
 calculate_similarity); expected values from the oracle fed with the padded ids and mask HuggingFace `tokenizers` produces."""
 import ctypes as C

@@ -27,7 +27,7 @@ def _gemm(lib, a, w, out, epi, bias=None, resid=None, pos=None, cos=None, sin=No
 
 @pytest.mark.parametrize("M,N,K", [(128, 256, 64), (128, 768, 768), (300, 2304, 768), (1000, 768, 1152),
                                    (77, 384, 384), (4096, 768, 768), (1, 256, 768), (129, 1152, 384),
-                                   (2177, 2304, 768), (2048, 256, 64), (5000, 768, 1152)])  # M >= 2048: CTA-pair tiles
+                                   (2177, 2304, 768), (2048, 256, 64), (5000, 768, 1152)])  # M >= 2048: many row blocks per worker
 def test_gemm_f16_store(srlib, cuda, M, N, K):
     g = torch.Generator(device="cuda").manual_seed(M * 7 + N)
     a = torch.randn(M, K, device=cuda, generator=g).half()
@@ -279,7 +279,7 @@ def test_gemm_layernorm_fold_pivot(srlib, cuda):
     torch.testing.assert_close(out.float(), ref, rtol=3e-3, atol=3e-3)
 
 
-@pytest.mark.parametrize("M,K", [(300, 768), (700, 1152), (2500, 768), (4224, 1152)])   # M >= 2048: CTA-pair tiles
+@pytest.mark.parametrize("M,K", [(300, 768), (700, 1152), (2500, 768), (4224, 1152)])   # M >= 2048: many row blocks per worker
 def test_gemm_resid_fp16_pair(srlib, cuda, M, K):
     """EPI_RESID_HL: the residual stream as an fp16 pair, in place -- x - pivot = hi + lo.  Three chained GEMMs on rows with a
     large common offset: after each one hi + lo + pivot_out must equal the fp32 reference to ~2^-22 of the row spread, hi must

@@ -2,7 +2,7 @@
 pkg/classification/unified_classifier.go:113): three task checkpoints over ONE base -- intent (sequence head), PII (token head),
 security (sequence head); ranks 8 / 16 / 32, their own alpha, not every projection adapted -- load as one model
 (sr_model_load_lora_shared) and a batch runs ONCE through the encoder, every task's copy of the rows with its own rank-r term
-added inside the projection GEMMs (K extension of the tcgen05 mainloop).  Expected values: the oracle on the MERGED weights
+added inside the projection GEMMs (K extension of the wgmma mainloop).  Expected values: the oracle on the MERGED weights
 W + (alpha / r) B A of each task (merge_weights, lora_adapter.rs:157-168), i.e. what three separate forwards would give;
 and the three-slot path of this library (load-time fold) on the same inputs."""
 import json

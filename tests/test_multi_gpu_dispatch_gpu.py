@@ -1,4 +1,4 @@
-"""In-library multi-GPU dispatch on real hardware (needs >= 2 visible GPUs: `gpurun --gpus 2`; skipped on one).
+"""In-library multi-GPU dispatch on real hardware (needs >= 2 visible GPUs; skipped on one).
 The reference router is ONE process (a goroutine per signal per request, classifier_signal_dispatch.go:114-129); the
 library replicates each slot on every visible GPU and spreads callers / batch pieces over them (abi_core.h).  The C
 harness plays the cgo side with 64 OS threads: every answer equals the single-threaded one to 1e-6 whichever GPU served

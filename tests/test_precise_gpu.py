@@ -1,6 +1,6 @@
 """The strict bound of BASELINE's north star -- "logits and embeddings within 1e-3 fp32" -- as an ABSOLUTE bound on the logits
 of the x8-scaled synthetic heads (SURVEY 8d), met by the precise path (sr_model_set_precise: every GEMM operand as an fp16
-hi + lo pair on the same tcgen05 kernel, fp32 in between; csrc/precise.cu), at 5 layers and at the full 22-layer depth.
+hi + lo pair on the same wgmma kernel, fp32 in between; csrc/precise.cu), at 5 layers and at the full 22-layer depth.
 Also measured here: what the production (fp16-operand) path gives on the same inputs, and its error on an UN-scaled head
 (classifier std 0.02, logits ~1): that is inside 1e-3 absolute without the precise path."""
 import tempfile

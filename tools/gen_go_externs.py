@@ -1,12 +1,12 @@
 """Parses the cgo preambles of the reference's Go files (the drop-in contract, SURVEY.md section 8b) into
 tests/golden/go_externs.json: for each of the three preambles the list of C function names Go links.
-/root/reference does not exist on the GPU box, so the list is committed as a fixture; re-run here when the reference moves.
+The reference checkout is not needed at test time: the list is committed as a fixture; re-run here when the reference moves.
     python tools/gen_go_externs.py"""
 import json
 import os
 import re
 
-REF = "/root/reference"
+REF = os.environ.get("SR_REFERENCE_DIR", "reference")   # checkout of vllm-project/semantic-router
 FILES = {
     "candle": "candle-binding/semantic-router.go",
     "onnx": "onnx-binding/semantic-router.go",

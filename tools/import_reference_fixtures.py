@@ -1,4 +1,4 @@
-"""Brings the reference-held test vectors of the hot path into tests/golden/ (the GPU box has no /root/reference).
+"""Brings the reference-held test vectors of the hot path into tests/golden/ (tests must not depend on a reference checkout).
 The only vector the reference holds for this path is candle-binding/test_data/long_prompt_fixtures.json: three prompts
 (~3 600 / ~7 300 / ~21 tokens) that its Rust and Go tests push through the 512-token classification cap
 (onnx-binding/src/model_architectures/classification/mmbert_classifier.rs:1250-1420,
@@ -7,7 +7,7 @@ Kept: id, text, the reference's own token estimates and its cap.      python too
 import json
 import os
 
-SRC = "/root/reference/candle-binding/test_data/long_prompt_fixtures.json"
+SRC = os.path.join(os.environ.get("SR_REFERENCE_DIR", "reference"), "candle-binding/test_data/long_prompt_fixtures.json")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 if __name__ == "__main__":
