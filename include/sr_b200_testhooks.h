@@ -40,6 +40,9 @@ SR_API int sr_test_gemm_fold(const void* a_f16, const void* w_f16, void* out, in
 SR_API int sr_test_gemm_resid_hl(const void* a_f16, const void* w_f16, void* hi_f16, void* lo_f16, int m, int n, int k,
                                  const float* bias, float* row_stats, float* pivot_out, const float* pivot_in,
                                  const float* pivot_in_stats);
+/* The thread-block cluster the GEMM launches for (epilogue, N, K): cluster_n CTAs on neighbouring column tiles of one row
+ * block share each A k-block (1: no clusters); workers = clusters of its persistent grid on this device. */
+SR_API int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers);
 SR_API int sr_test_hl_to_f32(const void* hi_f16, const void* lo_f16, const float* pivot, int t, int hdim, float* x);
 SR_API int sr_test_attention(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int max_len,
                       int num_heads, int window);

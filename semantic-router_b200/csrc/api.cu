@@ -570,6 +570,12 @@ int sr_test_gemm_resid_hl(const void* a, const void* w, void* hi, void* lo, int 
   g.pivot_out = pivot_out; g.pivot_in = pivot_in; g.pivot_in_stats = pivot_in_stats;
   return gemm_f16(nullptr, g);
 }
+int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers) {
+  if (!cluster_n || !workers) return -1;
+  *cluster_n = gemm_cluster_size(epi, n, k);
+  *workers = gemm_cluster_workers(epi, n, k);
+  return *workers > 0 ? 0 : -1;
+}
 int sr_test_hl_to_f32(const void* hi, const void* lo, const float* pivot, int t, int hdim, float* x) {
   return hl_to_f32(nullptr, static_cast<const __half*>(hi), static_cast<const __half*>(lo), pivot, t, hdim, x);
 }

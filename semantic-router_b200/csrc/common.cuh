@@ -135,6 +135,30 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorM
       "r"(c1), "l"(policy)
       : "memory");
 }
+// The same load, delivered to every CTA of the cluster whose bit is set in `cta_mask`: the box lands at the same shared
+// offset in each of them and signals the mbarrier at the same offset in each of them (complete_tx of the box bytes).
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0),
+      "r"(c1), "h"(cta_mask)
+      : "memory");
+}
+// Arrive on the mbarrier at the same shared offset as `bar` in CTA `cta` of the cluster (cluster rank; may be this CTA).
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
+// Every thread of every CTA of the cluster (a plain CTA barrier when the kernel runs without clusters).
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;
 constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
 constexpr uint64_t kEvictNormal = 0x1000000000000000ull;

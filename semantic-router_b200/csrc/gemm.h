@@ -85,6 +85,11 @@ struct GemmDesc {
 };
 
 int gemm_f16(cudaStream_t stream, const GemmDesc& g);
+// Thread-block cluster size gemm_f16 launches for a GEMM: that many CTAs, on neighbouring column tiles of one row block,
+// share each A k-block (1: no clusters).
+int gemm_cluster_size(int epi, int N, int K);
+// Workers of its persistent grid: co-resident clusters of that shape on the current device (SMs without clusters).
+int gemm_cluster_workers(int epi, int N, int K);
 int make_tmap_f16_kmajor(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t k, uint32_t box_rows);
 
 }  // namespace srb

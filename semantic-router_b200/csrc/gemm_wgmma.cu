@@ -11,10 +11,15 @@
 //   * warps 0..3  : epilogue (shared fp32 tile -> registers, one row per lane -> fused math -> swizzled box -> TMA store)
 //   * the accumulator tile in shared memory is the hand-off: the epilogue of tile i overlaps the mainloop of tile i+1,
 //     whose accumulators live in the MMA warpgroup's registers until the epilogue has released the shared tile.
+//   * thread-block clusters (gemm_cluster_size): the cn CTAs of a cluster compute neighbouring column tiles of one row
+//     block; each loads a 1/cn slice of the shared A box and multicasts it (TMA .multicast::cluster), and frees a
+//     stage by arriving on the empty barrier of every CTA that wrote into it.  Tiles, the wgmma sequence,
+//     the accumulation order and the epilogues are the same as without clusters: results are bitwise identical.
 // Fused epilogues: bias, RoPE (rotate-half, modernbert.rs:61-85), fp32 residual add (:300-303),
 // GeGLU = gelu_erf(a)*b (:238), erf-GELU (BERT intermediate).
 #include "gemm.h"
 
+#include <atomic>
 #include <cstdlib>
 #include <mutex>
 
@@ -143,7 +148,9 @@ __device__ __forceinline__ void fold_scale(float rstd, uint32_t* a, uint32_t* b)
   }
 }
 
-template <int EPI>
+// CN: thread-block cluster size -- CN neighbouring column tiles of one row block share A (1: no clusters; a compile-time
+// constant, so that the unclustered instantiations carry none of the cluster arithmetic)
+template <int EPI, int CN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_aux,
@@ -174,23 +181,34 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int k1_blocks = (p.K + BK - 1) / BK;
   // K extension: the accumulator also takes A2[M, K2] x W2[N, K2]^T -- same stages, same MMAs, other tensor maps
   const int k_blocks = k1_blocks + (p.K2 + BK - 1) / BK;
-  const int num_tiles = m_blocks * n_blocks;
+  // Thread-block clusters of cn CTAs along N (1: none).  The schedule below hands out CLUSTER tiles -- cn neighbouring
+  // 128 x 128 tiles of one row block -- and CTA rn of the cluster computes tile (m_c, cn n_c + rn) of cluster tile
+  // (m_c, n_c).  The cn CTAs share the A row block: each loads a 1/cn slice of the A box and multicasts it to all of
+  // them, so an A k-block is read out of L2 once per cluster instead of once per CTA.  All CTAs of a cluster walk the
+  // same cluster tiles and k-blocks in lockstep; a tile past N is still loaded (TMA zero-fills) and computed, and its
+  // stores are skipped.  (Sharing W across row blocks as well was measured slower at every projection shape.)
+  constexpr int cn = CN;
+  const int rn = blockIdx.x % cn;
+  const int n_cblocks = (n_blocks + cn - 1) / cn;
+  const int num_tiles = m_blocks * n_cblocks;   // cluster tiles (= tiles without clusters)
+  auto tile_m = [&](int t) { return t / n_cblocks; };
+  auto tile_n = [&](int t) { return (t % n_cblocks) * cn + rn; };
   auto row_base = [&](int m_blk) { return m_blk * BM; };
-  // contiguous tile range per CTA (n fastest): one CTA walks all N tiles of an M block back to back, so the
+  // contiguous tile range per cluster (n fastest): one cluster walks all N tiles of its M blocks back to back, so the
   // A row-block stays hot in L2 and per-row epilogue state (RoPE cos/sin) is reused across tiles
-  const int num_workers = gridDim.x;
+  const int num_workers = gridDim.x / cn;
   const int base = num_tiles / num_workers, rem = num_tiles % num_workers;
-  const int bid = blockIdx.x;
+  const int bid = blockIdx.x / cn;   // worker = cluster
   int t_begin = bid * base + (bid < rem ? bid : rem);
   int t_end = t_begin + base + (bid < rem ? 1 : 0);
   // EPI_TOPK, grouped schedule (p.grouped): worker w owns query block w % m_blocks for its whole life (its running
   // top-8 lists live in registers) and walks the stored-row tiles g, g + G, g + 2G, ... with g = w / m_blocks,
   // G = workers / m_blocks.  The m_blocks workers of a group therefore ask for the SAME stored-row tile at about the
   // same time: one HBM read, the rest L2 hits -- the store streams once per batch instead of once per query block.
-  // Tiles are numbered t = m_blk * n_blocks + n_blk as everywhere else; `t_step` is the distance between two tiles of
-  // this worker (1 for the contiguous ranges).
+  // Tiles are numbered t = m_blk * n_blocks + n_blk as everywhere else (EPI_TOPK runs without clusters: cluster tiles
+  // are tiles); `t_step` is the distance between two tiles of this worker (1 for the contiguous ranges).
   int t_step = 1;
-  // Interleaved schedule (p.interleave; the residual GEMMs): worker w takes tiles w, w + W, w + 2W, ...  With
+  // Interleaved schedule (p.interleave; the residual GEMMs): worker (cluster) w takes tiles w, w + W, w + 2W, ...  With
   // n fastest in the tile numbering the N / BN tiles of one row block run AT THE SAME TIME on neighbouring workers, so
   // each A k-block is pulled from HBM once and hit in L2 by the others, where the contiguous ranges could lose the row
   // block from L2 to the residual stream passing through between two tiles of one worker.
@@ -217,14 +235,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 4);        // one arrival per MMA warp
+      // one arrival per MMA warp of every CTA this CTA's producer multicasts into: the cn CTAs of its cluster
+      mbar_init(&empty_bar[s], 4 * cn);
     }
     mbar_init(tfull_bar, 128);            // every thread of the MMA warpgroup, after its fragment stores
     mbar_init(tempty_bar, kEpiWarps);
     for (int i = 0; i < kEpiWarps * kStageBufs; ++i) mbar_init(&resid_bar[i], 1);
     mbar_fence_init();
   }
-  __syncthreads();
+  // no CTA of the cluster multicasts into another or arrives on its barriers before those barriers exist
+  if constexpr (CN > 1) cluster_sync();
+  else __syncthreads();
   // PDL: everything above overlapped the previous kernel's tail; nothing below may start before its writes are visible
   griddep_launch_dependents();
   griddep_wait();
@@ -234,8 +255,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     if (lane == 0) {
       int s = 0;
       uint32_t ph = 0;
+      // this CTA's slice of the shared A box (tensor-map box height BM / cn rows, a multiple of the 8-row swizzle atom,
+      // so the slices assemble into exactly the tile layout one full-box load would give), multicast to the whole cluster
+      const int a_rows = BM / cn;
+      const uint16_t a_mask = static_cast<uint16_t>((1u << cn) - 1);
       for (int t = t_begin; t < t_end; t += t_step) {
-        const int m_blk = t / n_blocks, n_blk = t % n_blocks;
+        const int m_blk = tile_m(t), n_blk = tile_n(t);
         // grouped weights (one matrix per task, stacked along N): the row block picks its matrix; blocks never straddle
         // two groups (grp_rows is a multiple of the block height, checked on the host)
         const int w_row0 = p.grp_rows > 0 ? ((m_blk * BM) / p.grp_rows) * p.N : 0;
@@ -245,8 +270,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           const CUtensorMap* ma = ext ? &tmap_a2 : &tmap_a;
           const CUtensorMap* mb = ext ? &tmap_b2 : &tmap_b;
           const int kc = (ext ? kb - k1_blocks : kb) * BK;
+          // the stage fills with the A slices of every CTA of the cluster and this CTA's own W box: the whole stage
           mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
-          tma_load_2d(smem_a + s * Cfg::kABytes, ma, &full_bar[s], kc, m_blk * BM);
+          uint8_t* da = smem_a + s * Cfg::kABytes + rn * a_rows * (BK * 2);
+          const int ya = m_blk * BM + rn * a_rows;
+          if (cn > 1) tma_load_2d_multicast(da, ma, &full_bar[s], kc, ya, a_mask);
+          else tma_load_2d(da, ma, &full_bar[s], kc, ya);
           tma_load_2d(smem_b + s * Cfg::kBBytes, mb, &full_bar[s], kc, (ext ? 0 : w_row0) + n_blk * BN);
           if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
         }
@@ -259,6 +288,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     int s = 0;
     uint32_t ph = 0;
     uint32_t eph = 0;   // tempty phase
+    // a stage of this CTA is written by the producers of every CTA of its cluster (A slices): freeing it is one
+    // arrival on the empty barrier of each of them, lane i for CTA i, so that the arrivals go out side by side on the
+    // MMA warp's critical path
+    auto release = [&](int st) {
+      if (cn == 1) {
+        if (lane == 0) mbar_arrive(&empty_bar[st]);
+      } else if (lane < cn) {
+        mbar_arrive_cluster(&empty_bar[st], lane);
+      }
+    };
     for (int t = t_begin; t < t_end; t += t_step) {
       int prev = -1;
       for (int kb = 0; kb < k_blocks; ++kb) {
@@ -278,13 +317,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         // the previous stage's MMAs have completed once at most this stage's group is pending: free that stage
         wgmma_wait<1>();
         __syncwarp();
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (prev >= 0) release(prev);
         prev = s;
         if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
       }
       wgmma_wait<0>();
       __syncwarp();
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (prev >= 0) release(prev);
       // hand the tile to the epilogue once it has read out the previous one
       mbar_wait(tempty_bar, eph ^ 1);
       eph ^= 1;
@@ -335,18 +374,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     const bool use_resid = (EPI == EPI_RESID) && p.has_resid;
 
     // EPI_RESID: residual boxes are TMA-loaded one chunk ahead (flat over (tile, chunk) of this CTA)
-    auto out_col = [&](int t, int c) { return (t % n_blocks) * (BN / kAccPerChunk * kOutPerChunk) + c * kOutPerChunk; };
+    auto out_col = [&](int t, int c) { return tile_n(t) * (BN / kAccPerChunk * kOutPerChunk) + c * kOutPerChunk; };
     auto chunk_valid = [&](int t, int c) { return t < t_end && out_col(t, c) < n_out; };
     auto issue_resid = [&](int t, int c, int buf) {  // lane 0 only
       if constexpr (kHL) {   // buf = pair index: hi box, then lo box, one barrier for both
         uint8_t* pb = my_bufs + buf * 2 * kStageBufBytes;
         mbar_expect_tx(&my_rbar[buf], 2 * kStageBufBytes);
-        tma_load_2d(pb, &tmap_out, &my_rbar[buf], out_col(t, c), row_base(t / n_blocks) + quad * 32);
-        tma_load_2d(pb + kStageBufBytes, &tmap_aux, &my_rbar[buf], out_col(t, c), row_base(t / n_blocks) + quad * 32);
+        tma_load_2d(pb, &tmap_out, &my_rbar[buf], out_col(t, c), row_base(tile_m(t)) + quad * 32);
+        tma_load_2d(pb + kStageBufBytes, &tmap_aux, &my_rbar[buf], out_col(t, c), row_base(tile_m(t)) + quad * 32);
       } else {
         mbar_expect_tx(&my_rbar[buf], kStageBufBytes);
         tma_load_2d(my_bufs + buf * kStageBufBytes, &tmap_out, &my_rbar[buf], out_col(t, c),
-                    row_base(t / n_blocks) + quad * 32);
+                    row_base(tile_m(t)) + quad * 32);
       }
     };
     // residual prefetch cursor: runs kAhead chunks in front of the chunk being processed (flat over this CTA's
@@ -354,11 +393,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     constexpr int kRing = kHL ? kPairs : kStageBufs;   // residual-load ring: boxes, or box pairs
     constexpr int kAhead = kHL ? 1 : (kStageBufs - 2 > 0 ? kStageBufs - 2 : 1);
     int pf_t = t_begin, pf_c = 0, pf_buf = 0;
+    // a tile wholly past N (the second CTA of a cluster on an odd last column) has no chunk: the epilogue skips it,
+    // and so must the cursor, or it would wait on that tile for good and starve every later tile of its residual
+    auto pf_skip = [&]() { while (pf_t < t_end && out_col(pf_t, 0) >= n_out) pf_t += t_step; };
+    pf_skip();
     auto pf_issue = [&]() {  // lane 0 only
       if (!chunk_valid(pf_t, pf_c)) return;
       issue_resid(pf_t, pf_c, pf_buf);
       if (++pf_buf == kRing) pf_buf = 0;
-      if (++pf_c >= kChunks || !chunk_valid(pf_t, pf_c)) { pf_t += t_step; pf_c = 0; }
+      if (++pf_c >= kChunks || !chunk_valid(pf_t, pf_c)) { pf_t += t_step; pf_c = 0; pf_skip(); }
     };
     if ((use_resid || kHL) && lane == 0) {
 #pragma unroll
@@ -386,7 +429,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       }
     };
     for (int t = t_begin; t < t_end; t += t_step) {
-      const int m_blk = t / n_blocks, n_blk = t % n_blocks;
+      const int m_blk = tile_m(t), n_blk = tile_n(t);
       const int row0 = row_base(m_blk) + quad * 32;
       if constexpr (EPI == EPI_TOPK) {
         if (m_blk != tk_mblk) {
@@ -740,7 +783,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     if (lane == 0) bulk_wait_read<0>();  // smem must outlive the last stores' reads
     __syncwarp();
   }
-  __syncthreads();
+  // no CTA leaves while another of its cluster may still arrive on its barriers
+  if constexpr (CN > 1) cluster_sync();
+  else __syncthreads();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -764,27 +809,70 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-template <int EPI>
+// Clusters of CN CTAs of gemm_kernel<EPI, CN> that are co-resident on the device.  A GPC holds a whole number of
+// clusters, so this is the occupancy query's answer, not num_sms / CN.  Asked once per epilogue and cluster size
+// (all devices of one box are the same part).
+template <int EPI, int CN>
+int max_clusters(int num_sms) {
+  constexpr int csize = CN;
+  static std::atomic<int> cached{0};
+  int n = cached.load(std::memory_order_relaxed);
+  if (n > 0) return n;
+  SRB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<EPI, CN>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<EPI>::kSmemBytes));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(csize * num_sms);
+  cfg.blockDim = dim3(kGemmThreads);
+  cfg.dynamicSmemBytes = GemmCfg<EPI>::kSmemBytes;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = csize;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  SRB_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&n, gemm_kernel<EPI, CN>, &cfg));
+  if (n <= 0) {
+    fprintf(stderr, "[srb200] gemm_f16: no %d-CTA cluster of this kernel fits the device\n", csize);
+    return -1;
+  }
+  cached.store(n, std::memory_order_relaxed);
+  return n;
+}
+
+template <int EPI, int CN = 1>
 int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
            const CUtensorMap& tx, const CUtensorMap& ta2, const CUtensorMap& tb2, const KArgs& ka, int num_sms,
            int grid_override = 0) {
   using Cfg = GemmCfg<EPI>;
   // per-device attribute; cheap enough to set on every launch (multi-GPU processes switch devices)
-  SRB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  const int m_blocks = (ka.M + BM - 1) / BM, n_blocks = (ka.N + BN - 1) / BN;
-  const int tiles = m_blocks * n_blocks;
-  const int grid = grid_override > 0 ? grid_override : (tiles < num_sms ? tiles : num_sms);
+  SRB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<EPI, CN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+  constexpr int csize = CN;
+  const int tiles = ((ka.M + BM - 1) / BM) * ((ka.N + BN * csize - 1) / (BN * csize));   // cluster tiles
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(kGemmThreads);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int nattr = 0;
+  if (pdl_enabled()) {
+    attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[nattr++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  // persistent grid: one worker per co-resident cluster (one per SM without clusters)
+  int workers = num_sms;
+  if constexpr (csize > 1) {
+    attr[nattr].id = cudaLaunchAttributeClusterDimension;
+    attr[nattr].val.clusterDim.x = csize;
+    attr[nattr].val.clusterDim.y = 1;
+    attr[nattr++].val.clusterDim.z = 1;
+    workers = max_clusters<EPI, CN>(num_sms);
+    if (workers <= 0) return -1;
+  }
+  const int grid = grid_override > 0 ? grid_override : csize * (tiles < workers ? tiles : workers);
+  cfg.gridDim = dim3(grid);
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<EPI>, ta, tb, tc, tx, ta2, tb2, ka));
+  cfg.numAttrs = nattr;
+  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<EPI, CN>, ta, tb, tc, tx, ta2, tb2, ka));
   note_launch();
   return 0;
 }
@@ -821,6 +909,43 @@ int make_tmap_f16_kmajor(CUtensorMap* out, const void* ptr, uint64_t rows, uint6
   return make_tmap_2d(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, k, rows, k, BK, box_rows);
 }
 
+// Measured at T = 131072 (ModernBERT-base, tools/gemm_prof.py), ms per GEMM.  H100 80GB HBM3 at a 400 W power limit
+// (power-capped SM clock), clusters of 1 x 1 / 2 x 1 (two row blocks share W) / 1 x 2 (two column tiles share A) /
+// 2 x 2:  Wqkv (EPI_ROPE, N 2304, K 768) 1.46 / 1.52 / 1.31 / 1.29;  Wi (EPI_GEGLU, N 2304) 1.39 / 1.39 / 1.28 / 1.46;
+// Wo2 (EPI_RESID_HL, N 768, K 1152) 0.93 / 1.00 / 0.89 / 0.98;  Wo (EPI_RESID_HL, K 768) 0.59 / 0.63 / 0.64 / 0.67.
+// The same card at 700 W, 1 x 1 / 1 x 2:  Wqkv 1.08 / 0.96;  Wi 1.00 / 0.94;  Wo2 0.69 / 0.74.
+// Only sharing A helps, so the kernel implements 1 x cn clusters alone, and only the two large LayerNorm-fold
+// projections use them.  The residual GEMMs, whose time goes to the fp16-pair epilogue rather than the operand feed,
+// run without clusters; so do the epilogues not measured here (EPI_F16, EPI_GELU, EPI_RESID) and EPI_TOPK, whose
+// grouped schedule gives each worker its own query block.  A pair is only formed when the column tiles pair up
+// exactly: with an odd N / 128 every other cluster would carry a CTA that computes a tile wholly past N.
+int gemm_cluster_size(int epi, int N, int K) {
+  (void)K;
+  const bool share_a = epi == EPI_ROPE || epi == EPI_GEGLU;
+  return share_a && ((N + BN - 1) / BN) % 2 == 0 ? 2 : 1;
+}
+
+static int device_sms() {
+  static int num_sms = 0;  // all devices of one box are the same part
+  if (!num_sms) {
+    int dev = 0, n = 0;
+    SRB_CUDA_CHECK(cudaGetDevice(&dev));
+    SRB_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+    num_sms = n;
+  }
+  return num_sms;
+}
+
+int gemm_cluster_workers(int epi, int N, int K) {
+  const int cn = gemm_cluster_size(epi, N, K);
+  const int num_sms = device_sms();
+  if (num_sms <= 0 || cn == 1) return num_sms;
+  // gemm_cluster_size forms pairs for these two epilogues only
+  if (epi == EPI_ROPE) return max_clusters<EPI_ROPE, 2>(num_sms);
+  if (epi == EPI_GEGLU) return max_clusters<EPI_GEGLU, 2>(num_sms);
+  return -1;
+}
+
 int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   if (g.M <= 0) return 0;
   if (g.K % 8 != 0 || g.N % 64 != 0 || g.ldo % 8 != 0) {
@@ -840,15 +965,12 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
     fprintf(stderr, "[srb200] gemm_f16: EPI_GEGLU needs N %% 128 == 0\n");
     return -1;
   }
-  static int num_sms = 0;  // all devices of one box are the same part
-  if (!num_sms) {
-    int dev = 0, n = 0;
-    SRB_CUDA_CHECK(cudaGetDevice(&dev));
-    SRB_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
-    num_sms = n;
-  }
+  const int num_sms = device_sms();
+  if (num_sms <= 0) return -1;
+  const int cn = gemm_cluster_size(g.epi, g.N, g.K);
+  // operand boxes: each CTA of a cluster loads 1/cn of the A box (kernel: TMA producer)
   CUtensorMap ta, tb, tc;
-  if (make_tmap_f16_kmajor(&ta, g.A, static_cast<uint64_t>(g.a_rows > 0 ? g.a_rows : g.M), g.K, BM)) return -1;
+  if (make_tmap_f16_kmajor(&ta, g.A, static_cast<uint64_t>(g.a_rows > 0 ? g.a_rows : g.M), g.K, BM / cn)) return -1;
   const int w_groups = g.w_groups > 1 ? g.w_groups : 1;
   if (w_groups > 1 && (g.w_group_rows <= 0 || g.w_group_rows % BM != 0 || g.N % BN != 0 || g.epi == EPI_TOPK)) {
     fprintf(stderr, "[srb200] gemm_f16: grouped weights need w_group_rows %% %d == 0 and whole column tiles\n", BM);
@@ -893,7 +1015,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
       fprintf(stderr, "[srb200] gemm_f16: K extension needs A2, W2 and K2 %% 8 == 0\n");
       return -1;
     }
-    if (make_tmap_f16_kmajor(&ta2, g.A2, static_cast<uint64_t>(g.a_rows > 0 ? g.a_rows : g.M), g.K2, BM)) return -1;
+    if (make_tmap_f16_kmajor(&ta2, g.A2, static_cast<uint64_t>(g.a_rows > 0 ? g.a_rows : g.M), g.K2, BM / cn)) return -1;
     if (make_tmap_f16_kmajor(&tb2, g.W2, g.N, g.K2, BN)) return -1;
     ka.K2 = g.K2;
   }
@@ -930,10 +1052,14 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   }
   switch (g.epi) {
     case EPI_F16: return launch<EPI_F16>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
-    case EPI_ROPE: return launch<EPI_ROPE>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
+    case EPI_ROPE:
+      return cn == 2 ? launch<EPI_ROPE, 2>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms)
+                     : launch<EPI_ROPE>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
     case EPI_RESID: return launch<EPI_RESID>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
     case EPI_RESID_HL: return launch<EPI_RESID_HL>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
-    case EPI_GEGLU: return launch<EPI_GEGLU>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
+    case EPI_GEGLU:
+      return cn == 2 ? launch<EPI_GEGLU, 2>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms)
+                     : launch<EPI_GEGLU>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
     case EPI_GELU: return launch<EPI_GELU>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
     case EPI_TOPK: {
       if (!g.topk_idx || !g.topk_score || !g.topk_lists || g.N % 256 != 0) {

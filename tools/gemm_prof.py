@@ -1,60 +1,154 @@
-import sys, os
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import torch
-import semantic_router_b200 as pkg
-L = pkg.lib()
-M = int(os.environ.get("M", 131072))
-def run(N, K, epi, out_dtype, n_out=None, resid=False):
-    a = torch.randn(M, K, device="cuda").half()
-    w = (torch.randn(N, K, device="cuda") * 0.05).half()
-    n_out = n_out or N
-    out = torch.zeros(M, n_out, device="cuda", dtype=out_dtype)
-    pos = torch.arange(M, device="cuda", dtype=torch.int32) % 512
-    cos = torch.rand(1024, 32, device="cuda"); sin = torch.rand(1024, 32, device="cuda")
-    def call():
-        L.sr_test_gemm(a.data_ptr(), w.data_ptr(), out.data_ptr(), M, N, K, epi, n_out, None, out.data_ptr() if resid else None,
-                       pos.data_ptr(), cos.data_ptr(), sin.data_ptr(), 1536 if epi == 1 else 0)
-    for _ in range(3): call()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(10): call()
-    e1.record(); torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / 10
-    print(f"M={M} N={N} K={K} epi={epi}: {ms*1e3:.1f} us  {2*M*N*K/ms/1e9:.1f} TFLOP/s")
-run(2304, 768, 1, torch.float16)            # Wqkv + RoPE
-run(2304, 768, 3, torch.float16, 1152)      # Wi + GeGLU
-run(768, 768, 2, torch.float32, resid=True) # attn out + residual
-run(768, 1152, 2, torch.float32, resid=True)# mlp out + residual
-run(2304, 768, 0, torch.float16)            # plain fp16 store
+"""Times the four projection GEMMs of one ModernBERT-base layer in the configuration the encoder runs them in, at
+T = M tokens (default 131072 = the headline batch 256 x seq 512):
 
-# ---- LayerNorm fold variants (gemm.h): producer = residual GEMM + fp16 copy + row statistics; consumers scale by rstd
-def run_fold(N, K, epi, out_dtype, n_out=None, producer=False):
-    a = torch.randn(M, K, device="cuda").half()
-    w = (torch.randn(N, K, device="cuda") * 0.05).half()
-    n_out = n_out or N
-    out = torch.zeros(M, n_out, device="cuda", dtype=out_dtype)
-    pos = torch.arange(M, device="cuda", dtype=torch.int32) % 512
-    cos = torch.rand(1024, 32, device="cuda"); sin = torch.rand(1024, 32, device="cuda")
-    stats = torch.rand(6, M, 2, device="cuda") + 1.0
-    raw = torch.zeros(M, 768, device="cuda", dtype=torch.float16)
-    def call():
-        if producer:
-            L.sr_test_gemm_fold(a.data_ptr(), w.data_ptr(), out.data_ptr(), M, N, K, epi, n_out, None, out.data_ptr(), None, None, None, 0,
-                                stats.data_ptr(), raw.data_ptr(), None, 0.0, 0, None, None, None)
-        else:
-            L.sr_test_gemm_fold(a.data_ptr(), w.data_ptr(), out.data_ptr(), M, N, K, epi, n_out, None, None, pos.data_ptr(), cos.data_ptr(),
-                                sin.data_ptr(), 1536 if epi == 1 else 0, None, None, stats.data_ptr(), 1e-5, 768, None, None, None)
-    for _ in range(3): call()
+  Wqkv  EPI_ROPE,     LayerNorm-fold consumer (fold stats, RoPE on the q/k columns)   N = 2304, K = 768
+  Wo    EPI_RESID_HL, fp16-pair residual producer (row stats, pivots in and out)      N = 768,  K = 768
+  Wi    EPI_GEGLU,    LayerNorm-fold consumer                                         N = 2304, K = 768
+  Wo2   EPI_RESID_HL                                                                  N = 768,  K = 1152
+
+Per GEMM: CUDA-event time over many launches, TFLOP/s, the algorithmic HBM bytes over that time, the modelled
+L2 -> SM operand traffic over that time for the thread-block cluster the library launches (each of the cluster_n CTAs
+loads 1/cluster_n of the shared A box and multicasts it to the others; W boxes are loaded per CTA), the number of
+co-resident clusters (workers of the persistent grid), and torch.mm on the same fp16 M, N, K as a cuBLAS reference point (no epilogue: a
+reference, not a target).  The GPU name, power limit and maximum SM clock are read in the same run.
+
+  python tools/gemm_prof.py [--root TREE] [--iters N] [--json OUT]
+
+--root loads the library built in another checkout of this project (to compare two builds in one run).
+"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+
+ap = argparse.ArgumentParser()
+ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ap.add_argument("--m", type=int, default=131072)
+ap.add_argument("--iters", type=int, default=20)
+ap.add_argument("--json", default=None, help="also write the rows as JSON here")
+args = ap.parse_args()
+sys.path.insert(0, os.path.abspath(args.root))
+
+import torch  # noqa: E402
+
+import semantic_router_b200 as pkg  # noqa: E402
+
+if not torch.cuda.is_available():
+    raise SystemExit("gemm_prof.py: no CUDA device")
+H = pkg.hooks()
+EPI_ROPE, EPI_GEGLU, EPI_RESID_HL = 1, 3, 6
+M, Hd, I = args.m, 768, 1152
+dev = "cuda"
+
+
+def cluster_shape(epi, n, k):
+    """(cluster_n, workers) the library launches for this GEMM; a build without clusters has one worker per SM."""
+    f = getattr(H, "sr_test_gemm_cluster", None)
+    if f is None:
+        return 1, torch.cuda.get_device_properties(0).multi_processor_count
+    f.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    cn, w = C.c_int(0), C.c_int(0)
+    assert f(epi, n, k, C.byref(cn), C.byref(w)) == 0
+    return cn.value, w.value
+
+
+def gpu_info():
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader",
+                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30)
+        return r.stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        return f"nvidia-smi unavailable ({e})"
+
+
+def timed(fn, iters):
+    for _ in range(3):
+        fn()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    for _ in range(10): call()
-    e1.record(); torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / 10
-    print(f"fold {'producer' if producer else 'consumer'} M={M} N={N} K={K} epi={epi}: {ms*1e3:.1f} us  {2*M*N*K/ms/1e9:.1f} TFLOP/s")
-if os.environ.get("FOLD", "1") != "0":
-    run_fold(2304, 768, 1, torch.float16)
-    run_fold(2304, 768, 3, torch.float16, 1152)
-    run_fold(768, 768, 2, torch.float32, producer=True)
-    run_fold(768, 1152, 2, torch.float32, producer=True)
+    for _ in range(iters):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / iters
+
+
+g = torch.Generator(device=dev).manual_seed(0)
+x_h = torch.randn(M, Hd, device=dev, generator=g).half()          # LayerNorm-fold A operand (raw fp16 rows)
+x_i = torch.randn(M, I, device=dev, generator=g).half()           # GeGLU output, the Wo2 A operand
+fold_stats = torch.rand(Hd // 128, M, 2, device=dev, generator=g) + 1.0
+pos = (torch.arange(M, device=dev, dtype=torch.int32) % 512).contiguous()
+cos = torch.rand(1024, 32, device=dev, generator=g)
+sin = torch.rand(1024, 32, device=dev, generator=g)
+w_qkv = (torch.randn(3 * Hd, Hd, device=dev, generator=g) * 0.02).half()
+w_i = (torch.randn(2 * I, Hd, device=dev, generator=g) * 0.02).half()
+w_o = (torch.randn(Hd, Hd, device=dev, generator=g) * 0.02).half()
+w_o2 = (torch.randn(Hd, I, device=dev, generator=g) * 0.02).half()
+qkv = torch.empty(M, 3 * Hd, device=dev, dtype=torch.float16)
+mid = torch.empty(M, I, device=dev, dtype=torch.float16)
+hi = torch.randn(M, Hd, device=dev, generator=g).half()
+lo = torch.zeros(M, Hd, device=dev, dtype=torch.float16)
+parts = Hd // 128
+recs = [torch.zeros(parts * M * 2 + M, device=dev) for _ in range(2)]   # [row stats | pivots], alternating in / out
+flip = [0]
+
+
+def p(t):
+    return t.data_ptr()
+
+
+def call_fold(a, w, out, n, epi, n_out, rope_cols):
+    rc = H.sr_test_gemm_fold(p(a), p(w), p(out), M, n, Hd, epi, n_out, None, None, p(pos) if epi == EPI_ROPE else None,
+                             p(cos) if epi == EPI_ROPE else None, p(sin) if epi == EPI_ROPE else None, rope_cols,
+                             None, None, p(fold_stats), 1e-5, Hd, None, None, None)
+    assert rc == 0
+
+
+def call_resid_hl(a, w, k):
+    dst, prev = recs[flip[0]], recs[flip[0] ^ 1]
+    flip[0] ^= 1
+    rc = H.sr_test_gemm_resid_hl(p(a), p(w), p(hi), p(lo), M, Hd, k, None, p(dst), dst[parts * M * 2:].data_ptr(),
+                                 prev[parts * M * 2:].data_ptr(), p(prev))
+    assert rc == 0
+
+
+# (name, epilogue, N, K, launch, HBM bytes: A + outputs (+ residual pair read) + row statistics)
+gemms = [
+    ("Wqkv", "EPI_ROPE fold", EPI_ROPE, 3 * Hd, Hd, lambda: call_fold(x_h, w_qkv, qkv, 3 * Hd, EPI_ROPE, 3 * Hd, 2 * Hd),
+     M * Hd * 2 + M * 3 * Hd * 2 + parts * M * 8 + 3 * Hd * Hd * 2),
+    ("Wo", "EPI_RESID_HL", EPI_RESID_HL, Hd, Hd, lambda: call_resid_hl(x_h, w_o, Hd),
+     M * Hd * 2 + 4 * M * Hd * 2 + 2 * parts * M * 8 + Hd * Hd * 2),
+    ("Wi", "EPI_GEGLU fold", EPI_GEGLU, 2 * I, Hd, lambda: call_fold(x_h, w_i, mid, 2 * I, EPI_GEGLU, I, 0),
+     M * Hd * 2 + M * I * 2 + parts * M * 8 + 2 * I * Hd * 2),
+    ("Wo2", "EPI_RESID_HL", EPI_RESID_HL, Hd, I, lambda: call_resid_hl(x_i, w_o2, I),
+     M * I * 2 + 4 * M * Hd * 2 + 2 * parts * M * 8 + Hd * I * 2),
+]
+BM = BN = 128
+info = gpu_info()
+print(f"# {info}   M={M}   root={os.path.abspath(args.root)}")
+print(f"# {'gemm':5s} {'epilogue':15s} {'N':>5s} {'K':>5s} {'cluster':>7s} {'workers':>7s} {'ms':>7s} {'TFLOP/s':>8s} {'HBM GB/s':>9s} "
+      f"{'L2->SM GB/s':>11s} {'mm ms':>7s} {'mm TFLOP/s':>10s}")
+rows = []
+for name, epi_name, epi, n, k, fn, hbm in gemms:
+    ms = timed(fn, args.iters)
+    cn, workers = cluster_shape(epi, n, k)
+    tiles = ((M + BM - 1) // BM) * ((n + BN - 1) // BN)
+    l2_bytes = tiles * k * 2 * (BM / cn + BN)
+    a = x_i if k == I else x_h
+    w = {"Wqkv": w_qkv, "Wo": w_o, "Wi": w_i, "Wo2": w_o2}[name]
+    ms_mm = timed(lambda: torch.mm(a, w.t()), args.iters)
+    flops = 2.0 * M * n * k
+    row = {"gemm": name, "epilogue": epi_name, "M": M, "N": n, "K": k, "cluster": f"1x{cn}", "clusters": workers, "ms": ms,
+           "tflops": flops / ms / 1e9, "hbm_gbs": hbm / ms / 1e6, "l2_sm_gbs": l2_bytes / ms / 1e6, "mm_ms": ms_mm,
+           "mm_tflops": flops / ms_mm / 1e9}
+    rows.append(row)
+    print(f"  {name:5s} {epi_name:15s} {n:5d} {k:5d} {row['cluster']:>7s} {workers:7d} {ms:7.3f} {row['tflops']:8.1f} "
+          f"{row['hbm_gbs']:9.0f} {row['l2_sm_gbs']:11.0f} {ms_mm:7.3f} {row['mm_tflops']:10.1f}")
+tot = sum(r["ms"] for r in rows)
+print(f"# four GEMMs: {tot:.3f} ms per layer, {22 * tot:.1f} ms per 22-layer step")
+if args.json:
+    os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
+    json.dump({"gpu": info, "rows": rows, "layer_ms": tot}, open(args.json, "w"), indent=1)
