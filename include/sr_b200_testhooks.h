@@ -43,6 +43,44 @@ SR_API int sr_test_gemm_resid_hl(const void* a_f16, const void* w_f16, void* hi_
 /* The thread-block cluster the GEMM launches for (epilogue, N, K): cluster_n CTAs on neighbouring column tiles of one row
  * block share each A k-block (1: no clusters); workers = clusters of its persistent grid on this device. */
 SR_API int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers);
+/* Every field of the GEMM descriptor (csrc/gemm.h GemmDesc, same names and meaning; epi = GemmEpilogue value).  Zeroed
+ * fields take GemmDesc's defaults. */
+typedef struct sr_gemm_desc {
+  int m, n, k;
+  const void* a;
+  int a_rows;
+  const void* w;
+  void* out;
+  int ldo;
+  int epi;
+  const float* bias;
+  const float* resid;
+  int ldr;
+  const int32_t* pos;
+  const float* rope_cos;
+  const float* rope_sin;
+  int rope_cols;
+  int32_t* topk_idx;
+  float* topk_score;
+  const uint8_t* topk_valid;
+  int topk_n;
+  float* row_stats;
+  void* raw16;
+  void* lo16;
+  float* pivot_out;
+  const float* pivot_in;
+  const float* pivot_in_stats;
+  const float* fold_stats;
+  float fold_eps;
+  int fold_h;
+  const void* a2;
+  const void* w2;
+  int k2;
+  int w_groups, w_group_rows;
+  int mask_block, mask_rows;
+} sr_gemm_desc;
+/* gemm_f16 on the legacy default stream with every descriptor field; EPI_TOPK's list count goes to *topk_lists. */
+SR_API int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists);
 SR_API int sr_test_hl_to_f32(const void* hi_f16, const void* lo_f16, const float* pivot, int t, int hdim, float* x);
 SR_API int sr_test_attention(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int max_len,
                       int num_heads, int window);

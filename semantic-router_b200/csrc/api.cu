@@ -576,6 +576,23 @@ int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers) {
   *workers = gemm_cluster_workers(epi, n, k);
   return *workers > 0 ? 0 : -1;
 }
+int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
+  if (!d) return -1;
+  GemmDesc g;
+  g.M = d->m; g.N = d->n; g.K = d->k; g.A = d->a; g.a_rows = d->a_rows; g.W = d->w; g.out = d->out; g.ldo = d->ldo;
+  g.epi = static_cast<GemmEpilogue>(d->epi);
+  g.bias = d->bias; g.resid = d->resid; g.ldr = d->ldr;
+  g.pos = d->pos; g.rope_cos = d->rope_cos; g.rope_sin = d->rope_sin; g.rope_cols = d->rope_cols;
+  g.topk_idx = d->topk_idx; g.topk_score = d->topk_score; g.topk_valid = d->topk_valid; g.topk_n = d->topk_n;
+  g.topk_lists = topk_lists;
+  g.row_stats = d->row_stats; g.raw16 = d->raw16; g.lo16 = d->lo16;
+  g.pivot_out = d->pivot_out; g.pivot_in = d->pivot_in; g.pivot_in_stats = d->pivot_in_stats;
+  g.fold_stats = d->fold_stats; g.fold_eps = d->fold_eps; g.fold_h = d->fold_h;
+  g.A2 = d->a2; g.W2 = d->w2; g.K2 = d->k2;
+  g.w_groups = d->w_groups; g.w_group_rows = d->w_group_rows;
+  g.mask_block = d->mask_block; g.mask_rows = d->mask_rows;
+  return gemm_f16(nullptr, g);
+}
 int sr_test_hl_to_f32(const void* hi, const void* lo, const float* pivot, int t, int hdim, float* x) {
   return hl_to_f32(nullptr, static_cast<const __half*>(hi), static_cast<const __half*>(lo), pivot, t, hdim, x);
 }

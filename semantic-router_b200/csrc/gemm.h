@@ -77,7 +77,8 @@ struct GemmDesc {
   const void* W2 = nullptr;            // fp16 [N, K2]
   int K2 = 0;                          // multiple of 8 (TMA zero-fills the last k-block)
   // ---- grouped weights: W = w_groups matrices [N, K] stacked along N; rows [g * w_group_rows, (g + 1) * w_group_rows) of A are
-  // multiplied with matrix g (w_group_rows a multiple of 256: a row block never straddles two groups).  One launch serves
+  // multiplied with matrix g (w_group_rows a multiple of 128, the row-block height: a row block never straddles two
+  // groups; gemm_f16 refuses anything else).  One launch serves
   // several tasks' merged weights (engine.h: LoraShared, grouped form).
   int w_groups = 0, w_group_rows = 0;
   // ---- EPI_F16 column-block mask (produces A2): out[r, c] = 0 unless c / mask_block == r / mask_rows

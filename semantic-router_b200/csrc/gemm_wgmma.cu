@@ -535,9 +535,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             int cidx = ocol0 + ci;
             const bool ok = cidx < p.topk_n && (!p.topk_valid || __ldg(p.topk_valid + (cidx < p.topk_n ? cidx : 0)));
             if (ok) {
+              // insertion into the descending list: strict > finds the slot (after any equal score, which has the lower
+              // column), and from there every entry shifts down one, ties included, so the tail is the one dropped
+              bool shift = false;
 #pragma unroll
-              for (int j = 0; j < kTopK; ++j) {   // insertion into the descending list
-                if (cv > tk_v[j]) {
+              for (int j = 0; j < kTopK; ++j) {
+                if (shift || cv > tk_v[j]) {
+                  shift = true;
                   const float tv = tk_v[j]; const int ti = tk_i[j];
                   tk_v[j] = cv; tk_i[j] = cidx;
                   cv = tv; cidx = ti;
