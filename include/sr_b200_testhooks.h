@@ -4,6 +4,7 @@
  */
 #ifndef SR_B200_TESTHOOKS_H
 #define SR_B200_TESTHOOKS_H
+#include <stddef.h>
 #include "sr_b200.h"
 #ifdef __cplusplus
 extern "C" {
@@ -91,6 +92,39 @@ SR_API int sr_test_attention_win(const void* qkv_f16, void* out_f16, const int32
                                  int max_len, int num_heads, int window);
 SR_API int sr_test_layernorm(const float* x, int t, int h, const float* w, const float* b, float eps, float* y32,
                       void* y16);
+
+/* ---- the row kernels of csrc/elementwise.cu, one hook per launcher (csrc/kernels.h: same arguments and meaning) -- */
+SR_API int sr_test_embed_ln_modernbert(const int32_t* ids, int t, int h, int vocab, const float* table, const float* ln_w,
+                                       float eps, float* x, void* h16, void* lo16);
+SR_API int sr_test_embed_ln_bert(const int32_t* ids, const int32_t* pos, int t, int h, int vocab, int max_pos,
+                                 const float* word, const float* pos_emb, const float* type0, const float* ln_w,
+                                 const float* ln_b, float eps, float* x, void* h16);
+SR_API int sr_test_positions(const int32_t* cu_seqlens, int batch, int32_t* pos);
+SR_API int sr_test_cast_f16(const float* x, size_t n, void* y16);
+/* mode: 0 mean, 1 first token; part [batch, 8, h] and arrived [batch] (zero on entry) are the caller's scratch */
+SR_API int sr_test_pool_rows(const float* x, const int32_t* cu_seqlens, int batch, int h, int mode, const float* ln_w,
+                             const float* ln_b, float eps, float* pooled, float* part, int32_t* arrived,
+                             const int32_t* div_lens);
+SR_API int sr_test_l2_normalize(const float* pooled, int batch, int h, int dim, float norm_eps, float* emb);
+/* Every field of the sequence-head weights (csrc/kernels.h SeqHeadWeights, same names and meaning). */
+typedef struct sr_seq_head_weights {
+  const float* dense_w;
+  const float* dense_b;
+  const float* norm_w;
+  int dense_mode;
+  const float* cls_w;
+  const float* cls_b;
+  int num_classes;
+  int argmax_last;
+  int gelu_erf;
+  float head_eps;
+} sr_seq_head_weights;
+SR_API int sr_test_seq_head(const float* pooled, int batch, int h, const sr_seq_head_weights* w, float* logits,
+                            float* probs, int32_t* cls, float* conf);
+SR_API int sr_test_token_head(const float* hidden32, const void* dense16, int t, int h, const float* norm_w,
+                              const float* pre_ln_w, float pre_ln_eps, const float* cls_w, const float* cls_b, int c,
+                              int argmax_last, float* logits, float* probs, int32_t* pred, float* conf, int gelu_erf,
+                              float head_eps);
 
 #ifdef __cplusplus
 }

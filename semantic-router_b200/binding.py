@@ -90,6 +90,13 @@ def load_library(path: Optional[str] = None):
     return L
 
 
+class SeqHeadWeights(C.Structure):
+    """sr_seq_head_weights (include/sr_b200_testhooks.h): every field of csrc/kernels.h SeqHeadWeights."""
+    _fields_ = [("dense_w", C.c_void_p), ("dense_b", C.c_void_p), ("norm_w", C.c_void_p), ("dense_mode", C.c_int),
+                ("cls_w", C.c_void_p), ("cls_b", C.c_void_p), ("num_classes", C.c_int), ("argmax_last", C.c_int),
+                ("gelu_erf", C.c_int), ("head_eps", C.c_float)]
+
+
 _hooks = None
 
 
@@ -110,6 +117,15 @@ def hooks():
                                         vp, vp, vp, C.c_float, C.c_int, vp, vp, vp]
         H.sr_test_gemm_resid_hl.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]
         H.sr_test_hl_to_f32.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
+        ci, cf = C.c_int, C.c_float
+        H.sr_test_embed_ln_modernbert.argtypes = [vp, ci, ci, ci, vp, vp, cf, vp, vp, vp]
+        H.sr_test_embed_ln_bert.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, cf, vp, vp]
+        H.sr_test_positions.argtypes = [vp, ci, vp]
+        H.sr_test_cast_f16.argtypes = [vp, C.c_size_t, vp]
+        H.sr_test_pool_rows.argtypes = [vp, vp, ci, ci, ci, vp, vp, cf, vp, vp, vp, vp]
+        H.sr_test_l2_normalize.argtypes = [vp, ci, ci, ci, cf, vp]
+        H.sr_test_seq_head.argtypes = [vp, ci, ci, C.POINTER(SeqHeadWeights), vp, vp, vp, vp]
+        H.sr_test_token_head.argtypes = [vp, vp, ci, ci, vp, vp, cf, vp, vp, ci, ci, vp, vp, vp, vp, ci, cf]
         _hooks = H
     return _hooks
 

@@ -616,6 +616,42 @@ int sr_test_attention_win(const void* qkv, void* out, const int32_t* cu, int bat
 int sr_test_layernorm(const float* x, int t, int hdim, const float* w, const float* b, float eps, float* y32, void* y16) {
   return layernorm_rows(nullptr, x, t, hdim, w, b, eps, y32, static_cast<__half*>(y16));
 }
+int sr_test_embed_ln_modernbert(const int32_t* ids, int t, int hdim, int vocab, const float* table, const float* ln_w, float eps,
+                                float* x, void* h16, void* lo16) {
+  return embed_ln_modernbert(nullptr, ids, t, hdim, vocab, table, ln_w, eps, x, static_cast<__half*>(h16),
+                             static_cast<__half*>(lo16));
+}
+int sr_test_embed_ln_bert(const int32_t* ids, const int32_t* pos, int t, int hdim, int vocab, int max_pos, const float* word,
+                          const float* pos_emb, const float* type0, const float* ln_w, const float* ln_b, float eps, float* x,
+                          void* h16) {
+  return embed_ln_bert(nullptr, ids, pos, t, hdim, vocab, max_pos, word, pos_emb, type0, ln_w, ln_b, eps, x,
+                       static_cast<__half*>(h16));
+}
+int sr_test_positions(const int32_t* cu, int batch, int32_t* pos) { return compute_positions(nullptr, cu, batch, pos); }
+int sr_test_cast_f16(const float* x, size_t n, void* y16) { return cast_rows_f16(nullptr, x, n, static_cast<__half*>(y16)); }
+int sr_test_pool_rows(const float* x, const int32_t* cu, int batch, int hdim, int mode, const float* ln_w, const float* ln_b,
+                      float eps, float* pooled, float* part, int32_t* arrived, const int32_t* div_lens) {
+  if (mode != POOL_MEAN && mode != POOL_CLS) return -1;
+  return pool_rows(nullptr, x, cu, batch, hdim, static_cast<PoolMode>(mode), ln_w, ln_b, eps, pooled, part, arrived, div_lens);
+}
+int sr_test_l2_normalize(const float* pooled, int batch, int hdim, int dim, float norm_eps, float* emb) {
+  return l2_normalize_rows(nullptr, pooled, batch, hdim, dim, norm_eps, emb);
+}
+int sr_test_seq_head(const float* pooled, int batch, int hdim, const sr_seq_head_weights* w, float* logits, float* probs,
+                     int32_t* cls, float* conf) {
+  if (!w) return -1;
+  SeqHeadWeights s;
+  s.dense_w = w->dense_w; s.dense_b = w->dense_b; s.norm_w = w->norm_w; s.dense_mode = w->dense_mode;
+  s.cls_w = w->cls_w; s.cls_b = w->cls_b; s.num_classes = w->num_classes; s.argmax_last = w->argmax_last;
+  s.gelu_erf = w->gelu_erf; s.head_eps = w->head_eps;
+  return seq_head(nullptr, pooled, batch, hdim, s, logits, probs, cls, conf);
+}
+int sr_test_token_head(const float* hidden32, const void* dense16, int t, int hdim, const float* norm_w, const float* pre_ln_w,
+                       float pre_ln_eps, const float* cls_w, const float* cls_b, int c, int argmax_last, float* logits,
+                       float* probs, int32_t* pred, float* conf, int gelu_erf, float head_eps) {
+  return token_head(nullptr, hidden32, static_cast<const __half*>(dense16), t, hdim, norm_w, pre_ln_w, pre_ln_eps, cls_w,
+                    cls_b, c, argmax_last, logits, probs, pred, conf, gelu_erf, head_eps);
+}
 
 #endif  // SRB_TEST_HOOKS
 

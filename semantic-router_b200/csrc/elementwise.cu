@@ -150,11 +150,16 @@ layernorm_kernel(const float* x, int T, const float* __restrict__ w, const float
   if (y16) row_store16<NV>(y16 + static_cast<size_t>(row) * (NV * 128), v);
 }
 
-__global__ void cast_f16_kernel(const float* __restrict__ x, size_t n4, __half* __restrict__ y) {
+// thread i < n / 4 converts float4 #i; thread n / 4 converts the last n % 4 elements one by one
+__global__ void cast_f16_kernel(const float* __restrict__ x, size_t n, __half* __restrict__ y) {
   const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n4) return;
-  const float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
-  reinterpret_cast<uint2*>(y)[i] = make_uint2(pack_half2(v.x, v.y), pack_half2(v.z, v.w));
+  const size_t n4 = n / 4;
+  if (i < n4) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
+    reinterpret_cast<uint2*>(y)[i] = make_uint2(pack_half2(v.x, v.y), pack_half2(v.z, v.w));
+  } else if (i == n4) {
+    for (size_t j = 4 * n4; j < n; ++j) y[j] = __float2half_rn(__ldg(x + j));
+  }
 }
 
 __global__ void positions_kernel(const int* __restrict__ cu, int* __restrict__ pos) {
@@ -496,8 +501,8 @@ int layernorm_rows(cudaStream_t stream, const float* x, int T, int H, const floa
 
 int cast_rows_f16(cudaStream_t stream, const float* x, size_t n, __half* y) {
   if (n == 0) return 0;
-  const size_t n4 = n / 4;
-  cast_f16_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, stream>>>(x, n4, y);
+  const size_t threads = n / 4 + (n % 4 != 0);
+  cast_f16_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, stream>>>(x, n, y);
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   return 0;

@@ -40,7 +40,7 @@ int embed_ln_bert(cudaStream_t stream, const int* ids, const int* pos, int T, in
 // Row LayerNorm of fp32 x[T,H]; optional outputs: y32 (may alias x) and y16.
 int layernorm_rows(cudaStream_t stream, const float* x, int T, int H, const float* w, const float* b, float eps,
                    float* y32, __half* y16);
-// fp32 -> fp16 row copy
+// fp32 -> fp16 copy of n elements, any n (x 16-byte and y 8-byte aligned)
 int cast_rows_f16(cudaStream_t stream, const float* x, size_t n, __half* y);
 
 enum PoolMode { POOL_MEAN = 0, POOL_CLS = 1 };

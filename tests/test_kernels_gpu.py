@@ -150,23 +150,6 @@ def test_attention(srlib, cuda, lens, window, impl):
     torch.testing.assert_close(out.float(), ref, rtol=2e-3, atol=2e-3)
 
 
-@pytest.mark.parametrize("H", [384, 768, 1024])
-def test_layernorm(srlib, cuda, H):
-    T = 1037
-    g = torch.Generator(device="cuda").manual_seed(H)
-    x = torch.randn(T, H, device=cuda, generator=g) * 3 + 0.5
-    w = torch.randn(H, device=cuda, generator=g)
-    b = torch.randn(H, device=cuda, generator=g)
-    y32 = torch.zeros_like(x)
-    y16 = torch.zeros(T, H, device=cuda, dtype=torch.float16)
-    rc = srlib.lib().sr_test_layernorm(x.data_ptr(), T, H, w.data_ptr(), b.data_ptr(), 1e-5, y32.data_ptr(), y16.data_ptr())
-    torch.cuda.synchronize()
-    assert rc == 0
-    ref = torch.nn.functional.layer_norm(x, (H,), w, b, 1e-5)
-    torch.testing.assert_close(y32, ref, rtol=1e-5, atol=1e-5)
-    torch.testing.assert_close(y16.float(), ref, rtol=1e-3, atol=1e-3)
-
-
 @pytest.mark.parametrize("M", [300, 2500])
 def test_gemm_layernorm_fold(srlib, cuda, M):
     """LayerNorm folded into the GEMMs around it: the residual GEMM emits fp16(x) and per-row (sum, sum of squares);
