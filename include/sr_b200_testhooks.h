@@ -27,14 +27,6 @@ SR_API int sr_test_hallucination_spans(const int32_t* pred, const float* conf, c
 SR_API int sr_test_gemm(const void* a_f16, const void* w_f16, void* out, int m, int n, int k, int epi, int ldo,
                  const float* bias, const float* resid, const int32_t* pos, const float* rope_cos,
                  const float* rope_sin, int rope_cols);
-/* sr_test_gemm plus the LayerNorm-fold operands (gemm.h): EPI_RESID may emit per-row (sum, sum of squares) partials
- * row_stats [n/128][m][2] and raw16 = fp16(out); EPI_ROPE / EPI_GEGLU (weights: W diag(gamma) with zero-sum rows) scale
- * the accumulator rows by the rstd computed from fold_stats over rows of length fold_h.  pivot_*: row pivots (gemm.h). */
-SR_API int sr_test_gemm_fold(const void* a_f16, const void* w_f16, void* out, int m, int n, int k, int epi, int ldo,
-                             const float* bias, const float* resid, const int32_t* pos, const float* rope_cos,
-                             const float* rope_sin, int rope_cols, float* row_stats, void* raw16_f16,
-                             const float* fold_stats, float fold_eps, int fold_h, float* pivot_out, const float* pivot_in,
-                             const float* pivot_in_stats);
 /* EPI_RESID_HL (gemm.h): the residual stream as an fp16 pair, in place.  (hi + lo) holds x - pivot_in; after the call it holds
  * x + a w^T (+bias) - pivot_out with pivot_out = pivot_in + (row mean of the old pair, from pivot_in_stats; 0 without), and
  * row_stats [n/128][m][2] the (sum, sum of squares) partials of the new pair. */
@@ -45,7 +37,9 @@ SR_API int sr_test_gemm_resid_hl(const void* a_f16, const void* w_f16, void* hi_
  * block share each A k-block (1: no clusters); workers = clusters of its persistent grid on this device. */
 SR_API int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers);
 /* Every field of the GEMM descriptor (csrc/gemm.h GemmDesc, same names and meaning; epi = GemmEpilogue value).  Zeroed
- * fields take GemmDesc's defaults. */
+ * fields take GemmDesc's defaults.  EPI_ROPE / EPI_GEGLU with fold_stats (weights: W diag(gamma) with zero-sum rows)
+ * scale the accumulator rows by the rstd computed from fold_stats over rows of length fold_h; the EPI_RESID_HL fields
+ * mean what they mean for sr_test_gemm_resid_hl (out = hi). */
 typedef struct sr_gemm_desc {
   int m, n, k;
   const void* a;
@@ -66,7 +60,7 @@ typedef struct sr_gemm_desc {
   const uint8_t* topk_valid;
   int topk_n;
   float* row_stats;
-  void* raw16;
+  void* reserved;   /* must be null: keeps the offsets of the fields below fixed for existing callers */
   void* lo16;
   float* pivot_out;
   const float* pivot_in;

@@ -97,6 +97,29 @@ class SeqHeadWeights(C.Structure):
                 ("gelu_erf", C.c_int), ("head_eps", C.c_float)]
 
 
+class GemmDesc(C.Structure):
+    """sr_gemm_desc (include/sr_b200_testhooks.h): every field of csrc/gemm.h GemmDesc."""
+    _fields_ = [(n, C.c_int) for n in ("m", "n", "k")] + [
+        ("a", C.c_void_p), ("a_rows", C.c_int), ("w", C.c_void_p), ("out", C.c_void_p), ("ldo", C.c_int),
+        ("epi", C.c_int), ("bias", C.c_void_p), ("resid", C.c_void_p), ("ldr", C.c_int), ("pos", C.c_void_p),
+        ("rope_cos", C.c_void_p), ("rope_sin", C.c_void_p), ("rope_cols", C.c_int), ("topk_idx", C.c_void_p),
+        ("topk_score", C.c_void_p), ("topk_valid", C.c_void_p), ("topk_n", C.c_int), ("row_stats", C.c_void_p),
+        ("reserved", C.c_void_p), ("lo16", C.c_void_p), ("pivot_out", C.c_void_p), ("pivot_in", C.c_void_p),
+        ("pivot_in_stats", C.c_void_p), ("fold_stats", C.c_void_p), ("fold_eps", C.c_float), ("fold_h", C.c_int), ("a2", C.c_void_p),
+        ("w2", C.c_void_p), ("k2", C.c_int)] + [(n, C.c_int) for n in ("w_groups", "w_group_rows", "mask_block", "mask_rows")]
+
+
+def run_gemm(**fields):
+    """sr_test_gemm_desc on the legacy default stream: GemmDesc fields by name, device buffers as addresses or as
+    objects with a data_ptr() method.  Returns (status, EPI_TOPK list count); does not synchronise."""
+    d = GemmDesc()
+    for k, v in fields.items():
+        setattr(d, k, v.data_ptr() if hasattr(v, "data_ptr") else v)
+    lists = C.c_int(0)
+    rc = hooks().sr_test_gemm_desc(C.byref(d), C.byref(lists))
+    return rc, lists.value
+
+
 _hooks = None
 
 
@@ -109,13 +132,13 @@ def hooks():
         H = C.CDLL(HOOKS_LIB_PATH)
         vp = C.c_void_p
         H.sr_test_gemm.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, C.c_int]
+        H.sr_test_gemm_resid_hl.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]
+        H.sr_test_gemm_desc.argtypes = [C.POINTER(GemmDesc), C.POINTER(C.c_int)]
+        H.sr_test_gemm_cluster.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp]
         H.sr_test_attention.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
         H.sr_test_attention_tc.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
         H.sr_test_attention_win.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
         H.sr_test_layernorm.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_float, vp, vp]
-        H.sr_test_gemm_fold.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, C.c_int,
-                                        vp, vp, vp, C.c_float, C.c_int, vp, vp, vp]
-        H.sr_test_gemm_resid_hl.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]
         H.sr_test_hl_to_f32.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
         ci, cf = C.c_int, C.c_float
         H.sr_test_embed_ln_modernbert.argtypes = [vp, ci, ci, ci, vp, vp, cf, vp, vp, vp]
@@ -136,7 +159,7 @@ def _attach_hooks(L):
     if not os.path.exists(HOOKS_LIB_PATH):
         return
     H = hooks()
-    for name in ("sr_test_gemm", "sr_test_gemm_fold", "sr_test_attention", "sr_test_attention_tc", "sr_test_attention_win",
+    for name in ("sr_test_gemm", "sr_test_attention", "sr_test_attention_tc", "sr_test_attention_win",
                  "sr_test_layernorm", "sr_test_bio_decode", "sr_test_hallucination_spans"):
         setattr(L, name, getattr(H, name))
 

@@ -547,20 +547,6 @@ int sr_test_gemm(const void* a, const void* w, void* out, int m, int n, int k, i
   g.rope_cols = rope_cols;
   return gemm_f16(nullptr, g);
 }
-int sr_test_gemm_fold(const void* a, const void* w, void* out, int m, int n, int k, int epi, int ldo, const float* bias,
-                      const float* resid, const int32_t* pos, const float* rope_cos, const float* rope_sin, int rope_cols,
-                      float* row_stats, void* raw16, const float* fold_stats, float fold_eps, int fold_h, float* pivot_out,
-                      const float* pivot_in, const float* pivot_in_stats) {
-  GemmDesc g;
-  g.M = m; g.N = n; g.K = k; g.A = a; g.W = w; g.out = out; g.ldo = ldo;
-  g.epi = static_cast<GemmEpilogue>(epi);
-  g.bias = bias; g.resid = resid; g.ldr = ldo; g.pos = pos; g.rope_cos = rope_cos; g.rope_sin = rope_sin;
-  g.rope_cols = rope_cols;
-  g.row_stats = row_stats; g.raw16 = raw16;
-  g.fold_stats = fold_stats; g.fold_eps = fold_eps; g.fold_h = fold_h;
-  g.pivot_out = pivot_out; g.pivot_in = pivot_in; g.pivot_in_stats = pivot_in_stats;
-  return gemm_f16(nullptr, g);
-}
 int sr_test_gemm_resid_hl(const void* a, const void* w, void* hi, void* lo, int m, int n, int k, const float* bias, float* row_stats,
                           float* pivot_out, const float* pivot_in, const float* pivot_in_stats) {
   GemmDesc g;
@@ -577,7 +563,7 @@ int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers) {
   return *workers > 0 ? 0 : -1;
 }
 int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
-  if (!d) return -1;
+  if (!d || d->reserved) return -1;
   GemmDesc g;
   g.M = d->m; g.N = d->n; g.K = d->k; g.A = d->a; g.a_rows = d->a_rows; g.W = d->w; g.out = d->out; g.ldo = d->ldo;
   g.epi = static_cast<GemmEpilogue>(d->epi);
@@ -585,7 +571,7 @@ int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
   g.pos = d->pos; g.rope_cos = d->rope_cos; g.rope_sin = d->rope_sin; g.rope_cols = d->rope_cols;
   g.topk_idx = d->topk_idx; g.topk_score = d->topk_score; g.topk_valid = d->topk_valid; g.topk_n = d->topk_n;
   g.topk_lists = topk_lists;
-  g.row_stats = d->row_stats; g.raw16 = d->raw16; g.lo16 = d->lo16;
+  g.row_stats = d->row_stats; g.lo16 = d->lo16;
   g.pivot_out = d->pivot_out; g.pivot_in = d->pivot_in; g.pivot_in_stats = d->pivot_in_stats;
   g.fold_stats = d->fold_stats; g.fold_eps = d->fold_eps; g.fold_h = d->fold_h;
   g.A2 = d->a2; g.W2 = d->w2; g.K2 = d->k2;

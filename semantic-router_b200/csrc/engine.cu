@@ -366,15 +366,6 @@ bool load_head(Loader& ld, const Json& cfgj, Arch arch, int H, const std::string
 // ------------------------------------------------------------------------------------------------
 // model load
 // ------------------------------------------------------------------------------------------------
-// SRB_LN_FOLD=0 keeps the separate LayerNorm kernels (exact LayerNorm input rounding; A/B measurements)
-bool ln_fold_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("SRB_LN_FOLD");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-
 // W'' = W diag(gamma), every row re-centred to sum zero, rounded to fp16.  Two refinement passes push the sum of the
 // ROUNDED row (what the tensor core multiplies) from ~1e-4 down to the last bit of its largest elements, so the
 // residual mean * sum(W''[n,:]) is far below the fp16 rounding of the output.
@@ -479,13 +470,17 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
       LayerWeights& lw = m->layers[li];
       if (st.find(Lp + "attn_norm.weight")) lw.attn_norm_w = ld.f32(Lp + "attn_norm.weight", {H});
       std::vector<float> wq, g_attn, g_mlp;
-      if (ld.host_f32(Lp + "attn.Wqkv.weight", wq, {3 * H, H})) lw.wqkv = ld.up_f16(wq);
+      // Wqkv runs LayerNorm-folded where its attn_norm follows a residual GEMM; layer 0 and layers without attn_norm
+      // multiply the plain weight (encoder_forward)
+      if (ld.host_f32(Lp + "attn.Wqkv.weight", wq, {3 * H, H})) {
+        if (li > 0 && lw.attn_norm_w && ld.host_f32(Lp + "attn_norm.weight", g_attn, {H}))
+          fold_weights(ld, wq, g_attn, 3 * H, H, &lw.wqkv_f);
+        else
+          lw.wqkv = ld.up_f16(wq);
+      }
       lw.wo = ld.f16(Lp + "attn.Wo.weight", {H, H});
       lw.mid_norm_w = ld.f32(Lp + "mlp_norm.weight", {H});
-      const bool fold = ln_fold_enabled() && H % 128 == 0;
-      if (fold && lw.attn_norm_w && ld.host_f32(Lp + "attn_norm.weight", g_attn, {H}))
-        fold_weights(ld, wq, g_attn, 3 * H, H, &lw.wqkv_f);
-      if (fold) ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
+      ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
       std::vector<float> wi, wi_perm;
       if (ld.host_f32(Lp + "mlp.Wi.weight", wi, {2 * I, H})) {
         // GeGLU interleave for the fused epilogue: 32-row groups [a(32j..) | b(32j..)] (gemm.h EPI_GEGLU)
@@ -495,8 +490,7 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
           memcpy(&wi_perm[static_cast<size_t>(64 * j + 32) * H], &wi[static_cast<size_t>(I + 32 * j) * H],
                  sizeof(float) * 32 * H);
         }
-        lw.wi = ld.up_f16(wi_perm);
-        if (fold && !g_mlp.empty()) fold_weights(ld, wi_perm, g_mlp, 2 * I, H, &lw.wi_f);
+        if (!g_mlp.empty()) fold_weights(ld, wi_perm, g_mlp, 2 * I, H, &lw.wi_f);
       }
       lw.wo2 = ld.f16(Lp + "mlp.Wo.weight", {H, I});
     }
@@ -753,11 +747,11 @@ Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::v
         const std::string Lp = P + "layers." + std::to_string(li) + ".";
         std::vector<float> g_attn, g_mlp;
         if (lw.wqkv_f) ld.host_f32(Lp + "attn_norm.weight", g_attn, {H});
-        if (lw.wi_f) ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
+        ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
         stack({Lp + "attn.Wqkv.weight"}, 3 * H, H, w);
         if (!ld.ok) break;
-        gw.wqkv = ld.up_f16(w);
         if (lw.wqkv_f) fold_weights(ld, w, g_attn, T * 3 * H, H, &gw.wqkv_f);
+        else gw.wqkv = ld.up_f16(w);
         stack({Lp + "attn.Wo.weight"}, H, H, w);
         if (!ld.ok) break;
         gw.wo = ld.up_f16(w);
@@ -773,8 +767,7 @@ Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::v
               memcpy(dst + static_cast<size_t>(64 * j + 32) * H, src + static_cast<size_t>(I + 32 * j) * H, sizeof(float) * 32 * H);
             }
           }
-          gw.wi = ld.up_f16(perm);
-          if (lw.wi_f) fold_weights(ld, perm, g_mlp, T * 2 * I, H, &gw.wi_f);
+          fold_weights(ld, perm, g_mlp, T * 2 * I, H, &gw.wi_f);
         }
         stack({Lp + "mlp.Wo.weight"}, H, I, w);
         if (!ld.ok) break;
@@ -804,7 +797,7 @@ Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::v
       const std::string Lp = P + "layers." + std::to_string(li) + ".";
       std::vector<float> g_attn, g_mlp;
       if (lw.wqkv_f) ld.host_f32(Lp + "attn_norm.weight", g_attn, {H});
-      if (lw.wi_f) ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
+      ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
       build_lora_proj(ld, sts, alpha, {{Lp + "attn.Wqkv", 0, 3 * H}}, 3 * H, H, rp, g_attn, ident, ll.qkv);
       build_lora_proj(ld, sts, alpha, {{Lp + "attn.Wo", 0, H}}, H, H, rp, none, ident, ll.wo);
       build_lora_proj(ld, sts, alpha, {{Lp + "mlp.Wi", 0, 2 * I}}, 2 * I, H, rp, g_mlp, geglu_perm, ll.wi);
@@ -972,15 +965,6 @@ int workspace_reserve(Model& m, int tokens, int seqs, size_t out_elems) {
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
-// SRB_RESID_HL=0 keeps the fp32 residual stream + fp16 copy on the LayerNorm-fold path (A/B measurements)
-static bool resid_hl_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("SRB_RESID_HL");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-
 int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers) {
   if (m.precise.on) return encoder_forward_precise(m, d_ids, d_cu, B, T, max_len, num_layers);
   const EncoderConfig& c = m.cfg;
@@ -1025,53 +1009,53 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
     return gemm_f16(s, gd);
   };
   if (c.arch == ARCH_MODERNBERT) {
-    // Residual stream as an fp16 pair (gemm.h: EPI_RESID_HL) whenever every LayerNorm of the stack is folded: w.h / w.lo hold
-    // x - pivot, the residual GEMMs update the pair in place, and the fp32 form is rebuilt once after the last layer.
-    bool hl = resid_hl_enabled() && w.lo != nullptr;
-    for (int li = 0; li < c.L && hl; ++li) hl = m.layers[li].wi_f != nullptr && (li == 0 || m.layers[li].wqkv_f != nullptr);
+    // Residual stream as an fp16 pair (gemm.h: EPI_RESID_HL): w.h / w.lo hold x - pivot, the residual GEMMs update the
+    // pair in place, and the fp32 form is rebuilt once after the last layer.  LayerNorm fold (gemm.h): each residual
+    // GEMM also leaves the per-row (sum, sum of squares) of x - pivot in w.row_stats; the projection that consumes
+    // LN(x) multiplies the raw rows w.h with W diag(gamma) and corrects per row in its epilogue -- no LayerNorm pass.
+    // Layer 0's attn_norm (when the checkpoint has one) is the exception: it runs on the fp32 embedding output.
+    const bool ln0 = m.layers[0].attn_norm_w != nullptr;
     { ProfScope ps(m, PC_EMBED);
-      if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, m.emb_word, m.emb_ln_w, c.ln_eps, hl ? nullptr : w.x, w.h, hl ? w.lo : nullptr)) return -1; }
-    // LayerNorm fold (gemm.h): the residual GEMM that finishes x also leaves fp16(x) in w.h and the per-row
-    // (sum, sum of squares) in w.row_stats; the projection that consumes LN(x) multiplies the raw rows with
-    // W diag(gamma) and corrects per row in its epilogue -- no LayerNorm pass over the fp32 stream.
-    // `folded` says which of the two forms w.h currently holds.
-    bool folded = false;
-    // one statistics record, padded so that the second record keeps the float2 alignment of the partials
+      if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, m.emb_word, m.emb_ln_w, c.ln_eps, ln0 ? w.x : nullptr, w.h, w.lo)) return -1; }
+    // one statistics record [H/128][T][2] partials + [T] pivots, padded so that the second record keeps the float2
+    // alignment of the partials; the residual GEMMs ping-pong between the two
     const size_t rec = (static_cast<size_t>(T) * (2 * static_cast<size_t>(H / 128) + 1) + 3) & ~static_cast<size_t>(3);
-    int n_rec = 0;                 // records written so far in this forward (ping-pong between the two)
+    const size_t piv_off = static_cast<size_t>(T) * 2 * (H / 128);
+    int n_rec = 0;                 // records written so far in this forward
     const float* cur_stats = nullptr;
-    auto emit_for = [&](GemmDesc& gd, bool want) {   // make this residual GEMM produce the fold operands
-      if (!want) return 0;
+    auto emit_for = [&](GemmDesc& gd) {   // this residual GEMM updates the pair and writes the next record
       float* dst = w.row_stats + (n_rec & 1) * rec;
-      gd.row_stats = dst;                                   // [H/128][T][2] partials, every one overwritten
-      gd.pivot_out = dst + static_cast<size_t>(T) * 2 * (H / 128);
+      gd.epi = EPI_RESID_HL; gd.out = w.h; gd.ldo = H; gd.lo16 = w.lo;
+      gd.row_stats = dst;                                   // every partial overwritten
+      gd.pivot_out = dst + piv_off;
       if (n_rec > 0) {                                      // pivot = the row mean after the previous residual GEMM
-        const float* prev = w.row_stats + ((n_rec - 1) & 1) * rec;
-        gd.pivot_in_stats = prev;
-        gd.pivot_in = prev + static_cast<size_t>(T) * 2 * (H / 128);
+        gd.pivot_in_stats = cur_stats;
+        gd.pivot_in = cur_stats + piv_off;
       }
-      if (hl) { gd.epi = EPI_RESID_HL; gd.out = w.h; gd.lo16 = w.lo; gd.resid = nullptr; gd.ldr = 0; }
-      else gd.raw16 = w.h;
       cur_stats = dst;
       ++n_rec;
-      return 0;
     };
     for (int li = 0; li < L; ++li) {
       const LayerWeights& lw = grouped ? m.lora.glayers[li] : m.layers[li];
       const LoraLayer& ll = lora_on ? m.lora.layers[li] : no_lora;
       const bool local = (li % c.global_every) != 0;
-      if (folded) {
-        // w.h = fp16(x) and w.row_stats were written by the previous layer's MLP-out GEMM
-      } else if (lw.attn_norm_w) {
-        ProfScope ps(m, PC_NORM);
-        if (layernorm_rows(s, w.x, T, H, lw.attn_norm_w, nullptr, c.ln_eps, nullptr, w.h)) return -1;
-      } else if (li != 0) {
-        ProfScope ps(m, PC_NORM);
-        if (cast_rows_f16(s, w.x, static_cast<size_t>(T) * H, w.h)) return -1;
-      }
+      const bool folded = lw.wqkv_f != nullptr;   // model_load: li > 0 with attn_norm
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = 3 * H; g.K = H; g.A = w.h; g.W = lw.wqkv; g.out = w.qkv; g.ldo = 3 * H;
-      if (folded) { g.W = lw.wqkv_f; g.fold_stats = cur_stats; g.fold_eps = c.ln_eps; g.fold_h = H; }
+      if (folded) {
+        g.W = lw.wqkv_f; g.fold_stats = cur_stats; g.fold_eps = c.ln_eps; g.fold_h = H;
+      } else if (li > 0 || ln0) {
+        // A = fp16(attn_norm(x)) or, without attn_norm, fp16(x) in w.ctx: free here (the previous Wo has consumed it,
+        // this layer's attention has not written it yet)
+        ProfScope ps(m, PC_NORM);
+        if (li == 0) {
+          if (layernorm_rows(s, w.x, T, H, lw.attn_norm_w, nullptr, c.ln_eps, nullptr, w.ctx)) return -1;
+        } else {
+          if (hl_to_f32(s, w.h, w.lo, cur_stats + piv_off, T, H, w.x)) return -1;
+          if (cast_rows_f16(s, w.x, static_cast<size_t>(T) * H, w.ctx)) return -1;
+        }
+        g.A = w.ctx;
+      }
       g.epi = EPI_ROPE; g.pos = w.pos; g.rope_cols = 2 * H;
       g.rope_cos = local ? m.rope_cos_l : m.rope_cos_g;
       g.rope_sin = local ? m.rope_sin_l : m.rope_sin_g;
@@ -1080,32 +1064,25 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       { ProfScope ps(m, PC_ATTN);   // sliding-window layers visit only the key blocks inside the window
         if (attention_wgmma_fwd(s, w.qkv, w.ctx, d_cu, B, max_len, c.heads, 64, local ? c.local_attention / 2 : 0)) return -1; }
       g = GemmDesc();
-      g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = H; g.A = w.ctx; g.W = lw.wo; g.out = w.x; g.ldo = H;
-      g.epi = EPI_RESID; g.resid = w.x; g.ldr = H;
-      const bool fold_mlp = lw.wi_f != nullptr;
-      if (emit_for(g, fold_mlp || hl)) return -1;
+      g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = H; g.A = w.ctx; g.W = lw.wo;
+      emit_for(g);
       if (lora_ext(g, ll.wo, false, PC_GEMM_WO)) return -1;
       { ProfScope ps(m, PC_GEMM_WO); if (run_proj(g)) return -1; }
-      if (!fold_mlp) { ProfScope ps(m, PC_NORM); if (layernorm_rows(s, w.x, T, H, lw.mid_norm_w, nullptr, c.ln_eps, nullptr, w.h)) return -1; }
       g = GemmDesc();
-      g.M = T; g.a_rows = w.cap_tokens; g.N = 2 * I; g.K = H; g.A = w.h; g.W = lw.wi; g.out = w.mid; g.ldo = I;
-      if (fold_mlp) { g.W = lw.wi_f; g.fold_stats = cur_stats; g.fold_eps = c.ln_eps; g.fold_h = H; }
+      g.M = T; g.a_rows = w.cap_tokens; g.N = 2 * I; g.K = H; g.A = w.h; g.W = lw.wi_f; g.out = w.mid; g.ldo = I;
+      g.fold_stats = cur_stats; g.fold_eps = c.ln_eps; g.fold_h = H;
       g.epi = EPI_GEGLU;
-      if (lora_ext(g, ll.wi, fold_mlp, PC_GEMM_WI)) return -1;
+      if (lora_ext(g, ll.wi, true, PC_GEMM_WI)) return -1;
       { ProfScope ps(m, PC_GEMM_WI); if (run_proj(g)) return -1; }
       g = GemmDesc();
-      g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = I; g.A = w.mid; g.W = lw.wo2; g.out = w.x; g.ldo = H;
-      g.epi = EPI_RESID; g.resid = w.x; g.ldr = H;
-      // the next layer's attn_norm rides on this GEMM (the last executed layer feeds final_norm, which the heads fuse)
-      folded = li + 1 < L && m.layers[li + 1].wqkv_f != nullptr;
-      if (emit_for(g, folded || hl)) return -1;
+      g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = I; g.A = w.mid; g.W = lw.wo2;
+      emit_for(g);
       if (lora_ext(g, ll.wo2, false, PC_GEMM_WO2)) return -1;
       { ProfScope ps(m, PC_GEMM_WO2); if (run_proj(g)) return -1; }
     }
-    if (hl) {   // x = pivot + hi + lo for the heads (final_norm, pooling, token heads read the fp32 stream)
+    {   // x = pivot + hi + lo for the heads (final_norm, pooling, token heads read the fp32 stream)
       ProfScope ps(m, PC_NORM);
-      const float* piv = n_rec > 0 ? w.row_stats + ((n_rec - 1) & 1) * rec + static_cast<size_t>(T) * 2 * (H / 128) : nullptr;
-      if (hl_to_f32(s, w.h, w.lo, piv, T, H, w.x)) return -1;
+      if (hl_to_f32(s, w.h, w.lo, cur_stats + piv_off, T, H, w.x)) return -1;
     }
   } else {
     ProfScope ps_embed(m, PC_EMBED);

@@ -16,8 +16,8 @@ enum GemmEpilogue {
   // The residual stream as an fp16 PAIR, in place: with x - pivot = hi + lo (hi = fp16(x - pivot), lo = fp16 of the rest),
   // out (hi) and lo16 [M,N] fp16 are read, updated to (x - pivot) + acc (+bias) re-centred on the new pivot, and written
   // back, together with the row statistics of the LayerNorm fold.  hi IS the raw fp16 copy the next projection
-  // multiplies, so the residual GEMM moves 4 + 4 bytes per element where fp32 + copy moves 4 + 6; the pair carries
-  // 22 significant bits of x - pivot.  row_stats and pivot_out are required.
+  // multiplies, so the residual GEMM moves 4 + 4 bytes per element; the pair carries 22 significant bits of
+  // x - pivot.  row_stats and pivot_out are required.
   EPI_RESID_HL = 6,
 };
 
@@ -38,9 +38,9 @@ struct GemmDesc {
   int rope_cols = 0;
   // ---- LayerNorm folded into the GEMMs around it (pre-LN models): LN(x) W^T = rstd * (x - mean 1) (W diag(gamma))^T
   // = rstd * x W''^T with W'' = W diag(gamma) re-centred so that every row sums to zero (the centring matrix commutes
-  // into the weights).  The residual GEMM that finishes x (EPI_RESID) also emits fp16(x) and the per-row (sum, sum of
-  // squares); the consuming projection (EPI_ROPE / EPI_GEGLU) multiplies the RAW fp16 rows with W'' and scales by the
-  // row's rstd in its epilogue.  No separate pass over the fp32 stream, no mean subtraction anywhere.
+  // into the weights).  The residual GEMM that finishes x (EPI_RESID_HL) leaves the fp16 pair, whose high half is the
+  // fp16 copy of x, and the per-row (sum, sum of squares); the consuming projection (EPI_ROPE / EPI_GEGLU) multiplies
+  // the RAW fp16 rows with W'' and scales by the row's rstd in its epilogue.  No LayerNorm pass, no mean subtraction.
   // Statistics are kept as PARTIALS over fixed 128-column slices, [N/128][M][2] fp32, each written exactly once and
   // summed by the consumer in slice order: bitwise reproducible whatever the tile shape, schedule or batch
   // composition (atomics would make the result depend on arrival order).
@@ -55,15 +55,15 @@ struct GemmDesc {
   const uint8_t* topk_valid = nullptr;
   int topk_n = 0;
   int* topk_lists = nullptr;        // host out
-  float* row_stats = nullptr;       // EPI_RESID: fp32 [N/128][M][2] (sum, sum of squares) per 128-column slice
-  void* raw16 = nullptr;            // EPI_RESID: fp16 [M, N] copy of the fp32 result (minus the row pivot), ld = N
+  float* row_stats = nullptr;       // EPI_RESID_HL: fp32 [N/128][M][2] (sum, sum of squares) per 128-column slice
   void* lo16 = nullptr;             // EPI_RESID_HL: fp16 [M, N] low halves (ld = N); `out` holds the high halves (ldo = N)
-  // Row pivot: LayerNorm is shift-invariant and the zero-sum rows of W'' cancel any per-row constant, so the fp16 copy
+  // Row pivot: LayerNorm is shift-invariant and the zero-sum rows of W'' cancel any per-row constant, so the pair
   // and the statistics are taken of x - pivot_r, with pivot_r = the row's mean after the PREVIOUS residual GEMM (read
   // from that GEMM's statistics).  Rounding x - pivot instead of x keeps the fold exact-ish for rows whose common
   // offset dwarfs their spread (fp16(x) alone would lose (x - mean) there); variances are also better conditioned.
-  float* pivot_out = nullptr;          // EPI_RESID: fp32 [M], this GEMM's pivots (written next to row_stats)
-  const float* pivot_in = nullptr;     // EPI_RESID: fp32 [M] pivots of the previous residual GEMM (null: pivot 0)
+  // gemm_f16 refuses row_stats and pivots on every other epilogue.
+  float* pivot_out = nullptr;          // EPI_RESID_HL: fp32 [M], this GEMM's pivots (written next to row_stats)
+  const float* pivot_in = nullptr;     // EPI_RESID_HL: fp32 [M] pivots of the previous residual GEMM (null: pivot 0)
   const float* pivot_in_stats = nullptr;  // its statistics partials [N/128][M][2]
   const float* fold_stats = nullptr;   // EPI_ROPE / EPI_GEGLU: fp32 [fold_h/128][M][2] partials of the A rows
   float fold_eps = 0.f;

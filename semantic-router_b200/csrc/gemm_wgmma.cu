@@ -52,8 +52,7 @@ struct GemmCfg {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kRawBufs = EPI == EPI_RESID ? 2 : 0;   // fp16 copy of the residual stream (LayerNorm fold)
-  static constexpr int kEpiBytes = kEpiWarps * (kBufs + kRawBufs) * kStageBufBytes;
+  static constexpr int kEpiBytes = kEpiWarps * kBufs * kStageBufBytes;
   static constexpr int kFit = (kSmemLimit - kAccBytes - kEpiBytes - 1024 /*align slack*/ - kBarrierBytes) / kStageBytes;
   static constexpr int kStages = kFit < 6 ? kFit : 6;   // as deep as shared memory allows, 6 at most
   static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + kEpiBytes + 1024 + kBarrierBytes;
@@ -68,13 +67,12 @@ struct KArgs {
   const float* rope_cos;
   const float* rope_sin;
   int rope_cols;
-  float* row_stats;          // EPI_RESID: accumulate (sum, sumsq) per row
-  int has_raw16;             // EPI_RESID: tmap_aux is the fp16 copy of the output
+  float* row_stats;          // EPI_RESID_HL: (sum, sumsq) per row and 128-column slice
   const float* fold_stats;   // EPI_ROPE / EPI_GEGLU: per-row (sum, sumsq) of the A rows (null: no fold)
   float fold_eps;
   float fold_inv_h;
   int fold_parts;            // 128-column slices the row statistics come in
-  float* pivot_out;          // EPI_RESID: row pivots (see gemm.h)
+  float* pivot_out;          // EPI_RESID_HL: row pivots (see gemm.h)
   const float* pivot_in;
   const float* pivot_in_stats;
   int* topk_idx;             // EPI_TOPK
@@ -342,13 +340,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   } else {
     // ================= epilogue warps: shared fp32 tile -> registers -> swizzled smem box -> TMA store =================
     const int quad = warp;  // 32-row quarter of the tile this warp owns (one row per lane)
-    uint8_t* my_bufs = smem_epi + warp * ((kStageBufs + Cfg::kRawBufs) * kStageBufBytes);
-    uint8_t* my_raw = my_bufs + kStageBufs * kStageBufBytes;   // [kRawBufs] fp16 boxes (32 rows x 64 columns)
-    const bool want_raw = (EPI == EPI_RESID) && p.has_raw16;
-    const bool want_stats = (EPI == EPI_RESID || kHL) && p.row_stats != nullptr;
+    uint8_t* my_bufs = smem_epi + warp * (kStageBufs * kStageBufBytes);
     const bool fold = (EPI == EPI_ROPE || EPI == EPI_GEGLU) && p.fold_stats != nullptr;
     float f_rstd = 1.f;   // fold: rstd of this thread's row
-    float pv = 0.f;       // fold producer: this thread's row pivot (EPI_RESID_HL: the pivot SHIFT of this GEMM)
+    float pv = 0.f;       // EPI_RESID_HL: the pivot SHIFT of this GEMM for this thread's row
     float pv_prev = 0.f;  // EPI_RESID_HL: the pivot the stored pair is relative to
     int pv_mblk = -1;
     int fold_mblk = -1;
@@ -473,7 +468,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           rope_mblk = m_blk;
         }
       }
-      float st1 = 0.f, st2 = 0.f;   // EPI_RESID: this row's (sum, sum of squares) over the current 128-column slice
+      float st1 = 0.f, st2 = 0.f;   // EPI_RESID_HL: this row's (sum, sum of squares) over the current 128-column slice
       if constexpr (kHL) {
         // pivot shift of this row: the stored pair is x - pivot_in; the new pivot is pivot_in + (mean of x - pivot_in),
         // read from the previous residual GEMM's statistics (0 for the first one: the embedding's pair is x itself)
@@ -488,20 +483,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
               s1 += __ldg(reinterpret_cast<const float2*>(p.pivot_in_stats) + static_cast<size_t>(k) * p.M + row).x;
             pv = s1 / static_cast<float>(p.N);
             pv_prev = __ldg(p.pivot_in + row);
-          }
-          pv_mblk = m_blk;
-        }
-      }
-      if constexpr (EPI == EPI_RESID) {
-        if (want_stats && m_blk != pv_mblk) {   // the row's pivot: its mean after the previous residual GEMM
-          pv = 0.f;
-          if (p.pivot_in_stats) {
-            const int row = row0 + lane < p.M ? row0 + lane : p.M - 1;
-            float s1 = 0.f;
-            const int parts = p.N >> 7;
-            for (int k = 0; k < parts; ++k)
-              s1 += __ldg(reinterpret_cast<const float2*>(p.pivot_in_stats) + static_cast<size_t>(k) * p.M + row).x;
-            pv = __ldg(p.pivot_in + row) + s1 / static_cast<float>(p.N);
           }
           pv_mblk = m_blk;
         }
@@ -568,7 +549,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       }
       if constexpr (kHL) {
         // 64-column chunks: the (hi, lo) boxes of the chunk arrive by TMA one chunk ahead, are updated in place in
-        // shared memory and leave by TMA; statistics per 128-column slice as in EPI_RESID
+        // shared memory and leave by TMA; statistics go out per 128-column slice
 #pragma unroll 1
         for (int c = 0; c < kChunks; ++c) {
           const int ocol0 = out_col(t, c);
@@ -668,28 +649,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
               x.x += b.x; x.y += b.y; x.z += b.z; x.w += b.w;
             }
             *q = x;
-            x.x -= pv; x.y -= pv; x.z -= pv; x.w -= pv;   // statistics and the fp16 copy are taken of x - pivot
-            st1 += (x.x + x.y) + (x.z + x.w);
-            st2 += (x.x * x.x + x.y * x.y) + (x.z * x.z + x.w * x.w);
-            if (want_raw) {   // fp16 copy: chunk c fills 16-byte units (c & 1) * 4 + i / 2 of the 64-column box
-              r[2 * i] = pack_half2(x.x, x.y);
-              r[2 * i + 1] = pack_half2(x.z, x.w);
-            }
-          }
-          if (want_stats && (c & 3) == 3) {   // a 128-column slice is complete: its partial goes out, once
-            if (row0 + lane < p.M) {
-              const size_t part = static_cast<size_t>((ocol0 - 96) >> 7);
-              *reinterpret_cast<float2*>(p.row_stats + 2 * (part * p.M + row0 + lane)) = make_float2(st1, st2);
-              if (part == 0 && p.pivot_out) p.pivot_out[row0 + lane] = pv;
-            }
-            st1 = 0.f;
-            st2 = 0.f;
-          }
-          if (want_raw) {
-            uint8_t* rb = my_raw + ((c >> 1) & 1) * kStageBufBytes;
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              sts16(rb + box_off(lane, (c & 1) * 4 + i), r[4 * i], r[4 * i + 1], r[4 * i + 2], r[4 * i + 3]);
           }
         } else if constexpr (EPI == EPI_F16 || EPI == EPI_GELU) {
 #pragma unroll
@@ -768,11 +727,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         __syncwarp();
         if (lane == 0) {
           tma_store_2d(&tmap_out, buf, ocol0, row0);  // rows >= M / cols >= N are clipped by the TMA unit
-          if constexpr (EPI == EPI_RESID) {
-            // the fp16 box completes every second chunk and rides in the same bulk group as that chunk's fp32 store
-            // (its staging box is next written two chunks later, after the wait_group.read above)
-            if (want_raw && (c & 1)) tma_store_2d(&tmap_aux, my_raw + ((c >> 1) & 1) * kStageBufBytes, ocol0 - 32, row0);
-          }
           bulk_commit();
         }
         if (++cb == kStageBufs) cb = 0;
@@ -961,8 +915,14 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
     return -1;
   }
   const bool is_hl = g.epi == EPI_RESID_HL;
-  if (is_hl && (!g.lo16 || !g.row_stats || !g.pivot_out || g.N % 128 != 0 || g.ldo != g.N || g.raw16 || g.resid)) {
-    fprintf(stderr, "[srb200] gemm_f16: EPI_RESID_HL needs out (hi) + lo16 with ld = N, row_stats, pivot_out, N %% 128 == 0\n");
+  if (is_hl && (!g.lo16 || !g.row_stats || !g.pivot_out || g.N % 128 != 0 || g.ldo != g.N || g.resid ||
+                (g.pivot_in != nullptr) != (g.pivot_in_stats != nullptr))) {
+    fprintf(stderr, "[srb200] gemm_f16: EPI_RESID_HL needs out (hi) + lo16 with ld = N, row_stats, pivot_out, "
+                    "pivot_in with pivot_in_stats, N %% 128 == 0\n");
+    return -1;
+  }
+  if (!is_hl && (g.lo16 || g.row_stats || g.pivot_out || g.pivot_in || g.pivot_in_stats)) {
+    fprintf(stderr, "[srb200] gemm_f16: lo16, row_stats and pivots belong to EPI_RESID_HL\n");
     return -1;
   }
   if (g.epi == EPI_GEGLU && g.N % 128 != 0) {
@@ -996,7 +956,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   ka.M = g.M; ka.N = g.N; ka.K = g.K;
   ka.bias = g.bias; ka.has_resid = g.resid != nullptr;
   ka.pos = g.pos; ka.rope_cos = g.rope_cos; ka.rope_sin = g.rope_sin; ka.rope_cols = g.rope_cols;
-  ka.row_stats = nullptr; ka.has_raw16 = 0;
+  ka.row_stats = g.row_stats;
   ka.pivot_out = g.pivot_out; ka.pivot_in = g.pivot_in; ka.pivot_in_stats = g.pivot_in_stats;
   ka.topk_idx = g.topk_idx; ka.topk_score = g.topk_score; ka.topk_valid = g.topk_valid; ka.topk_n = g.topk_n;
   ka.grouped = 0;
@@ -1006,10 +966,6 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   static const int interleave_min_k = [] { const char* e = getenv("SRB_RESID_INTERLEAVE"); return (e && e[0] == '2') ? 0 : 768; }();
   ka.interleave = (((g.epi == EPI_RESID && g.resid != nullptr) || is_hl) && resid_interleave && (is_hl || g.K > interleave_min_k) &&
                    g.N / BN > 1) ? 1 : 0;
-  if ((g.pivot_in != nullptr) != (g.pivot_in_stats != nullptr) || ((g.pivot_out || g.pivot_in) && !g.row_stats)) {
-    fprintf(stderr, "[srb200] gemm_f16: pivots come with row_stats, pivot_in with pivot_in_stats\n");
-    return -1;
-  }
   ka.fold_stats = nullptr; ka.fold_eps = 0.f; ka.fold_inv_h = 0.f; ka.fold_parts = 0;
   ka.K2 = 0; ka.mask_block = 0; ka.mask_rows = 0;
   ka.grp_rows = w_groups > 1 ? g.w_group_rows : 0;
@@ -1030,21 +986,8 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
     }
     ka.mask_block = g.mask_block; ka.mask_rows = g.mask_rows;
   }
-  CUtensorMap tx = tc;   // auxiliary output map (fp16 copy of the residual stream); unused otherwise
-  if (is_hl) {
-    if (make_tmap_2d(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.lo16, g.N, g.M, g.N, 64, 32)) return -1;
-    ka.row_stats = g.row_stats;
-  } else if (g.row_stats || g.raw16) {
-    if (g.epi != EPI_RESID || g.N % 128 != 0) {
-      fprintf(stderr, "[srb200] gemm_f16: row_stats / raw16 belong to EPI_RESID with N %% 128 == 0\n");
-      return -1;
-    }
-    ka.row_stats = g.row_stats;
-    if (g.raw16) {
-      if (make_tmap_2d(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.raw16, g.N, g.M, g.N, 64, 32)) return -1;
-      ka.has_raw16 = 1;
-    }
-  }
+  CUtensorMap tx = tc;   // auxiliary map (EPI_RESID_HL: the low halves of the pair); unused otherwise
+  if (is_hl && make_tmap_2d(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.lo16, g.N, g.M, g.N, 64, 32)) return -1;
   if (g.fold_stats) {
     if ((g.epi != EPI_ROPE && g.epi != EPI_GEGLU) || g.fold_h <= 0 || g.fold_h % 128 != 0) {
       fprintf(stderr, "[srb200] gemm_f16: LayerNorm fold belongs to EPI_ROPE / EPI_GEGLU with the row length\n");

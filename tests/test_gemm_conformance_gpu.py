@@ -31,25 +31,12 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 S16 = 0x7E5A          # sentinel bits: fp16 NaN with a payload
 S32 = 0x7FC0DEAD      # fp32 NaN with a payload
-vp, ci = C.c_void_p, C.c_int
 DEV = "cuda"
-
-
-class GemmDesc(C.Structure):
-    _fields_ = [("m", ci), ("n", ci), ("k", ci), ("a", vp), ("a_rows", ci), ("w", vp), ("out", vp), ("ldo", ci),
-                ("epi", ci), ("bias", vp), ("resid", vp), ("ldr", ci), ("pos", vp), ("rope_cos", vp), ("rope_sin", vp),
-                ("rope_cols", ci), ("topk_idx", vp), ("topk_score", vp), ("topk_valid", vp), ("topk_n", ci),
-                ("row_stats", vp), ("raw16", vp), ("lo16", vp), ("pivot_out", vp), ("pivot_in", vp),
-                ("pivot_in_stats", vp), ("fold_stats", vp), ("fold_eps", C.c_float), ("fold_h", ci), ("a2", vp),
-                ("w2", vp), ("k2", ci), ("w_groups", ci), ("w_group_rows", ci), ("mask_block", ci), ("mask_rows", ci)]
 
 
 @pytest.fixture(scope="module")
 def lib(srlib, cuda):
-    H = srlib.hooks()
-    H.sr_test_gemm_desc.argtypes = [C.POINTER(GemmDesc), C.POINTER(C.c_int)]
-    H.sr_test_gemm_cluster.argtypes = [ci, ci, ci, vp, vp]
-    return H
+    return srlib.hooks()
 
 
 _TAU_SEEN = {}
@@ -66,15 +53,12 @@ def _tau_report():
             print(f"  {k:10s} {v:.3e}" + (f"  (2^{math.log2(v):.2f})" if v > 0 else ""))
 
 
-def run(lib, sync=True, **kw):
-    d = GemmDesc()
-    for k, v in kw.items():
-        setattr(d, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
-    lists = C.c_int(0)
-    rc = lib.sr_test_gemm_desc(C.byref(d), C.byref(lists))
+def run(sync=True, **kw):
+    import semantic_router_b200 as pkg
+    rc, lists = pkg.binding.run_gemm(**kw)
     if sync:
         torch.cuda.synchronize()
-    return rc, lists.value
+    return rc, lists
 
 
 def _cluster(lib, epi, n, k):
@@ -208,8 +192,8 @@ def problem(epi, M, N, K, seed, *, bias=False, resid=True, k2=0, fold=False, rop
     return p
 
 
-def check_parity(lib, p, tag=None):
-    rc, _ = run(lib, **p.desc)
+def check_parity(p, tag=None):
+    rc, _ = run(**p.desc)
     assert rc == 0
     p.check_sentinels()
     got = p.result()
@@ -252,7 +236,7 @@ def _shape_cases():
 def test_shape_edges(lib, epi, M, N, K, i):
     p = problem(epi, M, N, K, seed=1000 * epi + i, bias=epi in (EPI_F16, EPI_RESID, EPI_GELU, EPI_RESID_HL),
                 resid=(i % 2 == 0), rope_cols=ROPE_COLS.get(N, 0))
-    check_parity(lib, p)
+    check_parity(p)
 
 
 K2_EPIS = [(EPI_F16, 320), (EPI_ROPE, 2304), (EPI_RESID, 192), (EPI_GEGLU, 2304), (EPI_GELU, 320), (EPI_RESID_HL, 640)]
@@ -263,7 +247,7 @@ K2_EPIS = [(EPI_F16, 320), (EPI_ROPE, 2304), (EPI_RESID, 192), (EPI_GEGLU, 2304)
 def test_k_extension(lib, epi, N, k2, M, K):
     p = problem(epi, M, N, K, seed=7 * k2 + epi, bias=epi in (EPI_F16, EPI_RESID, EPI_GELU, EPI_RESID_HL), k2=k2,
                 rope_cols=ROPE_COLS.get(N, 0))
-    check_parity(lib, p)
+    check_parity(p)
 
 
 @pytest.mark.parametrize("k2", [0, 64, 24])
@@ -273,7 +257,7 @@ def test_layernorm_fold(lib, epi, N, M, k2):
     """The fold scales the whole accumulator (the K extension included: A2 is produced without rstd) by the row's rstd,
     which depends on the LayerNorm epsilon for rows of small variance."""
     p = problem(epi, M, N, 768, seed=31 * M + k2, k2=k2, fold=True, rope_cols=ROPE_COLS.get(N, 0), w_scale=0.01)
-    check_parity(lib, p, tag=go.EPI_NAMES[epi] + "+fold")
+    check_parity(p, tag=go.EPI_NAMES[epi] + "+fold")
 
 
 @pytest.mark.parametrize("mask_rows", [128, 256])
@@ -283,7 +267,7 @@ def test_mask_producer(lib, block, mask_rows):
     tasks = 3
     R = (tasks * block + 63) // 64 * 64
     p = problem(EPI_F16, tasks * mask_rows, R, 200, seed=block + mask_rows, mask_block=block, mask_rows=mask_rows)
-    check_parity(lib, p, tag="f16+mask")
+    check_parity(p, tag="f16+mask")
 
 
 @pytest.mark.parametrize("rows", [128, 256])
@@ -293,7 +277,7 @@ def test_grouped_weights(lib, epi, N, K, rows):
     when w_group_rows is a multiple of 128, which is what gemm_f16 accepts."""
     p = problem(epi, 3 * rows - 5, N, K, seed=rows + epi, w_groups=3, w_group_rows=rows, rope_cols=ROPE_COLS.get(N, 0),
                 bias=epi == EPI_F16)
-    check_parity(lib, p, tag=go.EPI_NAMES[epi] + "+grp")
+    check_parity(p, tag=go.EPI_NAMES[epi] + "+grp")
 
 
 # ---- the cache scan: GEMV (B <= 4), fused top-8 epilogue (one row block, and the grouped schedule), two-pass (k > 8)
@@ -372,7 +356,7 @@ def test_cluster_pair_equals_unclustered_halves(lib, epi, fold, k2):
         p = problem(epi, M, 2304, 768, seed=M + 3 * k2 + fold, k2=k2, fold=fold, rope_cols=1536,
                     w_scale=0.01 if fold else 0.05)
         d = p.desc
-        assert run(lib, **d)[0] == 0
+        assert run(**d)[0] == 0
         full = p.out[:M].clone()
         p.out.view(torch.int16).fill_(S16)
         half_out = p.n_out // 2
@@ -382,7 +366,7 @@ def test_cluster_pair_equals_unclustered_halves(lib, epi, fold, k2):
                 dh["w2"] = d["w2"][1152 * h:1152 * (h + 1)]
             if epi == EPI_ROPE:
                 dh["rope_cols"] = 1152 if h == 0 else 1536 - 1152
-            assert run(lib, **dh)[0] == 0
+            assert run(**dh)[0] == 0
         assert torch.equal(_bits(full), _bits(p.out[:M])), M
 
 
@@ -393,13 +377,13 @@ def test_k_extension_is_concatenation(lib, epi, N, k2):
     M, K = 2333, 768
     p = problem(epi, M, N, K, seed=k2 + N, k2=k2, rope_cols=ROPE_COLS.get(N, 0), resid=False)
     d = p.desc
-    assert run(lib, **d)[0] == 0
+    assert run(**d)[0] == 0
     ext = p.out[:M].clone()
     cat_a = torch.cat([d["a"], d["a2"]], 1).contiguous()
     cat_w = torch.cat([d["w"], d["w2"]], 1).contiguous()
     dc = {k: v for k, v in d.items() if k not in ("a2", "w2", "k2")}
     dc.update(a=cat_a, w=cat_w, k=K + k2)
-    assert run(lib, **dc)[0] == 0
+    assert run(**dc)[0] == 0
     assert torch.equal(_bits(ext), _bits(p.out[:M]))
 
 
@@ -409,12 +393,12 @@ def test_grouped_weights_are_per_group_gemms(lib, epi, rows):
     M, N, K = 3 * rows, 384, 200
     p = problem(epi, M, N, K, seed=rows, w_groups=3, w_group_rows=rows, resid=False)
     d = p.desc
-    assert run(lib, **d)[0] == 0
+    assert run(**d)[0] == 0
     grouped = p.out[:M].clone()
     for g in range(3):
         dg = {k: v for k, v in d.items() if k not in ("w_groups", "w_group_rows")}
         dg.update(m=rows, a=d["a"][g * rows:], a_rows=rows, w=d["w"][g * N:(g + 1) * N], out=p.out[g * rows:])
-        assert run(lib, **dg)[0] == 0
+        assert run(**dg)[0] == 0
     assert torch.equal(_bits(grouped), _bits(p.out[:M]))
 
 
@@ -430,14 +414,14 @@ def test_stale_rows(lib, epi, N, M):
     d = p.desc
     out0 = p.out.clone()
     lo0 = p.lo.clone() if p.lo is not None else None
-    assert run(lib, **d)[0] == 0
+    assert run(**d)[0] == 0
     p.check_sentinels()
     stale = [p.out[:M].clone()] + ([p.lo[:M].clone()] if p.lo is not None else [])
     p.out.copy_(out0)
     if lo0 is not None:
         p.lo.copy_(lo0)
     exact = dict(d, a=d["a"][:M].clone(), a2=d["a2"][:M].clone(), a_rows=M)
-    assert run(lib, **exact)[0] == 0
+    assert run(**exact)[0] == 0
     again = [p.out[:M]] + ([p.lo[:M]] if p.lo is not None else [])
     for x, y in zip(stale, again):
         assert torch.equal(_bits(x), _bits(y))
@@ -447,20 +431,17 @@ def test_stale_rows(lib, epi, N, M):
 _CHILD = r'''
 import os, sys
 sys.path[:0] = [sys.argv[1], os.path.join(sys.argv[1], "tests")]
-import ctypes as C
 import numpy as np
 import torch
 import semantic_router_b200 as pkg
 import test_gemm_conformance_gpu as t
-H = pkg.hooks()
-H.sr_test_gemm_desc.argtypes = [C.POINTER(t.GemmDesc), C.POINTER(C.c_int)]
 res = {}
 # fp32 residual GEMMs in place: interleaved by default for K > 768, for every K with SRB_RESID_INTERLEAVE=2;
 # N = 704 ends in a half-empty column tile, where the residual prefetch cursor must stop at n_out
 for name, (M, N, K) in {"resid_704_1152": (2333, 704, 1152), "resid_768_768": (2333, 768, 768),
                         "resid_704_768": (16897, 704, 768)}.items():
     p = t.problem(t.EPI_RESID, M, N, K, seed=N + K, bias=True)
-    assert t.run(H, **p.desc)[0] == 0
+    assert t.run(**p.desc)[0] == 0
     res[name] = p.out.cpu().numpy()
 # three chained fp16-pair residual GEMMs with pivots, queued back to back as the encoder issues them (the PDL chain)
 M, N = 2333, 768
@@ -472,7 +453,7 @@ for step in range(3):
     ds = dict(p.desc, row_stats=dst, pivot_out=dst[part:])
     if step:
         ds.update(pivot_in=prev[part:], pivot_in_stats=prev)
-    assert t.run(H, sync=False, **ds)[0] == 0
+    assert t.run(sync=False, **ds)[0] == 0
 torch.cuda.synchronize()
 res["hl_hi"], res["hl_lo"] = p.out.cpu().numpy(), p.lo.cpu().numpy()
 res["hl_stats"] = torch.cat(recs).cpu().numpy()
@@ -523,6 +504,8 @@ REFUSED = {
     "mask_not_f16": dict(epi=EPI_GELU, N=128, K=64, mask=(8, 128)),
     "group_rows_192": dict(epi=EPI_F16, N=128, K=64, groups=192),
     "group_rows_64": dict(epi=EPI_F16, N=128, K=64, groups=64),
+    "stats_not_pair": dict(epi=EPI_RESID, N=128, K=64, row_stats=True),
+    "pivot_not_pair": dict(epi=EPI_F16, N=128, K=64, pivot_out=True),
 }
 
 
@@ -544,6 +527,10 @@ def test_refusals(lib, case):
         d.update(mask_block=c["mask"][0], mask_rows=c["mask"][1])
     if "groups" in c:
         d.update(w_groups=3, w_group_rows=c["groups"])
-    rc, _ = run(lib, **d)
+    if "row_stats" in c:
+        d.update(row_stats=torch.zeros(N // 128, M, 2, device=dev))
+    if "pivot_out" in c:
+        d.update(pivot_out=torch.zeros(M, device=dev))
+    rc, _ = run(**d)
     assert rc != 0
     assert (out.view(torch.int16) == S16).all()

@@ -10,6 +10,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 EPI_F16, EPI_ROPE, EPI_RESID, EPI_GEGLU, EPI_GELU = range(5)
+EPI_RESID_HL = 6
 
 
 def _ptr(t):
@@ -21,6 +22,14 @@ def _gemm(lib, a, w, out, epi, bias=None, resid=None, pos=None, cos=None, sin=No
     N = w.shape[0]
     rc = lib.sr_test_gemm(_ptr(a), _ptr(w), _ptr(out), M, N, K, epi, out.shape[1], _ptr(bias), _ptr(resid),
                           _ptr(pos), _ptr(cos), _ptr(sin), rope_cols)
+    torch.cuda.synchronize()
+    assert rc == 0
+
+
+def _gemm_desc(srlib, a, w, out, epi, **fields):
+    """sr_test_gemm_desc: A [M, K], W [N, K], ldo = out's row length; `fields` are further GemmDesc fields"""
+    M, K = a.shape
+    rc, _ = srlib.binding.run_gemm(m=M, n=w.shape[0], k=K, a=a, w=w, out=out, ldo=out.shape[1], epi=epi, **fields)
     torch.cuda.synchronize()
     assert rc == 0
 
@@ -151,32 +160,24 @@ def test_attention(srlib, cuda, lens, window, impl):
 
 
 @pytest.mark.parametrize("M", [300, 2500])
-def test_gemm_layernorm_fold(srlib, cuda, M):
-    """LayerNorm folded into the GEMMs around it: the residual GEMM emits fp16(x) and per-row (sum, sum of squares);
-    the consuming projections multiply the raw rows with W diag(gamma) re-centred to zero-sum rows (the mean subtraction
-    moves into the weights) and scale by the row's rstd in the epilogue.
+def test_gemm_layernorm_fold_from_pair(srlib, cuda, M):
+    """LayerNorm folded into the GEMMs around it: the fp16-pair residual GEMM leaves fp16(x) in hi and per-row (sum, sum
+    of squares); the consuming projections multiply the raw rows with W diag(gamma) re-centred to zero-sum rows (the mean
+    subtraction moves into the weights) and scale by the row's rstd in the epilogue.
     Checked against torch LayerNorm + plain matmuls, for the RoPE and the GeGLU consumer."""
     from oracle import encoder_oracle as eo
-    lib = srlib.lib()
     H, I, nH = 768, 1152, 12
     g = torch.Generator(device="cuda").manual_seed(M)
-    # ---- producer: x += a @ w^T, fp16 copy, row statistics
+    # ---- producer: (hi + lo) += a @ w^T, row statistics (pivot 0)
     a = torch.randn(M, H, device=cuda, generator=g).half()
     w = (torch.randn(H, H, device=cuda, generator=g) * 0.05).half()
     x0 = torch.randn(M, H, device=cuda, generator=g) * 2 + 0.3
-    x = x0.clone()
+    raw = x0.half()
+    lo = (x0 - raw.float()).half()
     stats = torch.full((H // 128, M, 2), float("nan"), device=cuda)   # per-128-column partials, each written once
-    raw = torch.full((M, H), float("nan"), device=cuda, dtype=torch.float16)
-    rc = lib.sr_test_gemm_fold(_ptr(a), _ptr(w), _ptr(x), M, H, H, EPI_RESID, H, None, _ptr(x), None, None, None, 0,
-                               _ptr(stats), _ptr(raw), None, 0.0, 0, None, None, None)
-    torch.cuda.synchronize()
-    assert rc == 0
+    _gemm_desc(srlib, a, w, raw, EPI_RESID_HL, lo16=lo, row_stats=stats, pivot_out=torch.empty(M, device=cuda))
     ref_x = a.float() @ w.float().t() + x0
-    torch.testing.assert_close(x, ref_x, rtol=1e-4, atol=2e-4)
     torch.testing.assert_close(raw.float(), ref_x, rtol=1e-3, atol=2e-3)
-    torch.testing.assert_close(stats[..., 0].sum(0), ref_x.sum(1), rtol=1e-4, atol=2e-2)
-    torch.testing.assert_close(stats[..., 1].sum(0), (ref_x * ref_x).sum(1), rtol=1e-4, atol=1e-1)
-    torch.testing.assert_close(stats[2, :, 0], ref_x[:, 256:384].sum(1), rtol=1e-4, atol=1e-2)
     gamma = 1 + 0.2 * torch.randn(H, device=cuda, generator=g)
     ln = torch.nn.functional.layer_norm(ref_x, (H,), gamma, None, 1e-5)
     # ---- consumer 1: Wqkv + RoPE over the raw rows
@@ -187,10 +188,8 @@ def test_gemm_layernorm_fold(srlib, cuda, M):
     cos, sin = eo.rope_tables(64, 160000.0, 1024)
     cos, sin = cos.to(cuda).contiguous(), sin.to(cuda).contiguous()
     out = torch.zeros(M, 3 * H, device=cuda, dtype=torch.float16)
-    rc = lib.sr_test_gemm_fold(_ptr(raw), _ptr(wq_f), _ptr(out), M, 3 * H, H, EPI_ROPE, 3 * H, None, None, _ptr(pos), _ptr(cos),
-                               _ptr(sin), 2 * H, None, None, _ptr(stats), 1e-5, H, None, None, None)
-    torch.cuda.synchronize()
-    assert rc == 0
+    _gemm_desc(srlib, raw, wq_f, out, EPI_ROPE, pos=pos, rope_cos=cos, rope_sin=sin, rope_cols=2 * H, fold_stats=stats,
+               fold_eps=1e-5, fold_h=H)
     full = (ln @ wq.t()).reshape(M, 3, nH, 64)
     c, s = cos[pos.long()][:, None, :], sin[pos.long()][:, None, :]
     ref = full.clone()
@@ -209,42 +208,36 @@ def test_gemm_layernorm_fold(srlib, cuda, M):
         perm[64 * j + 32:64 * j + 64] = wi_f[I + 32 * j:I + 32 * j + 32]
     perm = perm.contiguous()
     mid = torch.zeros(M, I, device=cuda, dtype=torch.float16)
-    rc = lib.sr_test_gemm_fold(_ptr(raw), _ptr(perm), _ptr(mid), M, 2 * I, H, EPI_GEGLU, I, None, None, None, None, None, 0,
-                               None, None, _ptr(stats), 1e-5, H, None, None, None)
-    torch.cuda.synchronize()
-    assert rc == 0
+    _gemm_desc(srlib, raw, perm, mid, EPI_GEGLU, fold_stats=stats, fold_eps=1e-5, fold_h=H)
     fi = ln @ wi.t()
     # products of two projections (|values| up to ~10): the bound is relative to that scale
     torch.testing.assert_close(mid.float(), torch.nn.functional.gelu(fi[:, :I]) * fi[:, I:], rtol=4e-3, atol=8e-3)
 
 
-def test_gemm_layernorm_fold_pivot(srlib, cuda):
+def test_gemm_layernorm_fold_pivot_from_pair(srlib, cuda):
     """Rows whose common offset dwarfs their spread (mean 300, std 1): fp16(x) alone would lose x - mean; the fold takes
-    its fp16 copy and statistics of x - pivot, the pivot being the row mean after the previous residual GEMM."""
-    lib = srlib.lib()
+    its fp16 copy (hi of the fp16 pair) and statistics of x - pivot, the pivot being the row mean after the previous
+    residual GEMM."""
     M, H = 700, 768
     g = torch.Generator(device="cuda").manual_seed(77)
     a = torch.randn(M, H, device=cuda, generator=g).half()
     w = (torch.randn(H, H, device=cuda, generator=g) * 0.02).half()
     x0 = torch.randn(M, H, device=cuda, generator=g) + 300.0 + 20.0 * torch.randn(M, 1, device=cuda, generator=g)
-    x = x0.clone()
+    raw = x0.half()
+    lo = (x0 - raw.float()).half()
     parts = H // 128
     recs = [torch.full((parts * M * 2 + M,), float("nan"), device=cuda) for _ in range(2)]
-    raw = torch.zeros(M, H, device=cuda, dtype=torch.float16)
-    def producer(k):
-        dst, prev = recs[k & 1], recs[(k - 1) & 1]
-        piv_out = dst[parts * M * 2:]
-        rc = lib.sr_test_gemm_fold(_ptr(a), _ptr(w), _ptr(x), M, H, H, EPI_RESID, H, None, _ptr(x), None, None, None, 0,
-                                   _ptr(dst), _ptr(raw), None, 0.0, 0, piv_out.data_ptr(),
-                                   prev[parts * M * 2:].data_ptr() if k else None, _ptr(prev) if k else None)
-        torch.cuda.synchronize()
-        assert rc == 0
     ref_x = x0.clone()
     for k in range(2):     # the second GEMM has a pivot (the first one's row means)
-        producer(k)
+        dst, prev = recs[k & 1], recs[(k - 1) & 1]
+        _gemm_desc(srlib, a, w, raw, EPI_RESID_HL, lo16=lo, row_stats=dst, pivot_out=dst[parts * M * 2:],
+                   pivot_in=prev[parts * M * 2:] if k else None, pivot_in_stats=prev if k else None)
         ref_x = a.float() @ w.float().t() + ref_x
-    torch.testing.assert_close(x, ref_x, rtol=1e-5, atol=1e-3)
     piv = recs[1][parts * M * 2:]
+    x = torch.empty(M, H, device=cuda)
+    assert srlib.hooks().sr_test_hl_to_f32(_ptr(raw), _ptr(lo), _ptr(piv), M, H, _ptr(x)) == 0
+    torch.cuda.synchronize()
+    torch.testing.assert_close(x, ref_x, rtol=1e-5, atol=1e-3)
     assert (piv - (ref_x - a.float() @ w.float().t()).mean(1)).abs().max() < 1e-2      # = mean after the first GEMM
     # consumer on the pivoted copy: LN(x) Wq^T with zero-sum-row weights
     gamma = 1 + 0.2 * torch.randn(H, device=cuda, generator=g)
@@ -254,10 +247,8 @@ def test_gemm_layernorm_fold_pivot(srlib, cuda):
     out = torch.zeros(M, 256, device=cuda, dtype=torch.float16)
     pos = torch.zeros(M, device=cuda, dtype=torch.int32)
     cos = torch.ones(4, 32, device=cuda); sin = torch.zeros(4, 32, device=cuda)
-    rc = lib.sr_test_gemm_fold(_ptr(raw), _ptr(wq_f), _ptr(out), M, 256, H, EPI_ROPE, 256, None, None, _ptr(pos), _ptr(cos), _ptr(sin),
-                               0, None, None, _ptr(recs[1]), 1e-5, H, None, None, None)
-    torch.cuda.synchronize()
-    assert rc == 0
+    _gemm_desc(srlib, raw, wq_f, out, EPI_ROPE, pos=pos, rope_cos=cos, rope_sin=sin, rope_cols=0, fold_stats=recs[1],
+               fold_eps=1e-5, fold_h=H)
     ref = torch.nn.functional.layer_norm(ref_x, (H,), gamma, None, 1e-5) @ wq.t()
     torch.testing.assert_close(out.float(), ref, rtol=3e-3, atol=3e-3)
 

@@ -101,9 +101,9 @@ def p(t):
 
 
 def call_fold(a, w, out, n, epi, n_out, rope_cols):
-    rc = H.sr_test_gemm_fold(p(a), p(w), p(out), M, n, Hd, epi, n_out, None, None, p(pos) if epi == EPI_ROPE else None,
-                             p(cos) if epi == EPI_ROPE else None, p(sin) if epi == EPI_ROPE else None, rope_cols,
-                             None, None, p(fold_stats), 1e-5, Hd, None, None, None)
+    rope = dict(pos=pos, rope_cos=cos, rope_sin=sin, rope_cols=rope_cols) if epi == EPI_ROPE else {}
+    rc, _ = pkg.binding.run_gemm(m=M, n=n, k=Hd, a=a, w=w, out=out, ldo=n_out, epi=epi, fold_stats=fold_stats,
+                                 fold_eps=1e-5, fold_h=Hd, **rope)
     assert rc == 0
 
 
