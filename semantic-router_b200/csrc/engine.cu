@@ -11,6 +11,7 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstring>
 #include <memory>
@@ -325,6 +326,179 @@ void rope_tables(int head_dim, double theta, int max_pos, std::vector<float>& cs
     }
 }
 
+// Tensor-name prefix of the encoder in a checkpoint.  ModernBERT: the first prefix the reference loaders try whose
+// tok_embeddings exist.  BERT: "bert." or "" by its word_embeddings or, in a head-only checkpoint, by its pooler.
+// false: no encoder embeddings under any known prefix.
+bool tensor_prefix(const SafeTensors& st, Arch arch, std::string& P) {
+  if (arch == ARCH_MODERNBERT) {
+    for (const char* p : {"model.", "_orig_mod.model.", "", "_orig_mod."})
+      if (st.find(std::string(p) + "embeddings.tok_embeddings.weight")) { P = p; return true; }
+    P.clear();
+    return false;
+  }
+  if (st.find("bert.embeddings.word_embeddings.weight")) { P = "bert."; return true; }
+  if (st.find("embeddings.word_embeddings.weight")) { P.clear(); return true; }
+  P = st.find("bert.pooler.dense.weight") ? "bert." : "";
+  return false;
+}
+
+std::string layer_prefix(const EncoderConfig& c, const std::string& P, int li) {
+  return P + (c.arch == ARCH_MODERNBERT ? "layers." : "encoder.layer.") + std::to_string(li) + ".";
+}
+
+// One encoder projection: how the checkpoint stores it and how the kernels read it.
+struct Segment {        // `stem`.weight [rows, K] fills source rows [row0, row0 + rows); its device rows carry `scale`
+  std::string stem;
+  int row0, rows;
+  float scale;
+};
+struct Projection {
+  std::vector<Segment> segs;
+  int N = 0, K = 0;                  // source shape
+  bool bias = false;                 // BERT: `stem`.bias [rows] beside every segment's weight
+  int dN = 0, dK = 0;                // device shape
+  std::vector<int> row_of, col_of;   // source row / column -> device row / column; empty: identity
+  std::string gamma;                 // LayerNorm weight the device weight is folded with (fold_weights); empty: none
+};
+Projection projection(std::vector<Segment> segs, int N, int K) {
+  Projection p;
+  p.segs = std::move(segs);
+  p.N = p.dN = N;
+  p.K = p.dK = K;
+  return p;
+}
+
+// The four projections of layer li in the order qkv, attention output, intermediate, output (LoraLayer, PreciseLayer).
+std::array<Projection, 4> layer_projections(const EncoderConfig& c, const std::string& P, int li, bool has_attn_norm) {
+  const int H = c.H, I = c.I;
+  const std::string Lp = layer_prefix(c, P, li);
+  std::array<Projection, 4> pr;
+  if (c.arch == ARCH_MODERNBERT) {
+    pr[0] = projection({{Lp + "attn.Wqkv", 0, 3 * H, 1.f}}, 3 * H, H);
+    pr[1] = projection({{Lp + "attn.Wo", 0, H, 1.f}}, H, H);
+    pr[2] = projection({{Lp + "mlp.Wi", 0, 2 * I, 1.f}}, 2 * I, H);
+    pr[3] = projection({{Lp + "mlp.Wo", 0, H, 1.f}}, H, I);
+    // Wqkv runs LayerNorm-folded where its attn_norm follows a residual GEMM; layer 0 and layers without attn_norm
+    // multiply the plain weight (encoder_forward).  Wi always runs folded with mlp_norm.
+    if (li > 0 && has_attn_norm) pr[0].gamma = Lp + "attn_norm.weight";
+    pr[2].gamma = Lp + "mlp_norm.weight";
+    // GeGLU interleave for the fused epilogue: 32-row groups [a(32j..) | b(32j..)] (gemm.h EPI_GEGLU)
+    pr[2].row_of.resize(static_cast<size_t>(2) * I);
+    for (int j = 0; j < I / 32; ++j)
+      for (int i = 0; i < 32; ++i) {
+        pr[2].row_of[32 * j + i] = 64 * j + i;
+        pr[2].row_of[I + 32 * j + i] = 64 * j + 32 + i;
+      }
+    return pr;
+  }
+  // MiniLM: heads of 32 are zero-padded to 64 (EncoderConfig::attn_w).  The kernels scale scores by 64^-0.5; the model
+  // wants 32^-0.5, so the query rows carry the missing sqrt(2).
+  const bool padded = c.attn_w != H;
+  const float qs = padded ? 1.41421356237309504880f : 1.f;
+  pr[0] = projection({{Lp + "attention.self.query", 0, H, qs}, {Lp + "attention.self.key", H, H, 1.f},
+                      {Lp + "attention.self.value", 2 * H, H, 1.f}}, 3 * H, H);
+  pr[1] = projection({{Lp + "attention.output.dense", 0, H, 1.f}}, H, H);
+  pr[2] = projection({{Lp + "intermediate.dense", 0, I, 1.f}}, I, H);
+  pr[3] = projection({{Lp + "output.dense", 0, H, 1.f}}, H, I);
+  for (Projection& p : pr) p.bias = true;
+  if (padded) {   // q / k / v rows (h*64 + d) <- (h*32 + d); the attention output reads the padded context columns
+    const int hd = H / c.heads;
+    pr[0].dN = 3 * c.attn_w;
+    pr[1].dK = c.attn_w;
+    pr[1].col_of.resize(H);
+    pr[0].row_of.resize(static_cast<size_t>(3) * H);
+    for (int i = 0; i < H; ++i) {
+      pr[1].col_of[i] = i / hd * 64 + i % hd;
+      for (int s = 0; s < 3; ++s) pr[0].row_of[s * H + i] = s * c.attn_w + pr[1].col_of[i];
+    }
+  }
+  return pr;
+}
+
+// Source-order host weight of a projection (its segments stacked, adapters merged unless the loader keeps them) and,
+// when `bias` is given, its bias
+bool read_projection(Loader& ld, const Projection& pr, std::vector<float>& w, std::vector<float>* bias) {
+  std::vector<float> v;
+  w.clear();
+  for (const Segment& s : pr.segs) {
+    if (!ld.host_f32(s.stem + ".weight", v, {s.rows, pr.K})) return false;
+    w.insert(w.end(), v.begin(), v.end());
+  }
+  if (bias) {
+    bias->clear();
+    for (const Segment& s : pr.segs) {
+      if (!ld.host_f32(s.stem + ".bias", v, {s.rows})) return false;
+      bias->insert(bias->end(), v.begin(), v.end());
+    }
+  }
+  return true;
+}
+
+// read_projection, then into the device layout: rows through row_of, columns through col_of, times the segment's scale,
+// zeros where no source element lands
+bool device_projection(Loader& ld, const Projection& pr, std::vector<float>& w, std::vector<float>* bias) {
+  if (!read_projection(ld, pr, w, bias)) return false;
+  std::vector<float> dw(static_cast<size_t>(pr.dN) * pr.dK, 0.f), db(bias ? pr.dN : 0, 0.f);
+  for (const Segment& s : pr.segs)
+    for (int n = s.row0; n < s.row0 + s.rows; ++n) {
+      const size_t r = pr.row_of.empty() ? n : pr.row_of[n];
+      for (int k = 0; k < pr.K; ++k)
+        dw[r * pr.dK + (pr.col_of.empty() ? k : pr.col_of[k])] = w[static_cast<size_t>(n) * pr.K + k] * s.scale;
+      if (bias) db[r] = (*bias)[n] * s.scale;
+    }
+  w.swap(dw);
+  if (bias) bias->swap(db);
+  return true;
+}
+
+// W'' = W diag(gamma), every row re-centred to sum zero, rounded to fp16.  Two refinement passes push the sum of the
+// ROUNDED row (what the tensor core multiplies) from ~1e-4 down to the last bit of its largest elements, so the
+// residual mean * sum(W''[n,:]) is far below the fp16 rounding of the output.
+__half* fold_weights(Loader& ld, const std::vector<float>& w, const std::vector<float>& gamma, int n, int k) {
+  std::vector<float> wf(w.size());
+  std::vector<double> row(k);
+  for (int r = 0; r < n; ++r) {
+    double s = 0.0;
+    for (int c = 0; c < k; ++c) { row[c] = static_cast<double>(w[static_cast<size_t>(r) * k + c]) * gamma[c]; s += row[c]; }
+    const double mu = s / k;
+    for (int c = 0; c < k; ++c) row[c] -= mu;
+    for (int pass = 0; pass < 3; ++pass) {
+      double rs = 0.0;
+      for (int c = 0; c < k; ++c) rs += __half2float(__float2half_rn(static_cast<float>(row[c])));
+      if (rs == 0.0) break;
+      for (int c = 0; c < k; ++c) row[c] -= rs / k;
+    }
+    for (int c = 0; c < k; ++c) wf[static_cast<size_t>(r) * k + c] = static_cast<float>(row[c]);
+  }
+  return ld.up_f16(wf);
+}
+
+// fp16 upload of `rows` device rows of K-wide weights, folded with `gamma` when it names a LayerNorm weight
+__half* upload_weight(Loader& ld, const std::vector<float>& w, const std::string& gamma, int rows, int K) {
+  if (gamma.empty()) return ld.up_f16(w);
+  std::vector<float> g;
+  return ld.host_f32(gamma, g, {K}) ? fold_weights(ld, w, g, rows, K) : nullptr;
+}
+
+// Device form of projection p of a layer: uploads `w` (T stacked device weights in the grouped form) into the plain or the
+// folded slot
+void store_projection(Loader& ld, const Projection& pr, int p, const std::vector<float>& w, int copies, LayerWeights& lw) {
+  __half** plain[] = {&lw.wqkv, &lw.wo, &lw.wi, &lw.wo2};
+  __half** slot = pr.gamma.empty() ? plain[p] : (p == 0 ? &lw.wqkv_f : &lw.wi_f);
+  *slot = upload_weight(ld, w, pr.gamma, copies * pr.dN, pr.dK);
+}
+
+// The ordinary model: the four projections of one layer (and BERT's biases) from the loader's checkpoint
+void load_projections(Loader& ld, const std::array<Projection, 4>& pr, LayerWeights& lw) {
+  float** biases[] = {&lw.bqkv, &lw.bo, &lw.bi, &lw.bo2};
+  for (int p = 0; p < 4 && ld.ok; ++p) {
+    std::vector<float> w, b;
+    if (!device_projection(ld, pr[p], w, pr[p].bias ? &b : nullptr)) return;
+    store_projection(ld, pr[p], p, w, 1, lw);
+    if (pr[p].bias) *biases[p] = ld.up_f32(b);
+  }
+}
+
 bool load_head(Loader& ld, const Json& cfgj, Arch arch, int H, const std::string& bert_prefix,
                int force_token_level, Head& hd) {
   const SafeTensors& st = *ld.st;
@@ -366,28 +540,6 @@ bool load_head(Loader& ld, const Json& cfgj, Arch arch, int H, const std::string
 // ------------------------------------------------------------------------------------------------
 // model load
 // ------------------------------------------------------------------------------------------------
-// W'' = W diag(gamma), every row re-centred to sum zero, rounded to fp16.  Two refinement passes push the sum of the
-// ROUNDED row (what the tensor core multiplies) from ~1e-4 down to the last bit of its largest elements, so the
-// residual mean * sum(W''[n,:]) is far below the fp16 rounding of the output.
-static void fold_weights(Loader& ld, const std::vector<float>& w, const std::vector<float>& gamma, int n, int k, __half** w_f) {
-  std::vector<float> wf(w.size());
-  std::vector<double> row(k);
-  for (int r = 0; r < n; ++r) {
-    double s = 0.0;
-    for (int c = 0; c < k; ++c) { row[c] = static_cast<double>(w[static_cast<size_t>(r) * k + c]) * gamma[c]; s += row[c]; }
-    const double mu = s / k;
-    for (int c = 0; c < k; ++c) row[c] -= mu;
-    for (int pass = 0; pass < 3; ++pass) {
-      double rs = 0.0;
-      for (int c = 0; c < k; ++c) rs += __half2float(__float2half_rn(static_cast<float>(row[c])));
-      if (rs == 0.0) break;
-      for (int c = 0; c < k; ++c) row[c] -= rs / k;
-    }
-    for (int c = 0; c < k; ++c) wf[static_cast<size_t>(r) * k + c] = static_cast<float>(row[c]);
-  }
-  *w_f = ld.up_f16(wf);
-}
-
 Model* model_load(const std::string& dir, int device, std::string* err, int flags) {
   std::string e;
   int ndev = 0;
@@ -419,20 +571,9 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
   EncoderConfig& c = m->cfg;
   const std::string mt = cfgj.str_or("model_type", "");
   std::string P;  // tensor-name prefix
-  if (mt == "modernbert" || st.find("model.embeddings.tok_embeddings.weight") ||
-      st.find("embeddings.tok_embeddings.weight") || st.find("_orig_mod.model.embeddings.tok_embeddings.weight")) {
-    c.arch = ARCH_MODERNBERT;
-    const char* prefixes[] = {"model.", "_orig_mod.model.", "", "_orig_mod."};
-    bool found = false;
-    for (const char* p : prefixes)
-      if (st.find(std::string(p) + "embeddings.tok_embeddings.weight")) { P = p; found = true; break; }
-    if (!found) ld.fail("no tok_embeddings tensor under any known prefix");
-  } else {
-    c.arch = ARCH_BERT;
-    if (st.find("bert.embeddings.word_embeddings.weight")) P = "bert.";
-    else if (st.find("embeddings.word_embeddings.weight")) P = "";
-    else ld.fail("no BERT word_embeddings tensor found");
-  }
+  c.arch = (mt == "modernbert" || tensor_prefix(st, ARCH_MODERNBERT, P)) ? ARCH_MODERNBERT : ARCH_BERT;
+  if (!tensor_prefix(st, c.arch, P))
+    ld.fail(c.arch == ARCH_MODERNBERT ? "no tok_embeddings tensor under any known prefix" : "no BERT word_embeddings tensor found");
   c.vocab = static_cast<int>(cfgj.num_or("vocab_size", 0));
   c.H = static_cast<int>(cfgj.num_or("hidden_size", 0));
   c.L = static_cast<int>(cfgj.num_or("num_hidden_layers", 0));
@@ -466,33 +607,11 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
     m->emb_ln_w = ld.f32(P + "embeddings.norm.weight", {H});
     m->layers.resize(c.L);
     for (int li = 0; li < c.L && ld.ok; ++li) {
-      const std::string Lp = P + "layers." + std::to_string(li) + ".";
+      const std::string Lp = layer_prefix(c, P, li);
       LayerWeights& lw = m->layers[li];
       if (st.find(Lp + "attn_norm.weight")) lw.attn_norm_w = ld.f32(Lp + "attn_norm.weight", {H});
-      std::vector<float> wq, g_attn, g_mlp;
-      // Wqkv runs LayerNorm-folded where its attn_norm follows a residual GEMM; layer 0 and layers without attn_norm
-      // multiply the plain weight (encoder_forward)
-      if (ld.host_f32(Lp + "attn.Wqkv.weight", wq, {3 * H, H})) {
-        if (li > 0 && lw.attn_norm_w && ld.host_f32(Lp + "attn_norm.weight", g_attn, {H}))
-          fold_weights(ld, wq, g_attn, 3 * H, H, &lw.wqkv_f);
-        else
-          lw.wqkv = ld.up_f16(wq);
-      }
-      lw.wo = ld.f16(Lp + "attn.Wo.weight", {H, H});
       lw.mid_norm_w = ld.f32(Lp + "mlp_norm.weight", {H});
-      ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
-      std::vector<float> wi, wi_perm;
-      if (ld.host_f32(Lp + "mlp.Wi.weight", wi, {2 * I, H})) {
-        // GeGLU interleave for the fused epilogue: 32-row groups [a(32j..) | b(32j..)] (gemm.h EPI_GEGLU)
-        wi_perm.resize(wi.size());
-        for (int j = 0; j < I / 32; ++j) {
-          memcpy(&wi_perm[static_cast<size_t>(64 * j) * H], &wi[static_cast<size_t>(32 * j) * H], sizeof(float) * 32 * H);
-          memcpy(&wi_perm[static_cast<size_t>(64 * j + 32) * H], &wi[static_cast<size_t>(I + 32 * j) * H],
-                 sizeof(float) * 32 * H);
-        }
-        if (!g_mlp.empty()) fold_weights(ld, wi_perm, g_mlp, 2 * I, H, &lw.wi_f);
-      }
-      lw.wo2 = ld.f16(Lp + "mlp.Wo.weight", {H, I});
+      load_projections(ld, layer_projections(c, P, li, lw.attn_norm_w != nullptr), lw);
     }
     m->final_norm_w = ld.f32(P + "final_norm.weight", {H});
     if (ld.ok) {
@@ -518,60 +637,11 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
     m->emb_ln_b = ld.f32(E + "LayerNorm.bias", {H});
     m->layers.resize(c.L);
     for (int li = 0; li < c.L && ld.ok; ++li) {
-      const std::string Lp = P + "encoder.layer." + std::to_string(li) + ".";
+      const std::string Lp = layer_prefix(c, P, li);
       LayerWeights& lw = m->layers[li];
-      std::vector<float> q, k, v, bq, bk, bv;
-      if (ld.host_f32(Lp + "attention.self.query.weight", q, {H, H}) &&
-          ld.host_f32(Lp + "attention.self.key.weight", k, {H, H}) &&
-          ld.host_f32(Lp + "attention.self.value.weight", v, {H, H}) &&
-          ld.host_f32(Lp + "attention.self.query.bias", bq, {H}) &&
-          ld.host_f32(Lp + "attention.self.key.bias", bk, {H}) &&
-          ld.host_f32(Lp + "attention.self.value.bias", bv, {H})) {
-        if (head_dim == 32) {
-          // rows (h*64 + d) <- rows (h*32 + d), zeros for d >= 32.  The kernels scale scores by 64^-0.5; the model
-          // wants 32^-0.5, so the query projection carries the missing sqrt(2).
-          auto pad_rows = [&](std::vector<float>& wgt, std::vector<float>& bias, float scale) {
-            std::vector<float> pw(static_cast<size_t>(c.attn_w) * H, 0.f), pb(c.attn_w, 0.f);
-            for (int h = 0; h < c.heads; ++h)
-              for (int d = 0; d < 32; ++d) {
-                const size_t src = static_cast<size_t>(h * 32 + d), dst = static_cast<size_t>(h * 64 + d);
-                for (int kk = 0; kk < H; ++kk) pw[dst * H + kk] = wgt[src * H + kk] * scale;
-                pb[dst] = bias[src] * scale;
-              }
-            wgt.swap(pw);
-            bias.swap(pb);
-          };
-          pad_rows(q, bq, 1.41421356237309504880f);
-          pad_rows(k, bk, 1.0f);
-          pad_rows(v, bv, 1.0f);
-        }
-        q.insert(q.end(), k.begin(), k.end());
-        q.insert(q.end(), v.begin(), v.end());
-        bq.insert(bq.end(), bk.begin(), bk.end());
-        bq.insert(bq.end(), bv.begin(), bv.end());
-        lw.wqkv = ld.up_f16(q);
-        lw.bqkv = ld.up_f32(bq);
-      }
-      if (head_dim == 32) {   // attention-output projection reads the padded context rows: zero columns for d >= 32
-        std::vector<float> wo;
-        if (ld.host_f32(Lp + "attention.output.dense.weight", wo, {H, H})) {
-          std::vector<float> pw(static_cast<size_t>(H) * c.attn_w, 0.f);
-          for (int o = 0; o < H; ++o)
-            for (int h = 0; h < c.heads; ++h)
-              for (int d = 0; d < 32; ++d)
-                pw[static_cast<size_t>(o) * c.attn_w + h * 64 + d] = wo[static_cast<size_t>(o) * H + h * 32 + d];
-          lw.wo = ld.up_f16(pw);
-        }
-      } else {
-        lw.wo = ld.f16(Lp + "attention.output.dense.weight", {H, H});
-      }
-      lw.bo = ld.f32(Lp + "attention.output.dense.bias", {H});
+      load_projections(ld, layer_projections(c, P, li, false), lw);
       lw.mid_norm_w = ld.f32(Lp + "attention.output.LayerNorm.weight", {H});
       lw.mid_norm_b = ld.f32(Lp + "attention.output.LayerNorm.bias", {H});
-      lw.wi = ld.f16(Lp + "intermediate.dense.weight", {I, H});
-      lw.bi = ld.f32(Lp + "intermediate.dense.bias", {I});
-      lw.wo2 = ld.f16(Lp + "output.dense.weight", {H, I});
-      lw.bo2 = ld.f32(Lp + "output.dense.bias", {H});
       lw.out_norm_w = ld.f32(Lp + "output.LayerNorm.weight", {H});
       lw.out_norm_b = ld.f32(Lp + "output.LayerNorm.bias", {H});
     }
@@ -599,7 +669,8 @@ int model_add_head(Model* m, const std::string& dir, int force_token_level, std:
   if (!st.open(dir + "/model.safetensors", &e)) { *err = e; return -1; }
   Loader ld{m, &st};
   Head hd;
-  const std::string bp = st.find("bert.pooler.dense.weight") ? "bert." : "";
+  std::string bp;
+  tensor_prefix(st, m->cfg.arch, bp);   // a head-only checkpoint has no embeddings: its pooler names the prefix
   if (!load_head(ld, cfgj, m->cfg.arch, m->cfg.H, bp, force_token_level, hd) || !ld.ok) {
     *err = ld.ok ? "no classifier.weight in " + dir : ld.err;
     return -1;
@@ -616,15 +687,14 @@ namespace {
 bool is_head_tensor(const std::string& n) {
   return n.compare(0, 11, "classifier.") == 0 || n.compare(0, 5, "head.") == 0 || n.find("pooler.") != std::string::npos;
 }
-struct AdapterSeg { std::string stem; int row0, rows; };   // one adapted nn.Linear inside a (possibly fused) projection
-
-// Stacks the adapters of every task for one projection [N, K] made of `segs` (engine.h: LoraProj).  gamma: LayerNorm
-// weight for the fold form (empty: none).  perm: destination row of source row n in the device weight (GeGLU
-// interleave), empty: identity.  Returns false on a malformed adapter; leaves lp empty when no task adapts the projection.
+// Stacks the adapters of every task for projection `pr` (engine.h: LoraProj): `b` rows land where pr.row_of puts the base
+// rows, and `a` gets a fold form when pr.gamma names one.  Padded-head encoders (pr.col_of) are refused before this.
+// Returns false on a malformed adapter; leaves lp empty when no task adapts the projection.
 bool build_lora_proj(Loader& ld, const std::vector<std::unique_ptr<SafeTensors>>& sts, const std::vector<double>& alpha,
-                     const std::vector<AdapterSeg>& segs, int N, int K, int rp, const std::vector<float>& gamma,
-                     const std::vector<int>& perm, LoraProj& lp) {
+                     const Projection& pr, int rp, LoraProj& lp) {
+  const std::vector<Segment>& segs = pr.segs;
   const int T = static_cast<int>(sts.size());
+  const int N = pr.dN, K = pr.K;
   const int nseg = static_cast<int>(segs.size());
   const int block = nseg * rp;
   const int R = (T * block + 63) / 64 * 64;
@@ -648,7 +718,7 @@ bool build_lora_proj(Loader& ld, const std::vector<std::unique_ptr<SafeTensors>>
       for (int j = 0; j < r; ++j) memcpy(&a[static_cast<size_t>(c0 + j) * K], &av[static_cast<size_t>(j) * K], sizeof(float) * K);
       for (int n = 0; n < segs[sg].rows; ++n) {
         const int src = segs[sg].row0 + n;
-        const int dst = perm.empty() ? src : perm[src];
+        const int dst = pr.row_of.empty() ? src : pr.row_of[src];
         for (int j = 0; j < r; ++j)
           b[static_cast<size_t>(dst) * R + c0 + j] = static_cast<float>(scaling * static_cast<double>(bv[static_cast<size_t>(n) * r + j]));
       }
@@ -657,7 +727,7 @@ bool build_lora_proj(Loader& ld, const std::vector<std::unique_ptr<SafeTensors>>
   if (!any) return true;
   lp.a = ld.up_f16(a);
   lp.b = ld.up_f16(b);
-  if (!gamma.empty()) fold_weights(ld, a, gamma, R, K, &lp.a_f);
+  if (!pr.gamma.empty()) lp.a_f = upload_weight(ld, a, pr.gamma, R, K);
   lp.R = R;
   lp.block = block;
   return ld.ok;
@@ -700,118 +770,33 @@ Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::v
   if (c.attn_w != c.H) { *err = "shared-LoRA serving is not available for padded-head (MiniLM) encoders"; model_free(m); return nullptr; }
   Loader ld{m, sts[0].get()};
   const int rp = (max_rank + 7) / 8 * 8;
-  const int H = c.H, I = c.I;
   m->lora.layers.resize(c.L);
   std::string P;
-  if (c.arch == ARCH_MODERNBERT) {
-    const char* prefixes[] = {"model.", "_orig_mod.model.", "", "_orig_mod."};
-    for (const char* p : prefixes)
-      if (sts[0]->find(std::string(p) + "embeddings.tok_embeddings.weight")) { P = p; break; }
-  } else if (sts[0]->find("bert.embeddings.word_embeddings.weight")) {
-    P = "bert.";
-  }
-  std::vector<int> geglu_perm;   // source row of Wi -> row of the interleaved device weight (model_load)
-  if (c.arch == ARCH_MODERNBERT) {
-    geglu_perm.resize(static_cast<size_t>(2) * I);
-    for (int j = 0; j < I / 32; ++j)
-      for (int i = 0; i < 32; ++i) {
-        geglu_perm[32 * j + i] = 64 * j + i;
-        geglu_perm[I + 32 * j + i] = 64 * j + 32 + i;
+  tensor_prefix(*sts[0], c.arch, P);
+  if (grouped) m->lora.glayers = m->layers;   // norms / biases are the base's (adapters touch projection weights only)
+  for (int li = 0; li < c.L && ld.ok; ++li) {
+    const auto pr = layer_projections(c, P, li, m->layers[li].attn_norm_w != nullptr);
+    LoraLayer& ll = m->lora.layers[li];
+    LoraProj* lps[] = {&ll.qkv, &ll.wo, &ll.wi, &ll.wo2};
+    for (int p = 0; p < 4 && ld.ok; ++p) {
+      if (!grouped) {
+        build_lora_proj(ld, sts, alpha, pr[p], rp, *lps[p]);
+        m->lora.max_R = std::max(m->lora.max_R, lps[p]->R);
+        continue;
       }
-  }
-  const std::vector<float> none;
-  const std::vector<int> ident;
-  if (grouped) {
-    // every task's merged weights, stacked along N.  Loader{.., sts[t]} merges task t's adapters exactly as a separately
-    // loaded model would (lora_fold, double precision, before the fp16 rounding).
-    m->lora.glayers = m->layers;   // norms / biases are the base's (adapters touch projection weights only)
-    auto stack = [&](const std::vector<std::string>& names, int rows_each, int K, std::vector<float>& out) {
-      // out = [task 0: names[0]; names[1]; ... | task 1: ... ], each name a [rows_each, K] Linear weight
-      out.clear();
-      out.reserve(static_cast<size_t>(T) * names.size() * rows_each * K);
+      // every task's merged weights, stacked along N.  Loader{.., sts[t]} merges task t's adapters exactly as a separately
+      // loaded model would (lora_fold, double precision, before the fp16 rounding).
+      std::vector<float> stack, w;
       for (int t = 0; t < T && ld.ok; ++t) {
         Loader lt{m, sts[t].get()};
         lt.lora_alpha = alpha[t];
-        for (const std::string& nm : names) {
-          std::vector<float> v;
-          if (!lt.host_f32(nm, v, {rows_each, K})) { ld.fail(lt.err.empty() ? "missing tensor " + nm : lt.err); return; }
-          out.insert(out.end(), v.begin(), v.end());
-        }
+        if (!device_projection(lt, pr[p], w, nullptr)) ld.fail(lt.err);
+        stack.insert(stack.end(), w.begin(), w.end());
       }
-    };
-    for (int li = 0; li < c.L && ld.ok; ++li) {
-      LayerWeights& gw = m->lora.glayers[li];
-      const LayerWeights& lw = m->layers[li];
-      std::vector<float> w;
-      if (c.arch == ARCH_MODERNBERT) {
-        const std::string Lp = P + "layers." + std::to_string(li) + ".";
-        std::vector<float> g_attn, g_mlp;
-        if (lw.wqkv_f) ld.host_f32(Lp + "attn_norm.weight", g_attn, {H});
-        ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
-        stack({Lp + "attn.Wqkv.weight"}, 3 * H, H, w);
-        if (!ld.ok) break;
-        if (lw.wqkv_f) fold_weights(ld, w, g_attn, T * 3 * H, H, &gw.wqkv_f);
-        else gw.wqkv = ld.up_f16(w);
-        stack({Lp + "attn.Wo.weight"}, H, H, w);
-        if (!ld.ok) break;
-        gw.wo = ld.up_f16(w);
-        stack({Lp + "mlp.Wi.weight"}, 2 * I, H, w);
-        if (!ld.ok) break;
-        {   // GeGLU interleave inside every task's block (model_load)
-          std::vector<float> perm(w.size());
-          for (int t = 0; t < T; ++t) {
-            const float* src = w.data() + static_cast<size_t>(t) * 2 * I * H;
-            float* dst = perm.data() + static_cast<size_t>(t) * 2 * I * H;
-            for (int j = 0; j < I / 32; ++j) {
-              memcpy(dst + static_cast<size_t>(64 * j) * H, src + static_cast<size_t>(32 * j) * H, sizeof(float) * 32 * H);
-              memcpy(dst + static_cast<size_t>(64 * j + 32) * H, src + static_cast<size_t>(I + 32 * j) * H, sizeof(float) * 32 * H);
-            }
-          }
-          fold_weights(ld, perm, g_mlp, T * 2 * I, H, &gw.wi_f);
-        }
-        stack({Lp + "mlp.Wo.weight"}, H, I, w);
-        if (!ld.ok) break;
-        gw.wo2 = ld.up_f16(w);
-      } else {
-        const std::string Lp = P + "encoder.layer." + std::to_string(li) + ".";
-        stack({Lp + "attention.self.query.weight", Lp + "attention.self.key.weight", Lp + "attention.self.value.weight"}, H, H, w);
-        if (!ld.ok) break;
-        gw.wqkv = ld.up_f16(w);
-        stack({Lp + "attention.output.dense.weight"}, H, H, w);
-        if (!ld.ok) break;
-        gw.wo = ld.up_f16(w);
-        stack({Lp + "intermediate.dense.weight"}, I, H, w);
-        if (!ld.ok) break;
-        gw.wi = ld.up_f16(w);
-        stack({Lp + "output.dense.weight"}, H, I, w);
-        if (!ld.ok) break;
-        gw.wo2 = ld.up_f16(w);
-      }
+      if (ld.ok) store_projection(ld, pr[p], p, stack, T, m->lora.glayers[li]);
     }
-    m->lora.grouped = true;
   }
-  for (int li = 0; li < c.L && ld.ok && !grouped; ++li) {
-    LoraLayer& ll = m->lora.layers[li];
-    const LayerWeights& lw = m->layers[li];
-    if (c.arch == ARCH_MODERNBERT) {
-      const std::string Lp = P + "layers." + std::to_string(li) + ".";
-      std::vector<float> g_attn, g_mlp;
-      if (lw.wqkv_f) ld.host_f32(Lp + "attn_norm.weight", g_attn, {H});
-      ld.host_f32(Lp + "mlp_norm.weight", g_mlp, {H});
-      build_lora_proj(ld, sts, alpha, {{Lp + "attn.Wqkv", 0, 3 * H}}, 3 * H, H, rp, g_attn, ident, ll.qkv);
-      build_lora_proj(ld, sts, alpha, {{Lp + "attn.Wo", 0, H}}, H, H, rp, none, ident, ll.wo);
-      build_lora_proj(ld, sts, alpha, {{Lp + "mlp.Wi", 0, 2 * I}}, 2 * I, H, rp, g_mlp, geglu_perm, ll.wi);
-      build_lora_proj(ld, sts, alpha, {{Lp + "mlp.Wo", 0, H}}, H, I, rp, none, ident, ll.wo2);
-    } else {
-      const std::string Lp = P + "encoder.layer." + std::to_string(li) + ".";
-      build_lora_proj(ld, sts, alpha, {{Lp + "attention.self.query", 0, H}, {Lp + "attention.self.key", H, H}, {Lp + "attention.self.value", 2 * H, H}},
-                      3 * H, H, rp, none, ident, ll.qkv);
-      build_lora_proj(ld, sts, alpha, {{Lp + "attention.output.dense", 0, H}}, H, H, rp, none, ident, ll.wo);
-      build_lora_proj(ld, sts, alpha, {{Lp + "intermediate.dense", 0, I}}, I, H, rp, none, ident, ll.wi);
-      build_lora_proj(ld, sts, alpha, {{Lp + "output.dense", 0, H}}, H, I, rp, none, ident, ll.wo2);
-    }
-    for (const LoraProj* lp : {&ll.qkv, &ll.wo, &ll.wi, &ll.wo2}) m->lora.max_R = std::max(m->lora.max_R, lp->R);
-  }
+  m->lora.grouped = grouped;
   if (!ld.ok) { *err = ld.err; model_free(m); return nullptr; }
   for (int t = 0; t < T; ++t) {
     const int h = model_add_head(m, dirs[t], token_level[t], err);
@@ -833,31 +818,23 @@ int checkpoint_has_adapters(const std::string& dir) {
   return 0;
 }
 
-// fp32 host copy of one tensor of <dir>/model.safetensors (precise.cu builds its split weights from the originals)
-bool load_host_tensor(const std::string& dir, const std::string& name, const std::vector<int64_t>& shape, std::vector<float>& out,
-                      std::string* err) {
-  static thread_local std::string cached_dir;
-  static thread_local std::unique_ptr<SafeTensors> cached;
-  if (!cached || cached_dir != dir) {
-    cached.reset(new SafeTensors());
-    cached_dir = dir;
-    if (!cached->open(dir + "/model.safetensors", err)) { cached.reset(); return false; }
-  }
-  const StTensor* t = cached->find(name);
-  if (!t) { *err = "missing tensor " + name; return false; }
-  if (t->shape != shape) { *err = "tensor " + name + " has an unexpected shape"; return false; }
-  if (!to_f32(*t, out)) { *err = "tensor " + name + " has unsupported dtype " + t->dtype; return false; }
-  return lora_fold(*cached, name, *t, lora_alpha_of(dir), out, err);   // same merged matrix the production weights hold
-}
-std::string modernbert_prefix(const std::string& dir) {
-  std::string err;
-  std::vector<float> tmp;
-  const char* prefixes[] = {"model.", "_orig_mod.model.", "", "_orig_mod."};
+bool read_source_projections(Model& m, std::string* err,
+                             const std::function<bool(int li, int p, const std::vector<float>& w, int N, int K)>& fn) {
   SafeTensors st;
-  if (!st.open(dir + "/model.safetensors", &err)) return "model.";
-  for (const char* p : prefixes)
-    if (st.find(std::string(p) + "embeddings.tok_embeddings.weight")) return p;
-  return "model.";
+  if (!st.open(m.dir + "/model.safetensors", err)) return false;
+  Loader ld{&m, &st};
+  ld.lora_alpha = lora_alpha_of(m.dir);
+  std::string P;
+  tensor_prefix(st, m.cfg.arch, P);
+  std::vector<float> w;
+  for (int li = 0; li < m.cfg.L; ++li) {
+    const auto pr = layer_projections(m.cfg, P, li, m.layers[li].attn_norm_w != nullptr);
+    for (int p = 0; p < 4; ++p) {
+      if (!read_projection(ld, pr[p], w, nullptr)) { *err = ld.err; return false; }
+      if (!fn(li, p, w, pr[p].N, pr[p].K)) return false;
+    }
+  }
+  return true;
 }
 
 void model_free(Model* m) {

@@ -7,6 +7,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <functional>
 #include <map>
 #include <mutex>
 #include <string>
@@ -201,6 +202,11 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
 Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
                               bool grouped, std::string* err);
 int checkpoint_has_adapters(const std::string& dir);
+// Opens <m.dir>/model.safetensors afresh and passes every layer's four projections (qkv, attention output, intermediate,
+// output) to fn as source-order fp32 [N, K] host weights, adapters merged as model_load merges them.  fn returning false
+// stops the walk (and leaves *err to fn).
+bool read_source_projections(Model& m, std::string* err,
+                             const std::function<bool(int li, int p, const std::vector<float>& w, int N, int K)>& fn);
 int model_add_head(Model* m, const std::string& dir, int force_token_level, std::string* err);
 void model_free(Model* m);
 
@@ -212,7 +218,7 @@ int profile_collect(Model& m);
 // All of the following enqueue on m.stream and do NOT synchronise.
 // ids/cu are device pointers (int32); T = cu[B]; max_len = longest sequence.
 int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers);
-// precise.cu: builds the split weights (re-reads <dir>/model.safetensors), the fp32-equivalent forward, buffer release
+// precise.cu: builds the split weights (read_source_projections), the fp32-equivalent forward, buffer release
 int precise_prepare(Model& m, std::string* err);
 int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers);
 void precise_free(Model& m);

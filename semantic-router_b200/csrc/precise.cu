@@ -1,4 +1,4 @@
-// "Precise" encoder path (ModernBERT / mmBERT): fp32-equivalent arithmetic on the same tcgen05 GEMM, for the strict
+// "Precise" encoder path (ModernBERT / mmBERT): fp32-equivalent arithmetic on the same wgmma GEMM, for the strict
 // parity bound BASELINE's north star states ("logits and embeddings within 1e-3 fp32").
 //
 // The production path multiplies fp16 operands (2^-11 relative rounding of every activation and weight, fp16 q / k / v /
@@ -9,7 +9,7 @@
 //   A W^T ~= A_hi W_hi^T + A_lo W_hi^T + A_hi W_lo^T         the dropped A_lo W_lo^T term is 2^-22 relative
 //
 // and runs it as ONE wgmma GEMM of three times the depth: A' = [A_hi | A_lo | A_hi] (K' = 3K), W' = [W_hi | W_hi | W_lo].
-// fp16 x fp16 products are exact in fp32 and the accumulator is the fp32 TMEM one, so the result carries fp32-accumulation
+// fp16 x fp16 products are exact in fp32 and the accumulator is fp32 in registers, so the result carries fp32-accumulation
 // error only.  Everything between the GEMMs is plain fp32 (LayerNorm, RoPE, GeGLU with erff, softmax attention on the CUDA
 // cores with expf): nothing is rounded to fp16 except through the split.  ~5x the time of the production path; selected
 // per model with sr_model_set_precise() -- it exists for parity, not for serving.
@@ -182,32 +182,19 @@ int grow(T*& p, size_t& cap, size_t n) {
 
 }  // namespace
 
-// engine.cu: fp32 host copy of one tensor of <dir>/model.safetensors (shape-checked)
-bool load_host_tensor(const std::string& dir, const std::string& name, const std::vector<int64_t>& shape, std::vector<float>& out,
-                      std::string* err);
-std::string modernbert_prefix(const std::string& dir);
-
 int precise_prepare(Model& m, std::string* err) {
   if (m.cfg.arch != ARCH_MODERNBERT) { *err = "the precise path covers ModernBERT / mmBERT encoders"; return -1; }
   if (!m.precise.layers.empty()) return 0;
   if (cudaSetDevice(m.device) != cudaSuccess) { *err = "cudaSetDevice failed"; return -1; }
-  const int H = m.cfg.H, I = m.cfg.I;
-  const std::string P = modernbert_prefix(m.dir);
   std::vector<PreciseLayer> layers(m.cfg.L);
-  for (int li = 0; li < m.cfg.L; ++li) {
-    const std::string Lp = P + "layers." + std::to_string(li) + ".";
-    std::vector<float> w;
+  const bool ok = read_source_projections(m, err, [&](int li, int p, const std::vector<float>& w, int n, int k) {
     PreciseLayer& pl = layers[li];
-    if (!load_host_tensor(m.dir, Lp + "attn.Wqkv.weight", {3 * H, H}, w, err)) return -1;
-    pl.wqkv = split_weight(m, w, 3 * H, H);
-    if (!load_host_tensor(m.dir, Lp + "attn.Wo.weight", {H, H}, w, err)) return -1;
-    pl.wo = split_weight(m, w, H, H);
-    if (!load_host_tensor(m.dir, Lp + "mlp.Wi.weight", {2 * I, H}, w, err)) return -1;
-    pl.wi = split_weight(m, w, 2 * I, H);
-    if (!load_host_tensor(m.dir, Lp + "mlp.Wo.weight", {H, I}, w, err)) return -1;
-    pl.wo2 = split_weight(m, w, H, I);
-    if (!pl.wqkv || !pl.wo || !pl.wi || !pl.wo2) { *err = "allocation of the split weights failed"; return -1; }
-  }
+    __half** slot[] = {&pl.wqkv, &pl.wo, &pl.wi, &pl.wo2};
+    *slot[p] = split_weight(m, w, n, k);
+    if (!*slot[p]) *err = "allocation of the split weights failed";
+    return *slot[p] != nullptr;
+  });
+  if (!ok) return -1;
   m.precise.layers.swap(layers);
   return 0;
 }
