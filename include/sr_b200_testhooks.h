@@ -77,13 +77,9 @@ typedef struct sr_gemm_desc {
 /* gemm_f16 on the legacy default stream with every descriptor field; EPI_TOPK's list count goes to *topk_lists. */
 SR_API int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists);
 SR_API int sr_test_hl_to_f32(const void* hi_f16, const void* lo_f16, const float* pivot, int t, int hdim, float* x);
-SR_API int sr_test_attention(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int max_len,
-                      int num_heads, int window);
-/* the production attention kernel (wgmma): global-layer entry (any window) and sliding-window entry (window >= 1) */
-SR_API int sr_test_attention_tc(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int total_tokens,
-                                int max_len, int num_heads, int window);
-SR_API int sr_test_attention_win(const void* qkv_f16, void* out_f16, const int32_t* d_cu_seqlens, int batch, int total_tokens,
-                                 int max_len, int num_heads, int window);
+/* attention_wgmma_fwd (csrc/kernels.h: same arguments and meaning; window 0 = global, kv_lens [batch] or null) */
+SR_API int sr_test_attention_wgmma(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int max_len,
+                                   int num_heads, int head_dim, int window, const int32_t* kv_lens);
 SR_API int sr_test_layernorm(const float* x, int t, int h, const float* w, const float* b, float eps, float* y32,
                       void* y16);
 

@@ -135,9 +135,7 @@ def hooks():
         H.sr_test_gemm_resid_hl.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]
         H.sr_test_gemm_desc.argtypes = [C.POINTER(GemmDesc), C.POINTER(C.c_int)]
         H.sr_test_gemm_cluster.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp]
-        H.sr_test_attention.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
-        H.sr_test_attention_tc.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
-        H.sr_test_attention_win.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+        H.sr_test_attention_wgmma.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         H.sr_test_layernorm.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_float, vp, vp]
         H.sr_test_hl_to_f32.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
         ci, cf = C.c_int, C.c_float
@@ -159,8 +157,7 @@ def _attach_hooks(L):
     if not os.path.exists(HOOKS_LIB_PATH):
         return
     H = hooks()
-    for name in ("sr_test_gemm", "sr_test_attention", "sr_test_attention_tc", "sr_test_attention_win",
-                 "sr_test_layernorm", "sr_test_bio_decode", "sr_test_hallucination_spans"):
+    for name in ("sr_test_gemm", "sr_test_layernorm", "sr_test_bio_decode", "sr_test_hallucination_spans"):
         setattr(L, name, getattr(H, name))
 
 

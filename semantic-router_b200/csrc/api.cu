@@ -582,22 +582,10 @@ int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
 int sr_test_hl_to_f32(const void* hi, const void* lo, const float* pivot, int t, int hdim, float* x) {
   return hl_to_f32(nullptr, static_cast<const __half*>(hi), static_cast<const __half*>(lo), pivot, t, hdim, x);
 }
-int sr_test_attention(const void* qkv, void* out, const int32_t* cu, int batch, int max_len, int num_heads, int window) {
-  return attention_fwd(nullptr, static_cast<const __half*>(qkv), static_cast<__half*>(out), cu, batch, max_len,
-                       num_heads, 64, window);
-}
-// the production attention kernel (attention_wgmma.cu) through the two entry shapes the engine uses: global layers
-// (window 0) and sliding-window layers
-int sr_test_attention_tc(const void* qkv, void* out, const int32_t* cu, int batch, int total_tokens, int max_len,
-                         int num_heads, int window) {
-  (void)total_tokens;
+int sr_test_attention_wgmma(const void* qkv, void* out, const int32_t* cu, int batch, int max_len, int num_heads,
+                            int head_dim, int window, const int32_t* kv_lens) {
   return attention_wgmma_fwd(nullptr, static_cast<const __half*>(qkv), static_cast<__half*>(out), cu, batch, max_len,
-                             num_heads, 64, window);
-}
-int sr_test_attention_win(const void* qkv, void* out, const int32_t* cu, int batch, int total_tokens, int max_len,
-                          int num_heads, int window) {
-  if (window <= 0) return -1;   // the sliding-window entry needs a window
-  return sr_test_attention_tc(qkv, out, cu, batch, total_tokens, max_len, num_heads, window);
+                             num_heads, head_dim, window, kv_lens);
 }
 int sr_test_layernorm(const float* x, int t, int hdim, const float* w, const float* b, float eps, float* y32, void* y16) {
   return layernorm_rows(nullptr, x, t, hdim, w, b, eps, y32, static_cast<__half*>(y16));

@@ -1,4 +1,4 @@
-// Host-callable launchers of the HBM-bound kernels (elementwise.cu), attention (attention.cu) and the
+// Host-callable launchers of the HBM-bound kernels (elementwise.cu), attention (attention_wgmma.cu) and the
 // cache scan (cache_scan.cu).  All pointers are device pointers; all launches are asynchronous on `stream`.
 #pragma once
 #include <cuda_fp16.h>
@@ -12,10 +12,6 @@ void note_launch(int n = 1);
 // SRB_PDL=1 turns programmatic dependent launch on for the GEMM kernels (default off)
 bool pdl_enabled();
 long long launches_total();
-
-// ---- attention.cu (mma.sync flash attention: the comparator of attention_wgmma.cu in the tests)
-int attention_fwd(cudaStream_t stream, const __half* qkv, __half* out, const int* cu_seqlens, int batch,
-                  int max_len, int num_heads, int head_dim, int window);
 
 // ---- attention_wgmma.cu (wgmma flash attention, head dim 64, optional sliding window |i - j| <= window; every layer)
 // kv_lens [batch] (optional, global attention only): keys >= kv_lens[b] of sequence b are masked for EVERY query row while
