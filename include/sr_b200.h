@@ -152,7 +152,10 @@ SR_API int sr_cache_size(const sr_cache* c);
 SR_API int sr_cache_dim(const sr_cache* c);
 /* queries float32 host [b, dim]; out_idx int32 [b,k] (global ids, -1 = none), out_score float [b,k].
  * Semantics: pkg/cache/inmemory_cache_search.go:65-89 (k = 1) and ffi/embedding.rs:1640-1681 (top-k):
- * descending score, lower index wins ties. */
+ * descending score, lower index wins ties.  Limits: 1 <= k <= 64, and ceil(size / 8192) * k <= 25600 (the candidates
+ * of the two-stage selection, 200 KB of shared memory per query; the fused route, b > 4 and k <= 8, has no size limit).
+ * Returns -1 outside them, with out_idx / out_score untouched.  sr_cache_topk_dev and sr_cache_topk_packed_dev share
+ * these limits. */
 SR_API int sr_cache_topk(sr_cache* c, const float* queries, int b, int k, int32_t* out_idx, float* out_score);
 /* device-resident variant: d_queries fp16 [b, dim]; results in device buffers owned by the cache, valid until the next
  * scan of this cache.  Asynchronous on `cuda_stream`: growing the scratch and queueing the scan are locked, but callers
@@ -165,7 +168,8 @@ SR_API const int32_t* sr_cache_dev_idx(const sr_cache* c);
  * the g gathered lists are merged on the device with the reference tie rule (descending score, lower global id first;
  * pkg/cache/inmemory_cache_search.go:65-89, ffi/embedding.rs:1640-1681).
  * sr_cache_topk_packed_dev: scan + pack into d_pairs_out [b,k] entries (device memory of the caller, e.g. the send buffer
- * of the collective).  sr_cache_merge_packed_dev: d_pairs_parts [g][b,k] entries -> d_out_idx / d_out_score [b,k]. */
+ * of the collective).  sr_cache_merge_packed_dev: d_pairs_parts [g][b,k] entries -> d_out_idx / d_out_score [b,k];
+ * g * k <= 6144 (every entry of a query in 48 KB of shared memory), -1 with the outputs untouched beyond that. */
 SR_API int sr_cache_topk_packed_dev(sr_cache* c, const void* d_queries_f16, int b, int k, void* d_pairs_out, void* cuda_stream);
 SR_API int sr_cache_merge_packed_dev(int device, const void* d_pairs_parts, int g, int b, int k, int32_t* d_out_idx,
                                      float* d_out_score, void* cuda_stream);

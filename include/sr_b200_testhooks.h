@@ -76,6 +76,11 @@ typedef struct sr_gemm_desc {
 } sr_gemm_desc;
 /* gemm_f16 on the legacy default stream with every descriptor field; EPI_TOPK's list count goes to *topk_lists. */
 SR_API int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists);
+/* The route sr_cache_topk takes for b queries over n stored rows of dimension dim (csrc/kernels.h cache_topk_plan):
+ * route 0 the empty store, 1 the GEMM's fused top-8 epilogue, 2 GEMV scores + two-stage selection, 3 GEMM scores +
+ * two-stage selection; chunks = score chunks of the two-stage routes (0 otherwise); candidates = stage-2 candidates per
+ * query (fused: the upper bound).  Returns -1 (route -1) wherever sr_cache_topk refuses the shape. */
+SR_API int sr_test_cache_plan(int b, int n, int dim, int k, int* route, int* chunks, int* candidates);
 SR_API int sr_test_hl_to_f32(const void* hi_f16, const void* lo_f16, const float* pivot, int t, int hdim, float* x);
 /* attention_wgmma_fwd (csrc/kernels.h: same arguments and meaning; window 0 = global, kv_lens [batch] or null) */
 SR_API int sr_test_attention_wgmma(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int max_len,

@@ -138,6 +138,7 @@ def hooks():
         H.sr_test_attention_wgmma.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         H.sr_test_layernorm.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_float, vp, vp]
         H.sr_test_hl_to_f32.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
+        H.sr_test_cache_plan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
         ci, cf = C.c_int, C.c_float
         H.sr_test_embed_ln_modernbert.argtypes = [vp, ci, ci, ci, vp, vp, cf, vp, vp, vp]
         H.sr_test_embed_ln_bert.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, cf, vp, vp]

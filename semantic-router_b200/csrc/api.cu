@@ -579,6 +579,13 @@ int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
   g.mask_block = d->mask_block; g.mask_rows = d->mask_rows;
   return gemm_f16(nullptr, g);
 }
+int sr_test_cache_plan(int b, int n, int dim, int k, int* route, int* chunks, int* candidates) {
+  const CachePlan p = cache_topk_plan(b, n, dim, k);
+  if (route) *route = p.route;
+  if (chunks) *chunks = p.chunks;
+  if (candidates) *candidates = p.candidates;
+  return p.route == CACHE_REFUSED ? -1 : 0;
+}
 int sr_test_hl_to_f32(const void* hi, const void* lo, const float* pivot, int t, int hdim, float* x) {
   return hl_to_f32(nullptr, static_cast<const __half*>(hi), static_cast<const __half*>(lo), pivot, t, hdim, x);
 }

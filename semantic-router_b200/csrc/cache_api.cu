@@ -36,7 +36,7 @@ int cfail(const char* msg) {
 // Grows the per-cache scratch.  Caller holds c->mu.  Buffers may still be referenced by work queued on the cache's
 // stream or on a caller's stream (sr_cache_topk_dev), so everything on the device drains before anything is freed.
 int ensure(sr_cache* c, int b, int k) {
-  const size_t need = cache_topk_workspace_bytes(b, c->size > 0 ? c->size : 1, k);
+  const size_t need = cache_topk_workspace_bytes(b, c->size > 0 ? c->size : 1, c->dim, k);
   if (b > c->q_cap || b * k > c->res_cap || need > c->ws_bytes) cudaDeviceSynchronize();
   if (b > c->q_cap) {
     if (c->d_q) cudaFree(c->d_q);

@@ -27,6 +27,10 @@ struct Cand {
   float v;
   int i;
 };
+// A launch gets 48 KB of shared memory without opting in, the kernel's static shared memory included: select_stage2 and
+// merge_packed_kernel hold one Cand per warp for block_argmax besides their dynamic candidate arrays.
+constexpr size_t kDefaultSmem = 48 * 1024;
+constexpr size_t kSelStaticSmem = sizeof(Cand) * (kSelThreads / 32);
 __device__ __forceinline__ bool better(float v, int i, float bv, int bi) {
   // larger score wins; equal score: lower (non-negative) index wins; index -1 = nothing
   if (i < 0) return false;
@@ -233,36 +237,6 @@ select_stage2(const int* __restrict__ cand_idx, const float* __restrict__ cand_s
   }
 }
 
-// merge of G per-shard lists holding GLOBAL ids
-__global__ void __launch_bounds__(kSelThreads)
-merge_kernel(const int* __restrict__ idx_parts, const float* __restrict__ score_parts, int G, int B, int k,
-             int* __restrict__ out_idx, float* __restrict__ out_score) {
-  __shared__ Cand red[kSelThreads / 32];
-  extern __shared__ uint8_t dyn[];
-  float* sv = reinterpret_cast<float*>(dyn);
-  int* si = reinterpret_cast<int*>(sv + G * k);
-  const int q = blockIdx.x;
-  for (int c = threadIdx.x; c < G * k; c += kSelThreads) {
-    const int g = c / k, j = c % k;
-    sv[c] = score_parts[(static_cast<size_t>(g) * B + q) * k + j];
-    si[c] = idx_parts[(static_cast<size_t>(g) * B + q) * k + j];
-  }
-  __syncthreads();
-  for (int r = 0; r < k; ++r) {
-    Cand c{-INFINITY, -1};
-    int where = -1;
-    for (int j = threadIdx.x; j < G * k; j += kSelThreads)
-      if (better(sv[j], si[j], c.v, c.i)) { c.v = sv[j]; c.i = si[j]; where = j; }
-    const Cand b = block_argmax(c, red);
-    if (where >= 0 && c.i == b.i && b.i >= 0) si[where] = -1;
-    if (threadIdx.x == 0) {
-      out_idx[static_cast<size_t>(q) * k + r] = b.i;
-      out_score[static_cast<size_t>(q) * k + r] = b.i >= 0 ? b.v : -INFINITY;
-    }
-    __syncthreads();
-  }
-}
-
 // Exchange format of a sharded cache (SURVEY 8e): one 8-byte entry per (query, rank) = {fp32 score, int32 GLOBAL id}.
 // Each rank packs its [B,k] result into this form, ONE all-gather moves B * k * 8 bytes per rank, and the merge below
 // reads the G gathered lists directly.
@@ -315,38 +289,57 @@ inline int chunk_rows(int B, int N) {
 
 constexpr int kFusedK = 8;        // list length of the GEMM's top-k epilogue (gemm.h EPI_TOPK)
 constexpr int kFusedLists = 320;  // upper bound of the lists per query (= 2 x CTAs launched <= 2 x SMs)
-inline bool fused_ok(int B, int k, int D) { return B > 4 && k <= kFusedK && D % 8 == 0; }
+constexpr int kMaxK = 64;         // stage 1 keeps 64 entries per warp (wv / wi)
+constexpr size_t kStage2SmemMax = 200 * 1024;   // stage 2 holds every candidate of its query in shared memory
 
-size_t cache_topk_workspace_bytes(int B, int N, int k) {
-  const int chunk = chunk_rows(B, N);
-  const size_t segs = (static_cast<size_t>(N) + kSegment - 1) / kSegment;
-  const size_t two_pass = align_up(static_cast<size_t>(B) * chunk * 4, 256) + 2 * align_up(static_cast<size_t>(B) * segs * k * 4, 256);
-  const size_t fused = 2 * align_up(static_cast<size_t>(B) * kFusedLists * kFusedK * 4, 256);
-  return two_pass > fused ? two_pass : fused;
+CachePlan cache_topk_plan(int B, int N, int D, int k) {
+  CachePlan p;
+  if (B <= 0 || k <= 0 || k > kMaxK || N < 0) return p;
+  if (N == 0) {
+    p.route = CACHE_EMPTY;
+    return p;
+  }
+  if (B > 4 && k <= kFusedK && D % 8 == 0) {
+    p.route = CACHE_FUSED;
+    p.candidates = kFusedLists * kFusedK;
+    p.workspace_bytes = 2 * align_up(static_cast<size_t>(B) * kFusedLists * kFusedK * 4, 256);
+    return p;
+  }
+  p.chunk_rows = chunk_rows(B, N);
+  p.chunks = (N + p.chunk_rows - 1) / p.chunk_rows;
+  p.segments = (N + kSegment - 1) / kSegment;
+  p.candidates = p.segments * k;
+  p.stage2_smem = static_cast<size_t>(p.candidates) * 8;
+  if (p.stage2_smem > kStage2SmemMax) return p;
+  p.route = (B <= 4 && D % 8 == 0 && static_cast<size_t>(B) * D * 4 <= 48 * 1024) ? CACHE_GEMV : CACHE_GEMM;
+  p.workspace_bytes = align_up(static_cast<size_t>(B) * p.chunk_rows * 4, 256) +
+                      2 * align_up(static_cast<size_t>(B) * p.candidates * 4, 256);
+  return p;
 }
+
+size_t cache_topk_workspace_bytes(int B, int N, int D, int k) { return cache_topk_plan(B, N, D, k).workspace_bytes; }
 
 int cache_topk(cudaStream_t stream, const __half* queries, int B, const __half* cache, const uint8_t* valid, int N,
                int D, int k, int id_offset, int* out_idx, float* out_score, void* workspace, size_t workspace_bytes) {
   if (B <= 0 || k <= 0) return 0;
-  if (k > 64) { fprintf(stderr, "[srb200] cache_topk: k=%d unsupported (<= 64)\n", k); return -1; }
-  if (workspace_bytes < cache_topk_workspace_bytes(B, N, k)) {
+  const CachePlan plan = cache_topk_plan(B, N, D, k);
+  if (plan.route == CACHE_REFUSED) {
+    fprintf(stderr, "[srb200] cache_topk: k=%d over %d rows unsupported (k <= %d, ceil(rows / %d) * k <= %d)\n", k, N,
+            kMaxK, kSegment, static_cast<int>(kStage2SmemMax / 8));
+    return -1;
+  }
+  if (workspace_bytes < plan.workspace_bytes) {
     fprintf(stderr, "[srb200] cache_topk: workspace too small\n");
     return -1;
   }
-  const int chunk = chunk_rows(B, N);
-  const int segs = (N + kSegment - 1) / kSegment;
   uint8_t* ws = static_cast<uint8_t*>(workspace);
-  float* scores = reinterpret_cast<float*>(ws);
-  int* cand_idx = reinterpret_cast<int*>(ws + align_up(static_cast<size_t>(B) * chunk * 4, 256));
-  float* cand_score = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(cand_idx) +
-                                               align_up(static_cast<size_t>(B) * segs * k * 4, 256));
-  if (N == 0) {
-    select_stage2<<<B, kSelThreads, 0, stream>>>(cand_idx, cand_score, 0, k, id_offset, out_idx, out_score);
+  if (plan.route == CACHE_EMPTY) {
+    select_stage2<<<B, kSelThreads, 0, stream>>>(nullptr, nullptr, 0, k, id_offset, out_idx, out_score);
     SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
+    note_launch();
     return 0;
   }
-  if (fused_ok(B, k, D)) {
+  if (plan.route == CACHE_FUSED) {
     // Scores never leave the SM: the GEMM's epilogue keeps a running top-8 per (query, CTA) and only those short lists
     // are written (B x <= 148 x 8 pairs); no 1 GiB score chunks, no selection pass over them.
     int* l_idx = reinterpret_cast<int*>(ws);
@@ -365,10 +358,15 @@ int cache_topk(cudaStream_t stream, const __half* queries, int B, const __half* 
     note_launch();
     return 0;
   }
+  const int chunk = plan.chunk_rows, segs = plan.segments;
+  float* scores = reinterpret_cast<float*>(ws);
+  int* cand_idx = reinterpret_cast<int*>(ws + align_up(static_cast<size_t>(B) * chunk * 4, 256));
+  float* cand_score = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(cand_idx) +
+                                               align_up(static_cast<size_t>(B) * plan.candidates * 4, 256));
   for (int row0 = 0; row0 < N; row0 += chunk) {
     const int n = (N - row0) < chunk ? (N - row0) : chunk;
     const int n_pad = static_cast<int>(align_up(n, 64));  // cache allocation is padded to 256 rows
-    if (B <= 4 && D % 8 == 0 && static_cast<size_t>(B) * D * 4 <= 48 * 1024) {
+    if (plan.route == CACHE_GEMV) {
       static int num_sms = 0;
       if (!num_sms) {
         int dev = 0;
@@ -398,22 +396,10 @@ int cache_topk(cudaStream_t stream, const __half* queries, int B, const __half* 
     SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   }
-  const int ncand = segs * k;
-  const size_t smem = static_cast<size_t>(ncand) * 8;
-  if (smem > 200 * 1024) { fprintf(stderr, "[srb200] cache_topk: too many candidates (%d)\n", ncand); return -1; }
-  if (smem > 48 * 1024)
+  const size_t smem = plan.stage2_smem;
+  if (smem + kSelStaticSmem > kDefaultSmem)
     SRB_CUDA_CHECK(cudaFuncSetAttribute(select_stage2, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  select_stage2<<<B, kSelThreads, smem, stream>>>(cand_idx, cand_score, ncand, k, id_offset, out_idx, out_score);
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
-  return 0;
-}
-
-int cache_merge_topk(cudaStream_t stream, const int* idx_parts, const float* score_parts, int G, int B, int k,
-                     int* out_idx, float* out_score) {
-  if (B <= 0) return 0;
-  merge_kernel<<<B, kSelThreads, static_cast<size_t>(G) * k * 8, stream>>>(idx_parts, score_parts, G, B, k, out_idx,
-                                                                          out_score);
+  select_stage2<<<B, kSelThreads, smem, stream>>>(cand_idx, cand_score, plan.candidates, k, id_offset, out_idx, out_score);
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   return 0;
@@ -430,7 +416,9 @@ int cache_pack_pairs(cudaStream_t stream, const int* idx, const float* score, in
 int cache_merge_packed(cudaStream_t stream, const void* pairs, int G, int B, int k, int* out_idx, float* out_score) {
   if (B <= 0) return 0;
   const size_t smem = static_cast<size_t>(G) * k * 8;
-  if (smem > 48 * 1024) { fprintf(stderr, "[srb200] cache_merge_packed: G * k = %d too large\n", G * k); return -1; }
+  if (smem > kDefaultSmem) { fprintf(stderr, "[srb200] cache_merge_packed: G * k = %d too large\n", G * k); return -1; }
+  if (smem + kSelStaticSmem > kDefaultSmem)
+    SRB_CUDA_CHECK(cudaFuncSetAttribute(merge_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   merge_packed_kernel<<<B, kSelThreads, smem, stream>>>(static_cast<const int2*>(pairs), G, B, k, out_idx, out_score);
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();

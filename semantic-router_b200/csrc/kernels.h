@@ -77,20 +77,32 @@ int token_head(cudaStream_t stream, const float* hidden32, const __half* dense16
                int gelu_erf = 0, float head_eps = 1e-12f);
 
 // ---- cache_scan.cu
+// The route cache_topk takes for (B queries, N stored rows, dimension D, k): the empty store; the GEMM's fused top-8
+// epilogue (B > 4, k <= 8); or scores in chunks of at most 1 GiB followed by the two-stage selection, the scores coming
+// from a GEMV (B <= 4 and B * D * 4 <= 48 KB) or from the GEMM.  Refused (route CACHE_REFUSED): B or k <= 0, k > 64,
+// or more than 200 KB of stage-2 candidates (ceil(N / 8192) * k > 25600).
+enum CacheRoute { CACHE_REFUSED = -1, CACHE_EMPTY = 0, CACHE_FUSED = 1, CACHE_GEMV = 2, CACHE_GEMM = 3 };
+struct CachePlan {
+  int route = CACHE_REFUSED;
+  int chunk_rows = 0;          // two-pass: stored rows per score chunk, a multiple of the 8192-row stage-1 segment
+  int chunks = 0;              // two-pass: score chunks (one score GEMV / GEMM and one stage-1 launch each)
+  int segments = 0;            // two-pass: stage-1 segments over the whole store, ceil(N / 8192)
+  int candidates = 0;          // stage-2 candidates per query (fused: the upper bound, 8 per list)
+  size_t stage2_smem = 0;      // two-pass: dynamic shared memory of stage 2, candidates x 8 bytes
+  size_t workspace_bytes = 0;  // what cache_topk needs for this route
+};
+CachePlan cache_topk_plan(int B, int N, int D, int k);
 // scores = Q[B,D] . C[N,D]^T (fp16 operands, fp32 accumulate); per query top-k (descending score, lower
 // index wins ties); rows with valid[i]==0 are skipped.  out_idx int32 [B,k] (global id = row + id_offset,
-// -1 when fewer than k valid rows), out_score fp32 [B,k].
+// -1 when fewer than k valid rows), out_score fp32 [B,k].  Returns -1 where cache_topk_plan refuses.
 int cache_topk(cudaStream_t stream, const __half* queries, int B, const __half* cache, const uint8_t* valid,
                int N, int D, int k, int id_offset, int* out_idx, float* out_score, void* workspace,
                size_t workspace_bytes);
-size_t cache_topk_workspace_bytes(int B, int N, int k);
-// k-way merge of G per-shard lists [G][B,k] -> [B,k]
-int cache_merge_topk(cudaStream_t stream, const int* idx_parts, const float* score_parts, int G, int B, int k,
-                     int* out_idx, float* out_score);
+size_t cache_topk_workspace_bytes(int B, int N, int D, int k);
 
 // sharded-cache exchange format: 8-byte entries {fp32 score, int32 global id}
 int cache_pack_pairs(cudaStream_t stream, const int* idx, const float* score, int n, void* pairs_out);
-// merge of G gathered lists in that format, pairs [G][B][k] -> [B,k]
+// merge of G gathered lists in that format, pairs [G][B][k] -> [B,k]; refused (-1) for G * k > 6144
 int cache_merge_packed(cudaStream_t stream, const void* pairs, int G, int B, int k, int* out_idx, float* out_score);
 
 }  // namespace srb
