@@ -87,18 +87,13 @@ SR_API int sr_classify_multi_ids(sr_model* m, const int* heads, int n_heads, con
  * model_architectures/lora/lora_adapter.rs:136-144) and its stated direction is one shared encoder for the intent / PII /
  * security tasks (src/semantic-router/pkg/classification/unified_classifier.go:113).  task_dirs[t] is a complete checkpoint
  * of task t: the SAME base tensors in every directory (checked bit for bit), `X.lora_A.weight` / `X.lora_B.weight` next to
- * the adapted `X.weight`s, its own classifier head, lora_config.json {"rank", "alpha"}.  ONE copy of the base is loaded;
- * a batch then runs ONCE through the encoder as n_tasks copies of its rows, every copy with its own task's rank-r term added
- * inside the projection GEMMs' accumulators (a K extension of the wgmma mainloop), instead of n_tasks forwards over
- * n_tasks merged models.  token_level[t]: 1 token head, 0 sequence head, -1 from config.json.
- * mode SR_LORA_LOWRANK: as described (one copy of the base: the memory form).  mode SR_LORA_GROUPED: every task's adapters are
- * folded into its own copy of the projection weights at load, the copies are stacked, and each 256-row block of a projection
- * GEMM picks its task's matrix in the TMA producer -- still ONE pass over n_tasks copies of the rows, no rank-r GEMMs and no
- * extra k-blocks, the arithmetic of n_tasks separately loaded models (the latency / throughput form). */
-enum { SR_LORA_LOWRANK = 0, SR_LORA_GROUPED = 1 };
-SR_API int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_level, int n_tasks, int mode, int device,
+ * the adapted `X.weight`s, its own classifier head, lora_config.json {"rank", "alpha"}.  Every task's adapters are folded
+ * into its own copy of the projection weights at load and the copies are stacked.  A batch then runs ONCE through the
+ * encoder as n_tasks copies of its rows, and each 256-row block of a projection GEMM picks its task's matrix in the TMA
+ * producer, instead of n_tasks forwards over n_tasks merged models: the arithmetic of n_tasks separately loaded models.
+ * token_level[t]: 1 token head, 0 sequence head, -1 from config.json. */
+SR_API int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_level, int n_tasks, int device,
                                      sr_model** out);
-SR_API int sr_lora_shared_mode(const sr_model* m);    /* SR_LORA_LOWRANK / SR_LORA_GROUPED, -1 for an ordinary model */
 SR_API int sr_lora_shared_tasks(const sr_model* m);   /* 0 for an ordinary model */
 /* 1: <model_dir>/model.safetensors carries lora_A / lora_B tensors, 0: it does not (a merged checkpoint), -1: unreadable */
 SR_API int sr_checkpoint_has_adapters(const char* model_dir);

@@ -68,11 +68,7 @@ typedef struct sr_gemm_desc {
   const float* fold_stats;
   float fold_eps;
   int fold_h;
-  const void* a2;
-  const void* w2;
-  int k2;
   int w_groups, w_group_rows;
-  int mask_block, mask_rows;
 } sr_gemm_desc;
 /* gemm_f16 on the legacy default stream with every descriptor field; EPI_TOPK's list count goes to *topk_lists. */
 SR_API int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists);

@@ -2,7 +2,7 @@
 
 The fp16 operands are exact in float64, so `value` is the epilogue of gemm.h applied to the exact product.  A kernel
 result x is correct when |x - value| <= TAU * coef + eps, where
-  * coef carries the accumulation error: TAU * S with S = sum_k |a_k w_k| (K extension included) per accumulator,
+  * coef carries the accumulation error: TAU * S with S = sum_k |a_k w_k| per accumulator,
     propagated through the epilogue (RoPE: |cos| S1 + |sin| S2; GELU / GeGLU: through the derivative; LayerNorm fold:
     times rstd);
   * eps is the epilogue's own error: fp32 rounding of its adds and products, the polynomial erf of the GELU epilogues,
@@ -78,8 +78,8 @@ def fold_rstd(stats: torch.Tensor, m: int, eps: float, h: int):
     return rstd, rel
 
 
-def accumulate(a, w, n, a2=None, w2=None, w_groups=0, w_group_rows=0):
-    """acc = A W^T (+ A2 W2^T) and S = |A| |W|^T (+ |A2| |W2|^T), float64; grouped weights: row r of A multiplies
+def accumulate(a, w, n, w_groups=0, w_group_rows=0):
+    """acc = A W^T and S = |A| |W|^T, float64; grouped weights: row r of A multiplies
     matrix r // w_group_rows of the stack W [w_groups * n, K]."""
     a, w = a.double(), w.double()
     m = a.shape[0]
@@ -96,33 +96,24 @@ def accumulate(a, w, n, a2=None, w2=None, w_groups=0, w_group_rows=0):
     else:
         acc = a @ w[:n].t()
         s = a.abs() @ w[:n].abs().t()
-    if a2 is not None:
-        a2, w2 = a2.double(), w2.double()
-        acc = acc + a2 @ w2.t()
-        s = s + a2.abs() @ w2.abs().t()
     return acc, s
 
 
 def gemm(epi: int, a: torch.Tensor, w: torch.Tensor, n: Optional[int] = None, *, bias=None, resid=None, pos=None,
          rope_cos=None, rope_sin=None, rope_cols: int = 0, fold_stats=None, fold_eps: float = 0.0, fold_h: int = 0,
-         a2=None, w2=None, w_groups: int = 0, w_group_rows: int = 0, mask_block: int = 0, mask_rows: int = 0) -> Ref:
+         w_groups: int = 0, w_group_rows: int = 0) -> Ref:
     """Reference of gemm_f16 for a = A [M, K] (only the M rows the GEMM computes), w = W [N, K] (grouped: the stack),
     n = N.  EPI_RESID / EPI_RESID_HL: resid = the stream before the GEMM (the fp16 pair as hi + lo), or None.
     EPI_GEGLU: w rows interleaved in 32-row (a | b) groups; the result is [M, N / 2]."""
     n = w.shape[0] if n is None else n
     m = a.shape[0]
-    acc, s = accumulate(a, w, n, a2, w2, w_groups, w_group_rows)
+    acc, s = accumulate(a, w, n, w_groups, w_group_rows)
     b = bias.double()[:n] if bias is not None else torch.zeros(n, dtype=torch.float64, device=acc.device)
     zero = torch.zeros_like(acc)
     if epi == EPI_F16:
         v = acc + b
-        coef = s.clone()
         eps = 2 * U32 * (b.abs() + v.abs()) + ulp16(v)
-        if mask_block > 0:
-            own = (torch.arange(m, device=v.device) // mask_rows)[:, None]
-            keep = (torch.arange(n, device=v.device) // mask_block)[None, :] == own
-            v, coef, eps = torch.where(keep, v, zero), torch.where(keep, coef, zero), torch.where(keep, eps, zero)
-        return Ref(v, coef, eps)
+        return Ref(v, s, eps)
     if epi in (EPI_RESID, EPI_RESID_HL):
         r = resid.double()[:m, :n] if resid is not None else zero
         v = r + acc + b

@@ -48,8 +48,7 @@ def load_library(path: Optional[str] = None):
     L.sr_embed_ids.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp]
     L.sr_embed_ids_padded.argtypes = [vp, vp, vp, vp, C.c_int, vp]
     L.sr_classify_multi_ids.argtypes = [vp, vp, C.c_int, vp, vp, C.c_int, vp, vp]
-    L.sr_model_load_lora_shared.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
-    L.sr_lora_shared_mode.argtypes = [vp]
+    L.sr_model_load_lora_shared.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(vp)]
     L.sr_lora_shared_tasks.argtypes = [vp]
     L.sr_checkpoint_has_adapters.argtypes = [C.c_char_p]
     L.sr_classify_lora_shared_ids.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp]
@@ -105,8 +104,8 @@ class GemmDesc(C.Structure):
         ("rope_cos", C.c_void_p), ("rope_sin", C.c_void_p), ("rope_cols", C.c_int), ("topk_idx", C.c_void_p),
         ("topk_score", C.c_void_p), ("topk_valid", C.c_void_p), ("topk_n", C.c_int), ("row_stats", C.c_void_p),
         ("reserved", C.c_void_p), ("lo16", C.c_void_p), ("pivot_out", C.c_void_p), ("pivot_in", C.c_void_p),
-        ("pivot_in_stats", C.c_void_p), ("fold_stats", C.c_void_p), ("fold_eps", C.c_float), ("fold_h", C.c_int), ("a2", C.c_void_p),
-        ("w2", C.c_void_p), ("k2", C.c_int)] + [(n, C.c_int) for n in ("w_groups", "w_group_rows", "mask_block", "mask_rows")]
+        ("pivot_in_stats", C.c_void_p), ("fold_stats", C.c_void_p), ("fold_eps", C.c_float), ("fold_h", C.c_int),
+        ("w_groups", C.c_int), ("w_group_rows", C.c_int)]
 
 
 def run_gemm(**fields):
@@ -295,15 +294,13 @@ class Model:
 
 class LoraSharedModel(Model):
     """ONE base encoder + the unmerged LoRA adapters and heads of several task checkpoints over it (sr_b200.h:
-    sr_model_load_lora_shared); a batch runs once, every task's rows with its own rank-r terms."""
+    sr_model_load_lora_shared); a batch runs once, every task's copy of the rows with that task's merged weights."""
 
-    LOWRANK, GROUPED = 0, 1
-
-    def __init__(self, task_dirs: Sequence[str], token_level: Sequence[int], device: int = 0, mode: int = 0):
+    def __init__(self, task_dirs: Sequence[str], token_level: Sequence[int], device: int = 0):
         self._h = C.c_void_p()
         dirs = (C.c_char_p * len(task_dirs))(*[d.encode() for d in task_dirs])
         tl = np.asarray(token_level, dtype=np.int32)
-        if lib().sr_model_load_lora_shared(dirs, _p(tl), len(task_dirs), mode, device, C.byref(self._h)) != 0:
+        if lib().sr_model_load_lora_shared(dirs, _p(tl), len(task_dirs), device, C.byref(self._h)) != 0:
             raise _err("sr_model_load_lora_shared")
         info = ModelInfo()
         lib().sr_model_info(self._h, C.byref(info))

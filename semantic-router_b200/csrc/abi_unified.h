@@ -9,8 +9,7 @@ namespace {
 Slot g_lora_intent, g_lora_pii, g_lora_security;
 // The three LoRA tasks as ONE shared-base model when their checkpoints are unmerged adapters over one base (sr_b200.h:
 // sr_model_load_lora_shared): a batch then runs once through the encoder instead of three times.  SR_B200_LORA_SHARED=0
-// keeps the three slots, =lowrank serves from ONE copy of the base with rank-r terms in the GEMMs (the memory form), the
-// default (=1 / =grouped) from the tasks' merged matrices stacked and picked per row block (the fast form).
+// keeps the three slots.
 Slot g_lora_shared;
 std::map<int, std::string> g_lora_labels[3];
 Slot g_unified;  // shared encoder + 3 heads (legacy unified classifier)
@@ -35,14 +34,13 @@ bool init_lora_unified_classifier(const char* intent, const char* pii, const cha
   if (!intent || !pii || !security) return false;
   if (g_lora_shared.ready()) return true;
   static const bool shared_on = [] { const char* e = getenv("SR_B200_LORA_SHARED"); return !(e && e[0] == '0'); }();
-  static const int shared_mode = [] { const char* e = getenv("SR_B200_LORA_SHARED"); return (e && e[0] == 'l') ? SR_LORA_LOWRANK : SR_LORA_GROUPED; }();
   const bool fresh = !g_lora_intent.ready() && !g_lora_pii.ready() && !g_lora_security.ready();
   if (shared_on && fresh && sr_checkpoint_has_adapters(intent) == 1 && sr_checkpoint_has_adapters(pii) == 1 &&
       sr_checkpoint_has_adapters(security) == 1) {
     const char* dirs[3] = {intent, pii, security};
     const int token_level[3] = {0, 1, 0};
     const bool ok = slot_init(g_lora_shared, intent, -2, true,
-                              [&](int device, sr_model** out) { return sr_model_load_lora_shared(dirs, token_level, 3, shared_mode, device, out); });
+                              [&](int device, sr_model** out) { return sr_model_load_lora_shared(dirs, token_level, 3, device, out); });
     if (ok) {
       if (SRB_ABI_HEAD_FLAVOR != 0)
         for (auto& rep : g_lora_shared.reps) sr_model_set_head_flavor(rep->model, SRB_ABI_HEAD_FLAVOR);

@@ -376,8 +376,8 @@ int sr_classify_multi_ids(sr_model* h, const int* heads, int n_heads, const int3
 }
 
 // ---- shared-base multi-task pass over unmerged LoRA checkpoints (engine.h: LoraShared) --------------------------------
-int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_level, int n_tasks, int mode, int device, sr_model** out) {
-  if (!task_dirs || n_tasks <= 0 || n_tasks > 8 || !out || mode < 0 || mode > 1) return fail("bad arguments");
+int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_level, int n_tasks, int device, sr_model** out) {
+  if (!task_dirs || n_tasks <= 0 || n_tasks > 8 || !out) return fail("bad arguments");
   std::vector<std::string> dirs;
   std::vector<int> tl;
   for (int t = 0; t < n_tasks; ++t) {
@@ -386,7 +386,7 @@ int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_lev
     tl.push_back(token_level ? token_level[t] : -1);
   }
   std::string err;
-  Model* m = model_load_lora_shared(dirs, tl, device, mode == SR_LORA_GROUPED, &err);
+  Model* m = model_load_lora_shared(dirs, tl, device, &err);
   if (!m) return fail("sr_model_load_lora_shared: " + err);
   sr_model* h = new sr_model();
   h->m = m;
@@ -398,7 +398,6 @@ int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_lev
 int sr_checkpoint_has_adapters(const char* model_dir) { return model_dir ? checkpoint_has_adapters(model_dir) : -1; }
 
 int sr_lora_shared_tasks(const sr_model* h) { return h ? h->m->lora.tasks : -1; }
-int sr_lora_shared_mode(const sr_model* h) { return h && h->m->lora.tasks > 0 ? (h->m->lora.grouped ? SR_LORA_GROUPED : SR_LORA_LOWRANK) : -1; }
 
 int sr_classify_lora_shared_ids(sr_model* h, const int32_t* ids, const int32_t* cu, int batch, int pooler_mode,
                                 float** probs_out, int32_t** cls_out, float** conf_out) {
@@ -412,11 +411,10 @@ int sr_classify_lora_shared_ids(sr_model* h, const int32_t* ids, const int32_t* 
   if (m.precise.on) return fail("the precise path serves merged weights only");
   const int T1 = cu[batch];
   if (T1 <= 0 || static_cast<long long>(T1) * nt > (1ll << 30)) return fail("bad arguments");
-  // the batch once per task, task-major: rows [t * T1p, t * T1p + T1) run with task t's adapters.  The grouped form pads every
-  // copy to whole 256-row GEMM blocks (a block multiplies ONE task's matrices); the pad rows form one extra sequence per copy
-  // that runs through the encoder and is read by nobody.
-  const bool grouped = m.lora.grouped;
-  const int T1p = grouped ? (T1 + 255) / 256 * 256 : T1;
+  // the batch once per task, task-major: rows [t * T1p, t * T1p + T1) run with task t's adapters.  Every copy is padded to
+  // whole 256-row GEMM blocks (a block multiplies ONE task's matrices); the pad rows form one extra sequence per copy that
+  // runs through the encoder and is read by nobody.
+  const int T1p = (T1 + 255) / 256 * 256;
   const int pad = T1p - T1;
   const int Bp = batch + (pad > 0 ? 1 : 0);
   std::vector<int32_t> rids(static_cast<size_t>(T1p) * nt, 0), rcu(static_cast<size_t>(Bp) * nt + 1);
@@ -574,9 +572,7 @@ int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
   g.row_stats = d->row_stats; g.lo16 = d->lo16;
   g.pivot_out = d->pivot_out; g.pivot_in = d->pivot_in; g.pivot_in_stats = d->pivot_in_stats;
   g.fold_stats = d->fold_stats; g.fold_eps = d->fold_eps; g.fold_h = d->fold_h;
-  g.A2 = d->a2; g.W2 = d->w2; g.K2 = d->k2;
   g.w_groups = d->w_groups; g.w_group_rows = d->w_group_rows;
-  g.mask_block = d->mask_block; g.mask_rows = d->mask_rows;
   return gemm_f16(nullptr, g);
 }
 int sr_test_cache_plan(int b, int n, int dim, int k, int* route, int* chunks, int* candidates) {

@@ -368,7 +368,7 @@ Projection projection(std::vector<Segment> segs, int N, int K) {
   return p;
 }
 
-// The four projections of layer li in the order qkv, attention output, intermediate, output (LoraLayer, PreciseLayer).
+// The four projections of layer li in the order qkv, attention output, intermediate, output (PreciseLayer).
 std::array<Projection, 4> layer_projections(const EncoderConfig& c, const std::string& P, int li, bool has_attn_norm) {
   const int H = c.H, I = c.I;
   const std::string Lp = layer_prefix(c, P, li);
@@ -480,8 +480,8 @@ __half* upload_weight(Loader& ld, const std::vector<float>& w, const std::string
   return ld.host_f32(gamma, g, {K}) ? fold_weights(ld, w, g, rows, K) : nullptr;
 }
 
-// Device form of projection p of a layer: uploads `w` (T stacked device weights in the grouped form) into the plain or the
-// folded slot
+// Device form of projection p of a layer: uploads `w` (T stacked device weights for a shared-LoRA model) into the plain or
+// the folded slot
 void store_projection(Loader& ld, const Projection& pr, int p, const std::vector<float>& w, int copies, LayerWeights& lw) {
   __half** plain[] = {&lw.wqkv, &lw.wo, &lw.wi, &lw.wo2};
   __half** slot = pr.gamma.empty() ? plain[p] : (p == 0 ? &lw.wqkv_f : &lw.wi_f);
@@ -687,55 +687,10 @@ namespace {
 bool is_head_tensor(const std::string& n) {
   return n.compare(0, 11, "classifier.") == 0 || n.compare(0, 5, "head.") == 0 || n.find("pooler.") != std::string::npos;
 }
-// Stacks the adapters of every task for projection `pr` (engine.h: LoraProj): `b` rows land where pr.row_of puts the base
-// rows, and `a` gets a fold form when pr.gamma names one.  Padded-head encoders (pr.col_of) are refused before this.
-// Returns false on a malformed adapter; leaves lp empty when no task adapts the projection.
-bool build_lora_proj(Loader& ld, const std::vector<std::unique_ptr<SafeTensors>>& sts, const std::vector<double>& alpha,
-                     const Projection& pr, int rp, LoraProj& lp) {
-  const std::vector<Segment>& segs = pr.segs;
-  const int T = static_cast<int>(sts.size());
-  const int N = pr.dN, K = pr.K;
-  const int nseg = static_cast<int>(segs.size());
-  const int block = nseg * rp;
-  const int R = (T * block + 63) / 64 * 64;
-  std::vector<float> a(static_cast<size_t>(R) * K, 0.f), b(static_cast<size_t>(N) * R, 0.f);
-  bool any = false;
-  for (int t = 0; t < T; ++t)
-    for (int sg = 0; sg < nseg; ++sg) {
-      const StTensor* ta = sts[t]->find(segs[sg].stem + ".lora_A.weight");
-      const StTensor* tb = sts[t]->find(segs[sg].stem + ".lora_B.weight");
-      if (!ta && !tb) continue;
-      if (!ta || !tb || ta->shape.size() != 2 || tb->shape.size() != 2 || ta->shape[1] != K || tb->shape[0] != segs[sg].rows ||
-          ta->shape[0] != tb->shape[1] || ta->shape[0] > rp) {
-        ld.fail("LoRA adapter of " + segs[sg].stem + " (task " + std::to_string(t) + ") does not fit the base weight");
-        return false;
-      }
-      const int r = static_cast<int>(ta->shape[0]);
-      std::vector<float> av, bv;
-      if (!to_f32(*ta, av) || !to_f32(*tb, bv)) { ld.fail("LoRA adapter of " + segs[sg].stem + " has an unsupported dtype"); return false; }
-      const double scaling = alpha[t] / static_cast<double>(r);   // lora_adapter.rs:117
-      const int c0 = t * block + sg * rp;
-      for (int j = 0; j < r; ++j) memcpy(&a[static_cast<size_t>(c0 + j) * K], &av[static_cast<size_t>(j) * K], sizeof(float) * K);
-      for (int n = 0; n < segs[sg].rows; ++n) {
-        const int src = segs[sg].row0 + n;
-        const int dst = pr.row_of.empty() ? src : pr.row_of[src];
-        for (int j = 0; j < r; ++j)
-          b[static_cast<size_t>(dst) * R + c0 + j] = static_cast<float>(scaling * static_cast<double>(bv[static_cast<size_t>(n) * r + j]));
-      }
-      any = true;
-    }
-  if (!any) return true;
-  lp.a = ld.up_f16(a);
-  lp.b = ld.up_f16(b);
-  if (!pr.gamma.empty()) lp.a_f = upload_weight(ld, a, pr.gamma, R, K);
-  lp.R = R;
-  lp.block = block;
-  return ld.ok;
-}
 }  // namespace
 
 Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
-                              bool grouped, std::string* err) {
+                              std::string* err) {
   const int T = static_cast<int>(dirs.size());
   if (T < 1 || token_level.size() != dirs.size()) { *err = "bad arguments"; return nullptr; }
   std::vector<std::unique_ptr<SafeTensors>> sts;
@@ -769,21 +724,12 @@ Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::v
   const EncoderConfig& c = m->cfg;
   if (c.attn_w != c.H) { *err = "shared-LoRA serving is not available for padded-head (MiniLM) encoders"; model_free(m); return nullptr; }
   Loader ld{m, sts[0].get()};
-  const int rp = (max_rank + 7) / 8 * 8;
-  m->lora.layers.resize(c.L);
   std::string P;
   tensor_prefix(*sts[0], c.arch, P);
-  if (grouped) m->lora.glayers = m->layers;   // norms / biases are the base's (adapters touch projection weights only)
+  m->lora.glayers = m->layers;   // norms / biases are the base's (adapters touch projection weights only)
   for (int li = 0; li < c.L && ld.ok; ++li) {
     const auto pr = layer_projections(c, P, li, m->layers[li].attn_norm_w != nullptr);
-    LoraLayer& ll = m->lora.layers[li];
-    LoraProj* lps[] = {&ll.qkv, &ll.wo, &ll.wi, &ll.wo2};
     for (int p = 0; p < 4 && ld.ok; ++p) {
-      if (!grouped) {
-        build_lora_proj(ld, sts, alpha, pr[p], rp, *lps[p]);
-        m->lora.max_R = std::max(m->lora.max_R, lps[p]->R);
-        continue;
-      }
       // every task's merged weights, stacked along N.  Loader{.., sts[t]} merges task t's adapters exactly as a separately
       // loaded model would (lora_fold, double precision, before the fp16 rounding).
       std::vector<float> stack, w;
@@ -796,7 +742,6 @@ Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::v
       if (ld.ok) store_projection(ld, pr[p], p, stack, T, m->lora.glayers[li]);
     }
   }
-  m->lora.grouped = grouped;
   if (!ld.ok) { *err = ld.err; model_free(m); return nullptr; }
   for (int t = 0; t < T; ++t) {
     const int h = model_add_head(m, dirs[t], token_level[t], err);
@@ -844,7 +789,7 @@ void model_free(Model* m) {
   precise_free(*m);
   for (void* p : m->allocs) cudaFree(p);
   Workspace& w = m->ws;
-  void* dev[] = {w.x, w.h, w.lo, w.qkv, w.ctx, w.mid, w.ids, w.pos, w.cu, w.pooled, w.pool_part, w.pool_arrived, w.logits, w.probs, w.cls, w.conf, w.emb, w.row_stats, w.kv_lens, w.lora_u};
+  void* dev[] = {w.x, w.h, w.lo, w.qkv, w.ctx, w.mid, w.ids, w.pos, w.cu, w.pooled, w.pool_part, w.pool_arrived, w.logits, w.probs, w.cls, w.conf, w.emb, w.row_stats, w.kv_lens};
   for (void* p : dev) if (p) cudaFree(p);
   void* host[] = {w.h_ids, w.h_cu, w.h_out, w.h_cls, w.h_conf};
   for (void* p : host) if (p) cudaFreeHost(p);
@@ -889,7 +834,6 @@ int workspace_reserve(Model& m, int tokens, int seqs, size_t out_elems) {
     rc |= regrow(w.ids, T);
     rc |= regrow(w.pos, T);
     rc |= regrow(w.row_stats, 2 * (T * (2 * static_cast<size_t>(H / 128 > 0 ? H / 128 : 1) + 1) + 4));
-    if (m.lora.max_R > 0) rc |= regrow(w.lora_u, T * static_cast<size_t>(m.lora.max_R));
     w.cap_tokens = rc ? 0 : static_cast<int>(T);
   }
   if (seqs > w.cap_seqs) {
@@ -962,25 +906,11 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
   GemmDesc g;
   g.M = T;
   g.a_rows = w.cap_tokens;
-  // shared-LoRA pass (engine.h: LoraShared): U = A-operand x a^T with every row keeping its own task's block, then the
-  // projection takes U b^T as a K extension of its accumulator
-  const bool lora_on = m.lora.tasks > 0 && m.lora.rows_per_task > 0;
-  if (lora_on && (T != m.lora.tasks * m.lora.rows_per_task || (!m.lora.grouped && !w.lora_u))) return -1;
-  auto lora_ext = [&](GemmDesc& gd, const LoraProj& lp, bool folded_form, int cat) {
-    if (!lora_on || !lp.b) return 0;
-    GemmDesc u;
-    u.M = T; u.a_rows = w.cap_tokens; u.N = lp.R; u.K = gd.K; u.A = gd.A; u.W = folded_form ? lp.a_f : lp.a;
-    u.out = w.lora_u; u.ldo = lp.R; u.epi = EPI_F16;
-    u.mask_block = lp.block; u.mask_rows = m.lora.rows_per_task;
-    if (!u.W) return -1;
-    { ProfScope ps(m, cat); if (gemm_f16(s, u)) return -1; }
-    gd.A2 = w.lora_u; gd.W2 = lp.b; gd.K2 = lp.R;
-    return 0;
-  };
-  const LoraLayer no_lora;
-  // grouped form: every projection GEMM picks the task's matrix per row block (gemm.h: w_groups)
-  const bool grouped = lora_on && m.lora.grouped;
-  if (grouped && (m.lora.rows_per_task % 256 != 0 || static_cast<int>(m.lora.glayers.size()) != c.L)) return -1;
+  // shared-LoRA pass (engine.h: LoraShared): every projection GEMM picks the task's matrix per row block (gemm.h: w_groups)
+  const bool grouped = m.lora.tasks > 0 && m.lora.rows_per_task > 0;
+  if (grouped && (T != m.lora.tasks * m.lora.rows_per_task || m.lora.rows_per_task % 256 != 0 ||
+                  static_cast<int>(m.lora.glayers.size()) != c.L))
+    return -1;
   auto run_proj = [&](GemmDesc& gd) {
     if (grouped) { gd.w_groups = m.lora.tasks; gd.w_group_rows = m.lora.rows_per_task; }
     return gemm_f16(s, gd);
@@ -1014,7 +944,6 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
     };
     for (int li = 0; li < L; ++li) {
       const LayerWeights& lw = grouped ? m.lora.glayers[li] : m.layers[li];
-      const LoraLayer& ll = lora_on ? m.lora.layers[li] : no_lora;
       const bool local = (li % c.global_every) != 0;
       const bool folded = lw.wqkv_f != nullptr;   // model_load: li > 0 with attn_norm
       g = GemmDesc();
@@ -1036,25 +965,21 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       g.epi = EPI_ROPE; g.pos = w.pos; g.rope_cols = 2 * H;
       g.rope_cos = local ? m.rope_cos_l : m.rope_cos_g;
       g.rope_sin = local ? m.rope_sin_l : m.rope_sin_g;
-      if (lora_ext(g, ll.qkv, folded, PC_GEMM_QKV)) return -1;
       { ProfScope ps(m, PC_GEMM_QKV); if (run_proj(g)) return -1; }
       { ProfScope ps(m, PC_ATTN);   // sliding-window layers visit only the key blocks inside the window
         if (attention_wgmma_fwd(s, w.qkv, w.ctx, d_cu, B, max_len, c.heads, 64, local ? c.local_attention / 2 : 0)) return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = H; g.A = w.ctx; g.W = lw.wo;
       emit_for(g);
-      if (lora_ext(g, ll.wo, false, PC_GEMM_WO)) return -1;
       { ProfScope ps(m, PC_GEMM_WO); if (run_proj(g)) return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = 2 * I; g.K = H; g.A = w.h; g.W = lw.wi_f; g.out = w.mid; g.ldo = I;
       g.fold_stats = cur_stats; g.fold_eps = c.ln_eps; g.fold_h = H;
       g.epi = EPI_GEGLU;
-      if (lora_ext(g, ll.wi, true, PC_GEMM_WI)) return -1;
       { ProfScope ps(m, PC_GEMM_WI); if (run_proj(g)) return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = I; g.A = w.mid; g.W = lw.wo2;
       emit_for(g);
-      if (lora_ext(g, ll.wo2, false, PC_GEMM_WO2)) return -1;
       { ProfScope ps(m, PC_GEMM_WO2); if (run_proj(g)) return -1; }
     }
     {   // x = pivot + hi + lo for the heads (final_norm, pooling, token heads read the fp32 stream)
@@ -1068,29 +993,24 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       return -1;
     for (int li = 0; li < L; ++li) {
       const LayerWeights& lw = grouped ? m.lora.glayers[li] : m.layers[li];
-      const LoraLayer& ll = lora_on ? m.lora.layers[li] : no_lora;
       g = GemmDesc();
       const int Hq = c.attn_w;   // == H unless the heads were padded (MiniLM)
       g.M = T; g.a_rows = w.cap_tokens; g.N = 3 * Hq; g.K = H; g.A = w.h; g.W = lw.wqkv; g.out = w.qkv; g.ldo = 3 * Hq;
       g.epi = EPI_F16; g.bias = lw.bqkv;
-      if (lora_ext(g, ll.qkv, false, PC_GEMM_QKV)) return -1;
       { ProfScope ps(m, PC_GEMM_QKV); if (run_proj(g)) return -1; }
       { ProfScope ps(m, PC_ATTN); if (attention_wgmma_fwd(s, w.qkv, w.ctx, d_cu, B, max_len, c.heads, 64, 0, m.cur_kv_lens)) return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = Hq; g.A = w.ctx; g.W = lw.wo; g.out = w.x; g.ldo = H;
       g.epi = EPI_RESID; g.resid = w.x; g.ldr = H; g.bias = lw.bo;
-      if (lora_ext(g, ll.wo, false, PC_GEMM_WO)) return -1;
       { ProfScope ps(m, PC_GEMM_WO); if (run_proj(g)) return -1; }
       { ProfScope ps(m, PC_NORM); if (layernorm_rows(s, w.x, T, H, lw.mid_norm_w, lw.mid_norm_b, c.ln_eps, w.x, w.h)) return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = I; g.K = H; g.A = w.h; g.W = lw.wi; g.out = w.mid; g.ldo = I;
       g.epi = EPI_GELU; g.bias = lw.bi;
-      if (lora_ext(g, ll.wi, false, PC_GEMM_WI)) return -1;
       { ProfScope ps(m, PC_GEMM_WI); if (run_proj(g)) return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = I; g.A = w.mid; g.W = lw.wo2; g.out = w.x; g.ldo = H;
       g.epi = EPI_RESID; g.resid = w.x; g.ldr = H; g.bias = lw.bo2;
-      if (lora_ext(g, ll.wo2, false, PC_GEMM_WO2)) return -1;
       { ProfScope ps(m, PC_GEMM_WO2); if (run_proj(g)) return -1; }
       { ProfScope ps(m, PC_NORM); if (layernorm_rows(s, w.x, T, H, lw.out_norm_w, lw.out_norm_b, c.ln_eps, w.x, w.h)) return -1; }
     }

@@ -84,7 +84,6 @@ struct Workspace {
   float* row_stats = nullptr;
   int* cu = nullptr;        // [B+1]
   int* kv_lens = nullptr;   // [B] valid keys per sequence (sr_embed_ids_padded: right-padded BERT rows whose pads stay queries)
-  __half* lora_u = nullptr; // [T, lora.max_R] rank-r projections of the current GEMM's input (shared-LoRA models)
   float* pooled = nullptr;  // [B,H]
   float* pool_part = nullptr;   // [B, kPoolParts, H] partial sums of the split pooling
   int* pool_arrived = nullptr;  // [B] arrival counters (zero between calls)
@@ -136,29 +135,12 @@ struct PreciseState {
 };
 
 // Shared-base multi-task serving from UNMERGED LoRA checkpoints (SURVEY section 8 f3; lora_adapter.rs:136-144): T task
-// checkpoints over one base load ONE copy of the base weights plus, per projection, the tasks' rank-r factors stacked:
-//   a [R, K]   rows t * block + j = A_t[j, :]            (down-projections of all tasks, one skinny GEMM: U = x a^T)
-//   b [N, R]   columns t * block + j = (alpha_t / r_t) B_t[:, j]
-// A batch is run as T copies of its rows (task-major); copy t keeps only its own column block of U (EPI_F16 mask) and
-// the projection GEMM takes U b^T into its accumulator as a K extension (gemm.h) -- base weights read once, three
-// tasks in one pass.  BERT's fused QKV has three segments per task (query / key / value adapters): block = 3 * rp.
-struct LoraProj {
-  __half* a = nullptr;
-  __half* a_f = nullptr;   // LayerNorm-fold form of `a` (A diag(gamma), rows centred) where the projection runs folded
-  __half* b = nullptr;
-  int R = 0;               // padded to a multiple of 64
-  int block = 0;           // columns of U per task
-};
-struct LoraLayer { LoraProj qkv, wo, wi, wo2; };
+// checkpoints over one base.  Every task's adapters are folded into its own copy of the projection weights at load
+// (W_t = W + (alpha_t / r_t) B_t A_t) and the T copies are stacked along N.  A batch runs ONCE as T copies of its rows
+// (task-major, each copy padded to whole 256-row blocks), and every row block of a projection GEMM picks its task's
+// matrix in the TMA producer (gemm.h: w_groups) -- the numerics of T separately loaded models in one pass.
 struct LoraShared {
   int tasks = 0;
-  int max_R = 0;
-  std::vector<LoraLayer> layers;
-  // GROUPED form (the latency / throughput form; the low-rank form above is the memory form): every task's adapters folded
-  // into its own copy of the projection weights at load (W_t = W + (alpha_t / r_t) B_t A_t), the T copies stacked along N; the
-  // batch still runs ONCE as T copies of its rows, and every row block of a projection GEMM picks its task's matrix in the TMA
-  // producer (gemm.h: w_groups) -- no rank-r GEMMs, no extra k-blocks, the numerics of T separately loaded models.
-  bool grouped = false;
   std::vector<LayerWeights> glayers;   // per layer: the base layer's norms / biases + the stacked projection weights
   std::vector<int> head_of_task;
   int rows_per_task = 0;   // set (under mu) for one forward: rows [t * rows_per_task, (t + 1) * rows_per_task) belong to task t
@@ -200,7 +182,7 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
 // One base + n task checkpoints (each a full unmerged-LoRA checkpoint over the SAME base weights, with its own head);
 // token_level[t]: 1 / 0 / -1 (from config.json).  Fails when the base tensors differ between the directories.
 Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
-                              bool grouped, std::string* err);
+                              std::string* err);
 int checkpoint_has_adapters(const std::string& dir);
 // Opens <m.dir>/model.safetensors afresh and passes every layer's four projections (qkv, attention output, intermediate,
 // output) to fn as source-order fp32 [N, K] host weights, adapters merged as model_load merges them.  fn returning false

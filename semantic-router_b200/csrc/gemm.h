@@ -68,21 +68,11 @@ struct GemmDesc {
   const float* fold_stats = nullptr;   // EPI_ROPE / EPI_GEGLU: fp32 [fold_h/128][M][2] partials of the A rows
   float fold_eps = 0.f;
   int fold_h = 0;                      // row length the statistics were taken over
-  // ---- K extension (unmerged LoRA, lora_adapter.rs:136-144): acc = A W^T + A2 W2^T in ONE accumulator.  A2 = [M, K2]
-  // holds the rank-r projections x A_t^T of every task side by side (a row carries its own task's block, zeros
-  // elsewhere), W2 = [N, K2] the matching (alpha / r) B_t blocks: the k-loop simply runs K2 / 64 steps longer, fed
-  // through a second pair of tensor maps.  Every epilogue sees the sum (a LayerNorm fold scales it by rstd as a whole,
-  // so A2 is produced WITHOUT rstd: raw rows times the folded A_t).
-  const void* A2 = nullptr;            // fp16 [a_rows >= M, K2]
-  const void* W2 = nullptr;            // fp16 [N, K2]
-  int K2 = 0;                          // multiple of 8 (TMA zero-fills the last k-block)
   // ---- grouped weights: W = w_groups matrices [N, K] stacked along N; rows [g * w_group_rows, (g + 1) * w_group_rows) of A are
   // multiplied with matrix g (w_group_rows a multiple of 128, the row-block height: a row block never straddles two
   // groups; gemm_f16 refuses anything else).  One launch serves
-  // several tasks' merged weights (engine.h: LoraShared, grouped form).
+  // several tasks' merged weights (engine.h: LoraShared).
   int w_groups = 0, w_group_rows = 0;
-  // ---- EPI_F16 column-block mask (produces A2): out[r, c] = 0 unless c / mask_block == r / mask_rows
-  int mask_block = 0, mask_rows = 0;
 };
 
 int gemm_f16(cudaStream_t stream, const GemmDesc& g);

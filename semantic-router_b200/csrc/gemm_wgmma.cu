@@ -81,8 +81,6 @@ struct KArgs {
   int topk_n;
   int grouped;               // EPI_TOPK: grouped tile schedule (see the kernel)
   int interleave;            // tiles w, w + W, ... per worker instead of a contiguous range
-  int K2;                    // K extension: k-blocks beyond K come from (tmap_a2, tmap_b2) -- low-rank adapters (gemm.h)
-  int mask_block, mask_rows; // EPI_F16: keep column c of row r only when c / mask_block == r / mask_rows (0: off)
   int grp_rows;              // > 0: W is a stack of [N, K] matrices, rows [g * grp_rows, (g + 1) * grp_rows) of A multiply matrix g
 };
 constexpr int kTopK = 8;
@@ -151,8 +149,7 @@ __device__ __forceinline__ void fold_scale(float rstd, uint32_t* a, uint32_t* b)
 template <int EPI, int CN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-            const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_aux,
-            const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_b2, const KArgs p) {
+            const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_aux, const KArgs p) {
   using Cfg = GemmCfg<EPI>;
   static_assert(Cfg::kSmemBytes <= kSmemLimit, "over the 227 KB shared-memory opt-in limit");
   constexpr bool kHL = EPI == EPI_RESID_HL;
@@ -176,9 +173,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int lane = threadIdx.x & 31;
   const int m_blocks = (p.M + BM - 1) / BM;
   const int n_blocks = (p.N + BN - 1) / BN;
-  const int k1_blocks = (p.K + BK - 1) / BK;
-  // K extension: the accumulator also takes A2[M, K2] x W2[N, K2]^T -- same stages, same MMAs, other tensor maps
-  const int k_blocks = k1_blocks + (p.K2 + BK - 1) / BK;
+  const int k_blocks = (p.K + BK - 1) / BK;
   // Thread-block clusters of cn CTAs along N (1: none).  The schedule below hands out CLUSTER tiles -- cn neighbouring
   // 128 x 128 tiles of one row block -- and CTA rn of the cluster computes tile (m_c, cn n_c + rn) of cluster tile
   // (m_c, n_c).  The cn CTAs share the A row block: each loads a 1/cn slice of the A box and multicasts it to all of
@@ -264,17 +259,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         const int w_row0 = p.grp_rows > 0 ? ((m_blk * BM) / p.grp_rows) * p.N : 0;
         for (int kb = 0; kb < k_blocks; ++kb) {
           mbar_wait(&empty_bar[s], ph ^ 1);
-          const bool ext = kb >= k1_blocks;
-          const CUtensorMap* ma = ext ? &tmap_a2 : &tmap_a;
-          const CUtensorMap* mb = ext ? &tmap_b2 : &tmap_b;
-          const int kc = (ext ? kb - k1_blocks : kb) * BK;
+          const int kc = kb * BK;
           // the stage fills with the A slices of every CTA of the cluster and this CTA's own W box: the whole stage
           mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
           uint8_t* da = smem_a + s * Cfg::kABytes + rn * a_rows * (BK * 2);
           const int ya = m_blk * BM + rn * a_rows;
-          if (cn > 1) tma_load_2d_multicast(da, ma, &full_bar[s], kc, ya, a_mask);
-          else tma_load_2d(da, ma, &full_bar[s], kc, ya);
-          tma_load_2d(smem_b + s * Cfg::kBBytes, mb, &full_bar[s], kc, (ext ? 0 : w_row0) + n_blk * BN);
+          if (cn > 1) tma_load_2d_multicast(da, &tmap_a, &full_bar[s], kc, ya, a_mask);
+          else tma_load_2d(da, &tmap_a, &full_bar[s], kc, ya);
+          tma_load_2d(smem_b + s * Cfg::kBBytes, &tmap_b, &full_bar[s], kc, w_row0 + n_blk * BN);
           if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
         }
       }
@@ -664,13 +656,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 v0 += b.x; v1 += b.y;
               }
               if constexpr (EPI == EPI_GELU) { v0 = gelu_erf_fast_f(v0); v1 = gelu_erf_fast_f(v1); }
-              if constexpr (EPI == EPI_F16) {
-                if (p.mask_block > 0) {   // adapter projections: a row keeps the column block of its own task only
-                  const int own = (row0 + lane) / p.mask_rows, col = ocol0 + hf * 32 + 2 * i;
-                  if (col / p.mask_block != own) v0 = 0.f;
-                  if ((col + 1) / p.mask_block != own) v1 = 0.f;
-                }
-              }
               h[i] = pack_half2(v0, v1);
             }
 #pragma unroll
@@ -799,8 +784,7 @@ int max_clusters(int num_sms) {
 
 template <int EPI, int CN = 1>
 int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
-           const CUtensorMap& tx, const CUtensorMap& ta2, const CUtensorMap& tb2, const KArgs& ka, int num_sms,
-           int grid_override = 0) {
+           const CUtensorMap& tx, const KArgs& ka, int num_sms, int grid_override = 0) {
   using Cfg = GemmCfg<EPI>;
   // per-device attribute; cheap enough to set on every launch (multi-GPU processes switch devices)
   SRB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<EPI, CN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
@@ -830,7 +814,7 @@ int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, co
   cfg.gridDim = dim3(grid);
   cfg.attrs = attr;
   cfg.numAttrs = nattr;
-  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<EPI, CN>, ta, tb, tc, tx, ta2, tb2, ka));
+  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<EPI, CN>, ta, tb, tc, tx, ka));
   note_launch();
   return 0;
 }
@@ -967,25 +951,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   ka.interleave = (((g.epi == EPI_RESID && g.resid != nullptr) || is_hl) && resid_interleave && (is_hl || g.K > interleave_min_k) &&
                    g.N / BN > 1) ? 1 : 0;
   ka.fold_stats = nullptr; ka.fold_eps = 0.f; ka.fold_inv_h = 0.f; ka.fold_parts = 0;
-  ka.K2 = 0; ka.mask_block = 0; ka.mask_rows = 0;
   ka.grp_rows = w_groups > 1 ? g.w_group_rows : 0;
-  CUtensorMap ta2 = ta, tb2 = tb;   // K extension (low-rank adapters): unused copies otherwise
-  if (g.K2 > 0) {
-    if (!g.A2 || !g.W2 || g.K2 % 8 != 0 || g.epi == EPI_TOPK) {
-      fprintf(stderr, "[srb200] gemm_f16: K extension needs A2, W2 and K2 %% 8 == 0\n");
-      return -1;
-    }
-    if (make_tmap_f16_kmajor(&ta2, g.A2, static_cast<uint64_t>(g.a_rows > 0 ? g.a_rows : g.M), g.K2, BM / cn)) return -1;
-    if (make_tmap_f16_kmajor(&tb2, g.W2, g.N, g.K2, BN)) return -1;
-    ka.K2 = g.K2;
-  }
-  if (g.mask_block > 0) {
-    if (g.epi != EPI_F16 || g.mask_rows <= 0) {
-      fprintf(stderr, "[srb200] gemm_f16: the column-block mask belongs to EPI_F16\n");
-      return -1;
-    }
-    ka.mask_block = g.mask_block; ka.mask_rows = g.mask_rows;
-  }
   CUtensorMap tx = tc;   // auxiliary map (EPI_RESID_HL: the low halves of the pair); unused otherwise
   if (is_hl && make_tmap_2d(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.lo16, g.N, g.M, g.N, 64, 32)) return -1;
   if (g.fold_stats) {
@@ -998,16 +964,16 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
     ka.fold_parts = g.fold_h / 128;
   }
   switch (g.epi) {
-    case EPI_F16: return launch<EPI_F16>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
+    case EPI_F16: return launch<EPI_F16>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_ROPE:
-      return cn == 2 ? launch<EPI_ROPE, 2>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms)
-                     : launch<EPI_ROPE>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
-    case EPI_RESID: return launch<EPI_RESID>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
-    case EPI_RESID_HL: return launch<EPI_RESID_HL>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
+      return cn == 2 ? launch<EPI_ROPE, 2>(stream, ta, tb, tc, tx, ka, num_sms)
+                     : launch<EPI_ROPE>(stream, ta, tb, tc, tx, ka, num_sms);
+    case EPI_RESID: return launch<EPI_RESID>(stream, ta, tb, tc, tx, ka, num_sms);
+    case EPI_RESID_HL: return launch<EPI_RESID_HL>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_GEGLU:
-      return cn == 2 ? launch<EPI_GEGLU, 2>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms)
-                     : launch<EPI_GEGLU>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
-    case EPI_GELU: return launch<EPI_GELU>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
+      return cn == 2 ? launch<EPI_GEGLU, 2>(stream, ta, tb, tc, tx, ka, num_sms)
+                     : launch<EPI_GEGLU>(stream, ta, tb, tc, tx, ka, num_sms);
+    case EPI_GELU: return launch<EPI_GELU>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_TOPK: {
       if (!g.topk_idx || !g.topk_score || !g.topk_lists || g.N % 256 != 0) {
         fprintf(stderr, "[srb200] gemm_f16: EPI_TOPK needs list buffers and N %% 256 == 0\n");
@@ -1023,10 +989,10 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
       if (grouped_on && m_blocks > 1 && groups >= 1 && n_blocks >= groups) {
         ka.grouped = 1;
         *g.topk_lists = groups * m_blocks;
-        return launch<EPI_TOPK>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms, groups * m_blocks);
+        return launch<EPI_TOPK>(stream, ta, tb, tc, tx, ka, num_sms, groups * m_blocks);
       }
       *g.topk_lists = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-      return launch<EPI_TOPK>(stream, ta, tb, tc, tx, ta2, tb2, ka, num_sms);
+      return launch<EPI_TOPK>(stream, ta, tb, tc, tx, ka, num_sms);
     }
   }
   return -1;

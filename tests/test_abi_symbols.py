@@ -143,11 +143,10 @@ def test_adapter_probe_and_shared_loader_without_gpu(lib, tmp_path):
     assert L.sr_checkpoint_has_adapters(dirs["merged"].encode()) == 0
     assert L.sr_checkpoint_has_adapters(dirs["lora"].encode()) == 1
     assert L.sr_checkpoint_has_adapters(str(tmp_path / "missing").encode()) == -1
-    for mode in (0, 1):
-        with pytest.raises(pkg.SrError, match="share one base"):
-            pkg.LoraSharedModel([dirs["lora"], dirs["other"]], [0, 0], device=0, mode=mode)
-        with pytest.raises(pkg.SrError, match="no lora_A"):
-            pkg.LoraSharedModel([dirs["merged"], dirs["merged"]], [0, 0], device=0, mode=mode)
+    with pytest.raises(pkg.SrError, match="share one base"):
+        pkg.LoraSharedModel([dirs["lora"], dirs["other"]], [0, 0], device=0)
+    with pytest.raises(pkg.SrError, match="no lora_A"):
+        pkg.LoraSharedModel([dirs["merged"], dirs["merged"]], [0, 0], device=0)
     import torch
     if not torch.cuda.is_available():
         with pytest.raises(pkg.SrError):                         # same base, adapters present: now it needs the device

@@ -2,7 +2,7 @@
 
 * Tensor-name prefixes: one synthetic ModernBERT checkpoint under each prefix the reference loaders try ("model.",
   "_orig_mod.model.", none, "_orig_mod.") gives byte-identical logits / probabilities and hidden rows through the ordinary
-  load, the precise path and both shared-LoRA forms; one BERT checkpoint with and without "bert." does the same, and a
+  load, the precise path and the shared-LoRA pass; one BERT checkpoint with and without "bert." does the same, and a
   head-only directory still finds "bert." through its pooler.
 * A checkpoint replaced in place (os.replace, as a trainer saving checkpoints does): the precise path of a model loaded
   afterwards from the same directory builds its weights from the new file, not from an earlier mapping."""
@@ -72,13 +72,12 @@ def _modernbert_results(srlib, cfg, prefix, seqs):
         r = m.classify_ids(seqs)
         out["precise_logits"], out["precise_hidden"] = r["logits"], _hidden(srlib, m, T)
         m.close()
-        for mode in (0, 1):
-            m = srlib.LoraSharedModel(dirs, [0, 0], device=0, mode=mode)
-            probs, cls, _ = m.classify_shared_ids(seqs)
-            for t in range(len(dirs)):
-                out[f"lora{mode}_probs{t}"], out[f"lora{mode}_cls{t}"] = probs[t], cls[t]
-            out[f"lora{mode}_hidden"] = _hidden(srlib, m, T)   # task 0's copy of the rows
-            m.close()
+        m = srlib.LoraSharedModel(dirs, [0, 0], device=0)
+        probs, cls, _ = m.classify_shared_ids(seqs)
+        for t in range(len(dirs)):
+            out[f"lora_probs{t}"], out[f"lora_cls{t}"] = probs[t], cls[t]
+        out["lora_hidden"] = _hidden(srlib, m, T)   # task 0's copy of the rows
+        m.close()
     return out
 
 

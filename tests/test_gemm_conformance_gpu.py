@@ -2,12 +2,10 @@
 descriptor (sr_test_gemm_desc).
 
 * Float64 parity: every epilogue at the shape edges (M around the 64-row cluster slices and the 128-row blocks, N with a
-  half-empty last column tile, K with a partial last k-block), the K extension, the LayerNorm fold, the column-block
-  mask, grouped weights and the cache scan, each element within the bound of oracle/gemm_oracle.py.  Every A (and A2)
-  has stale NaN / inf rows past M, as behind the engine's a_rows = cap_tokens, and every output has sentinel rows past M
+  half-empty last column tile, K with a partial last k-block), the LayerNorm fold, grouped weights and the cache scan,
+  each element within the bound of oracle/gemm_oracle.py.  Every A has stale NaN / inf rows past M, as behind the engine's a_rows = cap_tokens, and every output has sentinel rows past M
   and sentinel columns [n_out, ldo) that must survive.
-* Bitwise invariants: clusters against the unclustered halves, the K extension against the concatenated GEMM, grouped
-  weights against per-group GEMMs, stale rows against a_rows = M, and the launch schedules chosen by environment
+* Bitwise invariants: clusters against the unclustered halves, grouped weights against per-group GEMMs, stale rows against a_rows = M, and the launch schedules chosen by environment
   variables (child processes) against the default.
 * Refusals: shapes gemm_f16 rejects return non-zero and leave the output alone.
 
@@ -128,8 +126,8 @@ class Problem:
             assert (bits[:, self.n_out:] == s).all(), "columns [n_out, ldo) were written"
 
 
-def problem(epi, M, N, K, seed, *, bias=False, resid=True, k2=0, fold=False, rope_cols=0, w_groups=0, w_group_rows=0,
-            mask_block=0, mask_rows=0, stale=True, w_scale=0.05):
+def problem(epi, M, N, K, seed, *, bias=False, resid=True, fold=False, rope_cols=0, w_groups=0, w_group_rows=0,
+            stale=True, w_scale=0.05):
     dev = torch.device(DEV)
     g = torch.Generator(device=dev).manual_seed(seed)
     a_rows = _up(M, 128) + 64 if stale else M
@@ -137,12 +135,6 @@ def problem(epi, M, N, K, seed, *, bias=False, resid=True, k2=0, fold=False, rop
     W = (torch.randn(N * max(w_groups, 1), K, generator=g, device=dev) * w_scale).half()
     d = dict(m=M, n=N, k=K, a=A, a_rows=a_rows, w=W, epi=epi)
     o = {}
-    if k2:
-        A2 = torch.randn(a_rows, k2, generator=g, device=dev).half()
-        W2 = (torch.randn(N, k2, generator=g, device=dev) * w_scale).half()
-        d.update(a2=A2, w2=W2, k2=k2)
-        o.update(a2=A2[:M], w2=W2)
-        _stale(A2, M)
     _stale(A, M)
     if bias:
         b = torch.randn(N, generator=g, device=dev)
@@ -159,9 +151,6 @@ def problem(epi, M, N, K, seed, *, bias=False, resid=True, k2=0, fold=False, rop
     if w_groups:
         d.update(w_groups=w_groups, w_group_rows=w_group_rows)
         o.update(w_groups=w_groups, w_group_rows=w_group_rows)
-    if mask_block:
-        d.update(mask_block=mask_block, mask_rows=mask_rows)
-        o.update(mask_block=mask_block, mask_rows=mask_rows)
     n_out = N // 2 if epi == EPI_GEGLU else N
     p = Problem(epi, M, n_out, d, o)
     if epi == EPI_RESID_HL:
@@ -239,35 +228,13 @@ def test_shape_edges(lib, epi, M, N, K, i):
     check_parity(p)
 
 
-K2_EPIS = [(EPI_F16, 320), (EPI_ROPE, 2304), (EPI_RESID, 192), (EPI_GEGLU, 2304), (EPI_GELU, 320), (EPI_RESID_HL, 640)]
-
-
-@pytest.mark.parametrize("k2,M,K", [(64, 129, 768), (192, 2333, 200), (24, 65, 72)])
-@pytest.mark.parametrize("epi,N", K2_EPIS, ids=[go.EPI_NAMES[e] for e, _ in K2_EPIS])
-def test_k_extension(lib, epi, N, k2, M, K):
-    p = problem(epi, M, N, K, seed=7 * k2 + epi, bias=epi in (EPI_F16, EPI_RESID, EPI_GELU, EPI_RESID_HL), k2=k2,
-                rope_cols=ROPE_COLS.get(N, 0))
-    check_parity(p)
-
-
-@pytest.mark.parametrize("k2", [0, 64, 24])
 @pytest.mark.parametrize("epi,N,M", [(EPI_ROPE, 2304, 2333), (EPI_ROPE, 320, 127), (EPI_GEGLU, 2304, 65),
                                      (EPI_GEGLU, 640, 2333)])
-def test_layernorm_fold(lib, epi, N, M, k2):
-    """The fold scales the whole accumulator (the K extension included: A2 is produced without rstd) by the row's rstd,
-    which depends on the LayerNorm epsilon for rows of small variance."""
-    p = problem(epi, M, N, 768, seed=31 * M + k2, k2=k2, fold=True, rope_cols=ROPE_COLS.get(N, 0), w_scale=0.01)
+def test_layernorm_fold(lib, epi, N, M):
+    """The fold scales the whole accumulator by the row's rstd, which depends on the LayerNorm epsilon for rows of small
+    variance."""
+    p = problem(epi, M, N, 768, seed=31 * M, fold=True, rope_cols=ROPE_COLS.get(N, 0), w_scale=0.01)
     check_parity(p, tag=go.EPI_NAMES[epi] + "+fold")
-
-
-@pytest.mark.parametrize("mask_rows", [128, 256])
-@pytest.mark.parametrize("block", [8, 24, 48, 64])
-def test_mask_producer(lib, block, mask_rows):
-    """The adapter projection U of the shared-LoRA pass: N = R as the engine pads it, every row keeps its task's block."""
-    tasks = 3
-    R = (tasks * block + 63) // 64 * 64
-    p = problem(EPI_F16, tasks * mask_rows, R, 200, seed=block + mask_rows, mask_block=block, mask_rows=mask_rows)
-    check_parity(p, tag="f16+mask")
 
 
 @pytest.mark.parametrize("rows", [128, 256])
@@ -345,16 +312,14 @@ def _bits(t):
     return t.view(torch.int32) if t.dtype == torch.float32 else t.view(torch.int16)
 
 
-@pytest.mark.parametrize("k2", [0, 64])
 @pytest.mark.parametrize("fold", [False, True])
 @pytest.mark.parametrize("epi", [EPI_ROPE, EPI_GEGLU], ids=["rope", "geglu"])
-def test_cluster_pair_equals_unclustered_halves(lib, epi, fold, k2):
+def test_cluster_pair_equals_unclustered_halves(lib, epi, fold):
     """N = 2304 (18 column tiles) runs as 2-CTA clusters sharing A by multicast; as two N = 1152 halves (9 tiles each)
     it runs without clusters.  The tiles, their wgmma sequences and epilogues are the same: bitwise equal outputs."""
     assert _cluster(lib, epi, 2304, 768) == 2 and _cluster(lib, epi, 1152, 768) == 1
     for M in (1, 40, 65, 127, 2333, 20000):
-        p = problem(epi, M, 2304, 768, seed=M + 3 * k2 + fold, k2=k2, fold=fold, rope_cols=1536,
-                    w_scale=0.01 if fold else 0.05)
+        p = problem(epi, M, 2304, 768, seed=M + fold, fold=fold, rope_cols=1536, w_scale=0.01 if fold else 0.05)
         d = p.desc
         assert run(**d)[0] == 0
         full = p.out[:M].clone()
@@ -362,29 +327,10 @@ def test_cluster_pair_equals_unclustered_halves(lib, epi, fold, k2):
         half_out = p.n_out // 2
         for h in range(2):
             dh = dict(d, n=1152, w=d["w"][1152 * h:1152 * (h + 1)], out=p.out[:, half_out * h:])
-            if k2:
-                dh["w2"] = d["w2"][1152 * h:1152 * (h + 1)]
             if epi == EPI_ROPE:
                 dh["rope_cols"] = 1152 if h == 0 else 1536 - 1152
             assert run(**dh)[0] == 0
         assert torch.equal(_bits(full), _bits(p.out[:M])), M
-
-
-@pytest.mark.parametrize("k2", [64, 24])
-@pytest.mark.parametrize("epi,N", [(EPI_RESID, 704), (EPI_ROPE, 2304)], ids=["resid", "rope"])
-def test_k_extension_is_concatenation(lib, epi, N, k2):
-    """For K % 64 == 0 the K extension runs the k-blocks of [A | A2] x [W | W2] in the same order."""
-    M, K = 2333, 768
-    p = problem(epi, M, N, K, seed=k2 + N, k2=k2, rope_cols=ROPE_COLS.get(N, 0), resid=False)
-    d = p.desc
-    assert run(**d)[0] == 0
-    ext = p.out[:M].clone()
-    cat_a = torch.cat([d["a"], d["a2"]], 1).contiguous()
-    cat_w = torch.cat([d["w"], d["w2"]], 1).contiguous()
-    dc = {k: v for k, v in d.items() if k not in ("a2", "w2", "k2")}
-    dc.update(a=cat_a, w=cat_w, k=K + k2)
-    assert run(**dc)[0] == 0
-    assert torch.equal(_bits(ext), _bits(p.out[:M]))
 
 
 @pytest.mark.parametrize("rows", [128, 256])
@@ -406,10 +352,10 @@ def test_grouped_weights_are_per_group_gemms(lib, epi, rows):
 @pytest.mark.parametrize("epi,N", [(EPI_F16, 320), (EPI_ROPE, 2304), (EPI_RESID, 192), (EPI_GEGLU, 2304),
                                    (EPI_GELU, 192), (EPI_RESID_HL, 640)], ids=lambda x: str(x))
 def test_stale_rows(lib, epi, N, M):
-    """Rows [M, a_rows) of A and A2 hold NaN / inf (the engine's A covers cap_tokens rows).  With a 2-CTA cluster at
-    M = 40 the second CTA's multicast slice (rows 64..127) lies wholly past M.  Rows < M must equal a run over exactly
-    M rows, and nothing past M or past n_out may be written (checked by the sentinels)."""
-    p = problem(epi, M, N, 200, seed=M + epi, k2=24, rope_cols=ROPE_COLS.get(N, 0),
+    """Rows [M, a_rows) of A hold NaN / inf (the engine's A covers cap_tokens rows).  With a 2-CTA cluster at M = 40
+    the second CTA's multicast slice (rows 64..127) lies wholly past M.  Rows < M must equal a run over exactly M rows,
+    and nothing past M or past n_out may be written (checked by the sentinels)."""
+    p = problem(epi, M, N, 200, seed=M + epi, rope_cols=ROPE_COLS.get(N, 0),
                 bias=epi in (EPI_F16, EPI_GELU, EPI_RESID_HL))
     d = p.desc
     out0 = p.out.clone()
@@ -420,7 +366,7 @@ def test_stale_rows(lib, epi, N, M):
     p.out.copy_(out0)
     if lo0 is not None:
         p.lo.copy_(lo0)
-    exact = dict(d, a=d["a"][:M].clone(), a2=d["a2"][:M].clone(), a_rows=M)
+    exact = dict(d, a=d["a"][:M].clone(), a_rows=M)
     assert run(**exact)[0] == 0
     again = [p.out[:M]] + ([p.lo[:M]] if p.lo is not None else [])
     for x, y in zip(stale, again):
@@ -500,8 +446,6 @@ REFUSED = {
     "n_mod_64": dict(epi=EPI_F16, N=100, K=64),
     "k_mod_8": dict(epi=EPI_F16, N=128, K=100),
     "geglu_n_mod_128": dict(epi=EPI_GEGLU, N=192, K=64),
-    "k2_mod_8": dict(epi=EPI_F16, N=128, K=64, k2=20),
-    "mask_not_f16": dict(epi=EPI_GELU, N=128, K=64, mask=(8, 128)),
     "group_rows_192": dict(epi=EPI_F16, N=128, K=64, groups=192),
     "group_rows_64": dict(epi=EPI_F16, N=128, K=64, groups=64),
     "stats_not_pair": dict(epi=EPI_RESID, N=128, K=64, row_stats=True),
@@ -521,10 +465,6 @@ def test_refusals(lib, case):
     out = torch.empty(M, ldo, device=dev, dtype=torch.float16)
     out.view(torch.int16).fill_(S16)
     d = dict(m=M, n=N, k=K, a=a, w=w, out=out, ldo=ldo, epi=c["epi"])
-    if "k2" in c:
-        d.update(a2=torch.randn(M, c["k2"], device=dev).half(), w2=torch.randn(N, c["k2"], device=dev).half(), k2=c["k2"])
-    if "mask" in c:
-        d.update(mask_block=c["mask"][0], mask_rows=c["mask"][1])
     if "groups" in c:
         d.update(w_groups=3, w_group_rows=c["groups"])
     if "row_stats" in c:

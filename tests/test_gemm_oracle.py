@@ -98,18 +98,7 @@ def test_fold_is_layernorm_then_matmul(epi):
     assert (rel < 1e-5).all()
 
 
-def test_k_extension_is_concatenation():
-    g = _gen(4)
-    M, K, K2, N = 50, 200, 24, 192
-    a, w, a2, w2 = _f16((M, K), g), _f16((N, K), g, 0.1), _f16((M, K2), g), _f16((N, K2), g, 0.1)
-    b = torch.randn(N, generator=g)
-    r = go.gemm(go.EPI_F16, a, w, bias=b, a2=a2, w2=w2)
-    cat = go.gemm(go.EPI_F16, torch.cat([a, a2], 1), torch.cat([w, w2], 1), bias=b)
-    torch.testing.assert_close(r.value, cat.value, rtol=1e-14, atol=1e-14)
-    torch.testing.assert_close(r.coef, cat.coef, rtol=1e-14, atol=0)
-
-
-def test_grouped_weights_and_mask():
+def test_grouped_weights():
     g = _gen(5)
     rows, G, K, N = 128, 3, 64, 128
     a, w = _f16((G * rows - 7, K), g), _f16((G * N, K), g, 0.1)
@@ -117,12 +106,6 @@ def test_grouped_weights_and_mask():
     for i in range(G):
         sl = slice(i * rows, (i + 1) * rows)
         torch.testing.assert_close(r.value[sl], a[sl].double() @ w[i * N:(i + 1) * N].double().t(), rtol=1e-14, atol=0)
-    # the column-block mask: row r keeps the columns of its own block r // mask_rows
-    m = go.gemm(go.EPI_F16, a, w[:N], mask_block=24, mask_rows=rows)
-    own = torch.arange(a.shape[0])[:, None] // rows
-    keep = (torch.arange(N)[None, :] // 24) == own
-    assert (m.value[~keep] == 0).all() and (m.coef[~keep] == 0).all() and (m.eps[~keep] == 0).all()
-    torch.testing.assert_close(m.value[keep], (a.double() @ w[:N].double().t())[keep], rtol=1e-14, atol=0)
 
 
 def test_gelu_derivative_and_bound_covers_rounding():

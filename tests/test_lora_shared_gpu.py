@@ -1,8 +1,8 @@
 """Shared-base multi-task pass over UNMERGED LoRA checkpoints (SURVEY section 8 f3; model_architectures/lora/lora_adapter.rs:136-144,
 pkg/classification/unified_classifier.go:113): three task checkpoints over ONE base -- intent (sequence head), PII (token head),
 security (sequence head); ranks 8 / 16 / 32, their own alpha, not every projection adapted -- load as one model
-(sr_model_load_lora_shared) and a batch runs ONCE through the encoder, every task's copy of the rows with its own rank-r term
-added inside the projection GEMMs (K extension of the wgmma mainloop).  Expected values: the oracle on the MERGED weights
+(sr_model_load_lora_shared) and a batch runs ONCE through the encoder, every task's copy of the rows multiplied with that task's
+merged projection weights (picked per row block in the GEMM's TMA producer).  Expected values: the oracle on the MERGED weights
 W + (alpha / r) B A of each task (merge_weights, lora_adapter.rs:157-168), i.e. what three separate forwards would give;
 and the three-slot path of this library (load-time fold) on the same inputs."""
 import json
@@ -50,24 +50,23 @@ def _modernbert_tasks(cfg, tmp, std=0.02):
 
 
 # Tolerances: token-level probabilities 3e-3 as in test_encoder_parity_gpu.py (no pooling to average the drift); sequence
-# probabilities 1.5e-3 -- measured 3.3e-4 .. 1.1e-3 on these x8-scaled heads where the three-slot path (adapters folded at load,
-# no rank-r intermediates) gives 2.6e-4 .. 1.2e-3 on the same inputs: the drift is the fp16 pipeline's, not the low-rank form's.  Adapter scale 0.02 gives |dW| ~ 10 % of |W| (a trained adapter's order of magnitude); 0.05 makes the
-# low-rank term as large as the base weights themselves -- every fp16-rounded intermediate then carries twice the signal, and
-# the bounds are doubled for that case (the three-slot path, adapters folded at load, drifts by the same amount: printed).
-# mode: the low-rank form (ONE copy of the base, rank-r terms in the GEMMs) and the grouped form (the tasks' merged matrices
-# stacked, picked per 256-row block in the TMA producer; every copy of the rows padded to whole blocks).  The grouped form has
-# the arithmetic of the three-slot path: it must agree with it to batch-composition noise (1e-5), not just to the tolerance.
-@pytest.mark.parametrize("mode", [0, 1], ids=["lowrank", "grouped"])
+# probabilities 1.5e-3, where the three-slot path (adapters folded at load) gives 2.6e-4 .. 1.2e-3 on these x8-scaled heads:
+# the drift is the fp16 pipeline's.  Adapter scale 0.02 gives |dW| ~ 10 % of |W| (a trained adapter's order of magnitude);
+# 0.05 makes the adapter term as large as the base weights themselves -- every fp16-rounded intermediate then carries twice
+# the signal, and the bounds are doubled for that case (the three-slot path drifts by the same amount: printed).
+# The shared pass stacks the tasks' merged matrices and picks one per 256-row block in the TMA producer (every copy of the
+# rows padded to whole blocks): it has the arithmetic of the three-slot path and must agree with it to batch-composition
+# noise (1e-5), not just to the tolerance.
 @pytest.mark.parametrize("std,tol", [(0.02, 1.0), (0.05, 2.0)])
 @pytest.mark.parametrize("lens", [[33, 200, 512], [7], [64] * 40 + [300, 511, 2, 129]])
-def test_three_tasks_one_pass_modernbert(srlib, cuda, lens, std, tol, mode):
+def test_three_tasks_one_pass_modernbert(srlib, cuda, lens, std, tol):
     cfg = eo.ModernBertConfig(vocab_size=1000, num_hidden_layers=4, max_position_embeddings=1024, pad_token_id=0)
     rng = np.random.default_rng(12 + len(lens))
     seqs = synth.make_ids(rng, lens, cfg.vocab_size)
     with tempfile.TemporaryDirectory() as tmp:
         dirs, merged, base = _modernbert_tasks(cfg, tmp, std)
-        m = srlib.LoraSharedModel(dirs, [t[3] for t in TASKS], device=0, mode=mode)
-        assert m.tasks == 3 and srlib.lib().sr_lora_shared_mode(m.handle) == mode
+        m = srlib.LoraSharedModel(dirs, [t[3] for t in TASKS], device=0)
+        assert m.tasks == 3
         probs, cls, conf = m.classify_shared_ids(seqs)
         probs2, cls2, _ = m.classify_shared_ids(seqs)                  # second call: the graph replay of small batches
         m.close()
@@ -105,9 +104,9 @@ def test_three_tasks_one_pass_modernbert(srlib, cuda, lens, std, tol, mode):
                 worst_between = max(worst_between, float(np.abs(slots[t]["probs"][i] - probs[t][i]).max()))
                 worst_slots[0] = max(worst_slots[0], float(np.abs(slots[t]["probs"][i] - ref["probs"][0]).max()))
             worst[tok] = max(worst[tok], float(d))
-    print(f"shared-LoRA pass ({['low-rank', 'grouped'][mode]}), adapters x{std}, lens={lens[:4]}..: max |dprob| vs merged-weight oracle: sequence heads {worst[0]:.2e}, "
+    print(f"shared-LoRA pass, adapters x{std}, lens={lens[:4]}..: max |dprob| vs merged-weight oracle: sequence heads {worst[0]:.2e}, "
           f"token head {worst[1]:.2e} (three-slot path vs oracle: {worst_slots[0]:.2e} / {worst_slots[1]:.2e}; between the two paths {worst_between:.2e})")
-    assert worst[0] < seq_tol and worst[1] < tok_tol and worst_between < (1e-5 if mode == 1 else 2 * tok_tol)
+    assert worst[0] < seq_tol and worst[1] < tok_tol and worst_between < 1e-5
     # and the adapters matter: the base alone answers differently
     bt = {k: torch.from_numpy(v) for k, v in base.items()}
     bt.update({k: merged[0][k] for k in ("head.dense.weight", "head.norm.weight", "classifier.weight", "classifier.bias")})
@@ -115,8 +114,7 @@ def test_three_tasks_one_pass_modernbert(srlib, cuda, lens, std, tol, mode):
     assert np.abs(refb["probs"][0] - probs[0][0]).max() > 1e-2
 
 
-@pytest.mark.parametrize("mode", [0, 1], ids=["lowrank", "grouped"])
-def test_three_tasks_one_pass_bert(srlib, cuda, mode):
+def test_three_tasks_one_pass_bert(srlib, cuda):
     """BERT-family base (the reference's LoRA classifiers are BERT or ModernBERT, classifiers/lora/intent_lora.rs:50-78): PEFT
     adapts query / key / value separately -- three segments of the fused QKV projection."""
     cfg = eo.BertConfig(vocab_size=800, num_hidden_layers=3, max_position_embeddings=512)
@@ -151,7 +149,7 @@ def test_three_tasks_one_pass_bert(srlib, cuda, mode):
             json.dump({"rank": rank, "alpha": alpha}, open(os.path.join(d, "lora_config.json"), "w"))
             dirs.append(d)
             merged.append({k: torch.from_numpy(v) for k, v in mg.items()})
-        m = srlib.LoraSharedModel(dirs, [0, 0], device=0, mode=mode)
+        m = srlib.LoraSharedModel(dirs, [0, 0], device=0)
         probs, cls, _ = m.classify_shared_ids(seqs, pooler_mode=1)
         m.close()
     for t in range(2):
@@ -175,8 +173,6 @@ def test_checkpoints_over_different_bases_are_refused(srlib, cuda):
             dirs.append(d)
         with pytest.raises(srlib.SrError, match="share one base"):
             srlib.LoraSharedModel(dirs, [0, 0], device=0)
-        with pytest.raises(srlib.SrError, match="share one base"):
-            srlib.LoraSharedModel(dirs, [0, 0], device=0, mode=1)
 
 
 def test_text_abi_serves_the_three_tasks_from_one_pass(srlib, cuda):
@@ -202,7 +198,7 @@ def test_text_abi_serves_the_three_tasks_from_one_pass(srlib, cuda):
         for d in dirs:
             tf.BUILDERS["modernbert"](os.path.join(d, "tokenizer.json"))
         res = {}
-        for mode in ("1", "lowrank", "0"):                           # grouped (default), low-rank, three slots
+        for mode in ("1", "0"):                                      # shared pass (default), three slots
             os.environ["SR_B200_LORA_SHARED"] = mode
             inst = os.path.join(tmp, f"libcandle_private_{mode}.so")
             shutil.copyfile(srlib.LIB_PATH, inst)                    # fresh global slots
@@ -217,20 +213,18 @@ def test_text_abi_serves_the_three_tasks_from_one_pass(srlib, cuda):
             n0 = L.sr_launch_count()
             r = L.classify_batch_with_lora(_arr(texts), len(texts))
             res[mode] = (r, L, L.sr_launch_count() - n0)
-        b = res["0"][0]
-        for key, tol3 in (("1", 1e-5), ("lowrank", 2e-3)):            # grouped: the three-slot arithmetic; low-rank: within tolerance
-            a = res[key][0]
-            assert a.batch_size == b.batch_size == len(texts)
-            flips = 0
-            for i in range(len(texts)):
-                assert abs(a.intent_results[i].confidence - b.intent_results[i].confidence) < tol3
-                assert abs(a.security_results[i].confidence - b.security_results[i].confidence) < tol3
-                assert abs(a.pii_results[i].confidence - b.pii_results[i].confidence) < 1.5 * tol3
-                flips += a.intent_results[i].category != b.intent_results[i].category
-                flips += a.security_results[i].threat_type != b.security_results[i].threat_type
-            assert flips <= (0 if key == "1" else 1)                 # a class may flip only on a near-tie of random weights
-        print(f"launches for {len(texts)} texts: grouped pass {res['1'][2]}, low-rank pass {res['lowrank'][2]}, three slots {res['0'][2]}")
-        assert res["1"][2] < res["lowrank"][2] < res["0"][2]
+        a, b = res["1"][0], res["0"][0]                               # the shared pass has the three-slot arithmetic
+        assert a.batch_size == b.batch_size == len(texts)
+        flips = 0
+        for i in range(len(texts)):
+            assert abs(a.intent_results[i].confidence - b.intent_results[i].confidence) < 1e-5
+            assert abs(a.security_results[i].confidence - b.security_results[i].confidence) < 1e-5
+            assert abs(a.pii_results[i].confidence - b.pii_results[i].confidence) < 1.5e-5
+            flips += a.intent_results[i].category != b.intent_results[i].category
+            flips += a.security_results[i].threat_type != b.security_results[i].threat_type
+        assert flips == 0
+        print(f"launches for {len(texts)} texts: shared pass {res['1'][2]}, three slots {res['0'][2]}")
+        assert res["1"][2] < res["0"][2]
         for r, L, _ in res.values():
             L.free_lora_batch_result(r)
     finally:

@@ -182,8 +182,8 @@ int sr_checkpoint_has_adapters(const char* dir) {
 struct MockShared { int tasks; };
 static std::mutex g_shared_mu;
 static std::vector<std::pair<const sr_model*, int>> g_shared;   // models loaded by sr_model_load_lora_shared -> tasks
-int sr_model_load_lora_shared(const char* const* dirs, const int* token_level, int n, int mode, int device, sr_model** out) {
-  if (!dirs || n <= 0 || !out || mode < 0 || mode > 1 || device < 0 || device >= sr_device_count()) return -1;
+int sr_model_load_lora_shared(const char* const* dirs, const int* token_level, int n, int device, sr_model** out) {
+  if (!dirs || n <= 0 || !out || device < 0 || device >= sr_device_count()) return -1;
   sr_model* m = nullptr;
   if (sr_model_load(dirs[0], device, &m) != 0) return -1;
   m->heads.clear();

@@ -1,6 +1,6 @@
 """Secondary measurement (SURVEY section 8 f3): three LoRA tasks (intent / PII tokens / security) over ONE ModernBERT-base --
-a batch through the shared-base pass (sr_classify_lora_shared_ids: one encoder pass over three copies of the rows, rank-16
-terms inside the projection GEMMs) against the three-slot path (three models with the adapters folded at load, three passes),
+a batch through the shared-base pass (sr_classify_lora_shared_ids: one encoder pass over three copies of the rows, each
+256-row block of a projection GEMM multiplied with its task's merged weights) against the three-slot path (three models with the adapters folded at load, three passes),
 through the host-buffer C ABI.  Synthetic weights; prints one JSON line."""
 import json, os, sys, tempfile, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -31,8 +31,7 @@ if not os.path.exists(os.path.join(root, ".complete")):
         json.dump({"rank": RANK, "alpha": ALPHA}, open(os.path.join(dirs[t], "lora_config.json"), "w"))
     open(os.path.join(root, ".complete"), "w").write("ok")
 
-shared = pkg.LoraSharedModel(dirs, [t[1] for t in TASKS], device=0, mode=0)
-grouped = pkg.LoraSharedModel(dirs, [t[1] for t in TASKS], device=0, mode=1)
+shared = pkg.LoraSharedModel(dirs, [t[1] for t in TASKS], device=0)
 slots = [pkg.Model(d, device=0) for d in dirs]
 rng = np.random.default_rng(7)
 
@@ -52,18 +51,14 @@ def timed(fn, n):
 
 
 out = {"workload": f"ModernBERT-base (22 layers), 3 LoRA tasks rank {RANK} on Wqkv / Wo / Wi / Wo-mlp, host-buffer C ABI",
-       "weights_resident": {"shared_pass (low-rank)": "one base + 3 x 4 x 22 rank-16 factor pairs", "grouped_pass": "base + three merged copies of the projections, stacked", "three_slots": "three merged models"}}
+       "weights_resident": {"shared_pass": "base + three merged copies of the projections, stacked", "three_slots": "three merged models"}}
 for B, S, n in ((1, 128, 200), (1, 512, 200), (8, 512, 60), (64, 512, 20)):
     seqs = [rng.integers(5, cfg.vocab_size, size=S, dtype=np.int32) for _ in range(B)]
     a = timed(lambda: shared.classify_shared_ids(seqs), n)
-    g = timed(lambda: grouped.classify_shared_ids(seqs), n)
     b = timed(lambda: three(seqs), n)
     ref = three(seqs)
     probs, _, _ = shared.classify_shared_ids(seqs)
     dmax = max(float(np.abs(probs[t] - ref[t]["probs"]).max()) for t in range(3))
-    probs, _, _ = grouped.classify_shared_ids(seqs)
-    gmax = max(float(np.abs(probs[t] - ref[t]["probs"]).max()) for t in range(3))
-    out[f"b{B}_s{S}"] = {"shared_pass": a, "grouped_pass": g, "three_slots": b, "speedup_p50": round(b["p50_ms"] / a["p50_ms"], 2),
-                         "speedup_grouped_p50": round(b["p50_ms"] / g["p50_ms"], 2), "max_dprob_between_paths": dmax,
-                         "max_dprob_grouped_vs_three_slots": gmax}
+    out[f"b{B}_s{S}"] = {"shared_pass": a, "three_slots": b, "speedup_p50": round(b["p50_ms"] / a["p50_ms"], 2),
+                         "max_dprob_vs_three_slots": dmax}
 print(json.dumps(out))
