@@ -34,7 +34,8 @@ SR_API int sr_test_gemm_resid_hl(const void* a_f16, const void* w_f16, void* hi_
                                  const float* bias, float* row_stats, float* pivot_out, const float* pivot_in,
                                  const float* pivot_in_stats);
 /* The thread-block cluster the GEMM launches for (epilogue, N, K): cluster_n CTAs on neighbouring column tiles of one row
- * block share each A k-block (1: no clusters); workers = clusters of its persistent grid on this device. */
+ * block share each A k-block (1: no clusters); workers = clusters of its persistent grid on this device (null: only
+ * cluster_n, which needs no device). */
 SR_API int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers);
 /* Every field of the GEMM descriptor (csrc/gemm.h GemmDesc, same names and meaning; epi = GemmEpilogue value).  Zeroed
  * fields take GemmDesc's defaults.  EPI_ROPE / EPI_GEGLU with fold_stats (weights: W diag(gamma) with zero-sum rows)

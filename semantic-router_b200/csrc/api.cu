@@ -555,8 +555,9 @@ int sr_test_gemm_resid_hl(const void* a, const void* w, void* hi, void* lo, int 
   return gemm_f16(nullptr, g);
 }
 int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers) {
-  if (!cluster_n || !workers) return -1;
+  if (!cluster_n) return -1;
   *cluster_n = gemm_cluster_size(epi, n, k);
+  if (!workers) return 0;   // the host-side rule alone: no device needed
   *workers = gemm_cluster_workers(epi, n, k);
   return *workers > 0 ? 0 : -1;
 }

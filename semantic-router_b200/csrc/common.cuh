@@ -183,6 +183,7 @@ __device__ __forceinline__ uint32_t box_off(int r, int c) { return static_cast<u
 __device__ __forceinline__ void sts16(uint8_t* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   *reinterpret_cast<uint4*>(p) = make_uint4(a, b, c, d);
 }
+__device__ __forceinline__ void sts_b32(uint8_t* p, uint32_t a) { *reinterpret_cast<uint32_t*>(p) = a; }
 
 
 // ------------------------------------------------------------------------------------------

@@ -124,6 +124,35 @@ __device__ __forceinline__ void wgmma_m64n128k16(float* d, uint64_t da, uint64_t
       : "l"(da), "l"(db), "r"(accumulate)
       : "memory");
 }
+// D[64 x 192] (+)= A[64 x 16] * B[192 x 16]^T: the same fragment layout as m64n128k16, with j = 0..23 (gemm_wide_kernel)
+__device__ __forceinline__ void wgmma_m64n192k16(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %98, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+      "%96, %97, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
+}
+
 // Byte offset of fp32 column `col` of row `row` in the shared accumulator tile: [BM][BN] fp32 rows, 16-byte units
 // XOR-swizzled by (row & 7) inside each 128-byte group, so that a warp reading one row per lane (8 units each) and the
 // MMA warpgroup writing its fragments both stay at the minimum number of shared-memory wavefronts.
@@ -731,6 +760,259 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   else __syncthreads();
 }
 
+// ================= the LayerNorm-fold projections (EPI_ROPE, EPI_GEGLU) on 128 x 192 tiles =================
+// gemm_kernel hands every 128 x 128 accumulator tile through 64 KB of shared memory to separate epilogue warps; for the
+// two large projections that hand-off, and the single MMA warpgroup that stalls on it, cost about a quarter of the
+// GEMM.  gemm_wide_kernel instead runs
+//   * warps 0..7 : two MMA warpgroups; warpgroup w owns rows 64 w .. 64 w + 63 of the tile: m64n192k16 per k-step,
+//     then the epilogue straight from its accumulator fragment (fold rstd, RoPE or GeGLU, fp16 pack) into a swizzled
+//     16-row box per warp, stored by TMA.
+//   * warp 8     : TMA producer; it fills the ring for the next tile while the warpgroups run the epilogue.
+// 288 threads: nine warps, three on one SM sub-partition, so ptxas allocates at most 16384 / 96 -> 168 registers per
+// thread.  The 96 accumulators and the epilogue fit in that without spilling (-Xptxas -v: 166-168).
+// The schedule (persistent contiguous ranges, 1 x cn clusters multicasting A, grouped weights, PDL), the per-element
+// accumulation over K and the epilogue expressions are those of gemm_kernel: the results are bitwise the same.
+// 192 = three 64-wide heads, and in the fragment columns c and c + 32 sit in the same thread, which is the pairing of
+// both rotate-half RoPE and the 32-row (a | b) interleave of the GeGLU weights.
+constexpr int BNW = 192;
+constexpr int kWideThreads = 32 * 9;
+
+template <int EPI>
+struct WideCfg {
+  static constexpr int kABytes = BM * BK * 2;
+  static constexpr int kBBytes = BNW * BK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  // output box per warp and 64-column accumulator group: 16 rows x 64 fp16 (RoPE, 128B swizzle) or x 32 fp16 (GeGLU's
+  // halved width, 64B swizzle)
+  static constexpr int kBoxCols = EPI == EPI_GEGLU ? 32 : 64;
+  static constexpr int kBoxBytes = 16 * kBoxCols * 2;
+  static constexpr int kEpiBytes = 8 * 3 * kBoxBytes;
+  static constexpr int kFit = (kSmemLimit - kEpiBytes - 1024 /*align slack*/ - kBarrierBytes) / kStageBytes;
+  static constexpr int kStages = kFit < 6 ? kFit : 6;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 + kBarrierBytes;
+  static_assert(kStages >= 3, "mainloop ring too shallow");
+};
+
+template <int EPI, int CN>
+__global__ void __launch_bounds__(kWideThreads, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap /*unused*/,
+                 const KArgs p) {
+  static_assert(EPI == EPI_ROPE || EPI == EPI_GEGLU, "the wide kernel serves the LayerNorm-fold projections");
+  using Cfg = WideCfg<EPI>;
+  static_assert(Cfg::kSmemBytes <= kSmemLimit, "over the 227 KB shared-memory opt-in limit");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;
+  uint8_t* smem_epi = smem + Cfg::kStages * Cfg::kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_epi + Cfg::kEpiBytes);
+  uint64_t* empty_bar = full_bar + Cfg::kStages;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int m_blocks = (p.M + BM - 1) / BM;
+  const int n_blocks = (p.N + BNW - 1) / BNW;
+  const int k_blocks = (p.K + BK - 1) / BK;
+  // cluster tiles and contiguous ranges exactly as gemm_kernel (see there)
+  constexpr int cn = CN;
+  const int rn = blockIdx.x % cn;
+  const int n_cblocks = (n_blocks + cn - 1) / cn;
+  const int num_tiles = m_blocks * n_cblocks;
+  const int num_workers = gridDim.x / cn;
+  const int base = num_tiles / num_workers, rem = num_tiles % num_workers;
+  const int bid = blockIdx.x / cn;
+  const int t_begin = bid * base + (bid < rem ? bid : rem);
+  const int t_end = t_begin + base + (bid < rem ? 1 : 0);
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_out);
+#pragma unroll
+    for (int s = 0; s < Cfg::kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8 * cn);   // one arrival per MMA warp of every CTA of the cluster
+    }
+    mbar_fence_init();
+  }
+  if constexpr (CN > 1) cluster_sync();
+  else __syncthreads();
+  griddep_launch_dependents();
+  griddep_wait();
+
+  if (warp == 8) {
+    // ================= TMA producer =================
+    if (lane == 0) {
+      int s = 0;
+      uint32_t ph = 0;
+      const int a_rows = BM / cn;
+      const uint16_t a_mask = static_cast<uint16_t>((1u << cn) - 1);
+      for (int t = t_begin; t < t_end; ++t) {
+        const int m_blk = t / n_cblocks, n_blk = (t % n_cblocks) * cn + rn;
+        const int w_row0 = p.grp_rows > 0 ? ((m_blk * BM) / p.grp_rows) * p.N : 0;
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          const int kc = kb * BK;
+          mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
+          uint8_t* da = smem_a + s * Cfg::kABytes + rn * a_rows * (BK * 2);
+          const int ya = m_blk * BM + rn * a_rows;
+          if (cn > 1) tma_load_2d_multicast(da, &tmap_a, &full_bar[s], kc, ya, a_mask);
+          else tma_load_2d(da, &tmap_a, &full_bar[s], kc, ya);
+          tma_load_2d(smem_b + s * Cfg::kBBytes, &tmap_b, &full_bar[s], kc, w_row0 + n_blk * BNW);
+          if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ================= MMA warpgroups, epilogue from the accumulator fragment =================
+    const int wg = warp >> 2;         // 64-row half of the tile
+    const int wq = warp & 3;          // fragment rows 16 wq .. 16 wq + 15 of that half
+    const int q = lane & 3;
+    const int fr = lane >> 2;         // this thread's rows: fr and fr + 8 of the warp's 16
+    const bool fold = p.fold_stats != nullptr;
+    const int n_out = (EPI == EPI_GEGLU) ? p.N / 2 : p.N;
+    uint8_t* my_boxes = smem_epi + warp * 3 * Cfg::kBoxBytes;
+    float acc[96];
+    float rstd[2] = {1.f, 1.f};   // per row of the thread: the fold's rstd and (EPI_ROPE) the position
+    int pos[2] = {0, 0};
+    int row_mblk = -1;
+    int s = 0;
+    uint32_t ph = 0;
+    auto release = [&](int st) {
+      if (cn == 1) {
+        if (lane == 0) mbar_arrive(&empty_bar[st]);
+      } else if (lane < cn) {
+        mbar_arrive_cluster(&empty_bar[st], lane);
+      }
+    };
+    for (int t = t_begin; t < t_end; ++t) {
+      const int m_blk = t / n_cblocks, n_blk = (t % n_cblocks) * cn + rn;
+      const int row0 = m_blk * BM + 64 * wg + 16 * wq;   // first row of this warp's boxes
+      if (m_blk != row_mblk) {   // per-row state (the same expressions as gemm_kernel)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + fr + 8 * h < p.M ? row0 + fr + 8 * h : p.M - 1;   // rows past M: never stored
+          if (fold) {
+            float s1 = 0.f, s2 = 0.f;
+            for (int k = 0; k < p.fold_parts; ++k) {
+              const float2 st = __ldg(reinterpret_cast<const float2*>(p.fold_stats) + static_cast<size_t>(k) * p.M + row);
+              s1 += st.x;
+              s2 += st.y;
+            }
+            const float mean = s1 * p.fold_inv_h;
+            const float var = fmaxf(s2 * p.fold_inv_h - mean * mean, 0.f);
+            rstd[h] = rsqrtf(var + p.fold_eps);
+          }
+          if constexpr (EPI == EPI_ROPE) {
+            if (p.rope_cols > 0) pos[h] = __ldg(p.pos + row);
+          }
+        }
+        row_mblk = m_blk;
+      }
+      int prev = -1;
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait(&full_bar[s], ph);
+        wgmma_fence();
+        const uint32_t a0 = smem_u32(smem_a + s * Cfg::kABytes) + wg * 64 * 128;
+        const uint32_t b0 = smem_u32(smem_b + s * Cfg::kBBytes);
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_m64n192k16(acc, gmma_desc_sw128(a0 + 32 * k), gmma_desc_sw128(b0 + 32 * k), (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        __syncwarp();
+        if (prev >= 0) release(prev);
+        prev = s;
+        if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (prev >= 0) release(prev);
+
+      const bool rotate = EPI == EPI_ROPE && n_blk * BNW < p.rope_cols;   // the tile holds rotated (q, k) heads
+      // this warp's boxes of the previous tile have been read out by the TMA unit
+      if (lane == 0) bulk_wait_read<0>();
+      __syncwarp();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {   // the thread's two rows
+        const int br = fr + 8 * h;     // row inside the boxes
+        // EPI_ROPE: cos / sin of the row's first-half head columns 8 jj + 2 q + {0, 1}, carrying its rstd -- loaded once
+        // per row and tile, after the mainloop.  Holding them across the mainloop, or both rows' at once, spills: at 288
+        // threads ptxas gives this kernel 168 registers (three of the nine warps share a sub-partition: 16384 / 96), and
+        // the 96 accumulators take most of them.
+        float c[EPI == EPI_ROPE ? 8 : 1], sv[EPI == EPI_ROPE ? 8 : 1];
+        if constexpr (EPI == EPI_ROPE) {
+          if (rotate) {
+            const float2* c2 = reinterpret_cast<const float2*>(p.rope_cos + static_cast<size_t>(pos[h]) * 32);
+            const float2* s2 = reinterpret_cast<const float2*>(p.rope_sin + static_cast<size_t>(pos[h]) * 32);
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const float2 cv = __ldg(c2 + 4 * jj + q), svv = __ldg(s2 + 4 * jj + q);
+              c[2 * jj] = cv.x; c[2 * jj + 1] = cv.y;
+              sv[2 * jj] = svv.x; sv[2 * jj + 1] = svv.y;
+            }
+            if (fold) {   // LayerNorm fold: the rstd factor of the row rides on the (linear) rotation
+#pragma unroll
+              for (int i = 0; i < 8; ++i) { c[i] *= rstd[h]; sv[i] *= rstd[h]; }
+            }
+          }
+        }
+#pragma unroll
+        for (int g = 0; g < 3; ++g) {   // 64-column accumulator group: one head (RoPE) or one (a | b) pair of 32 (GeGLU)
+          uint8_t* box = my_boxes + g * Cfg::kBoxBytes;
+          const int col0 = n_blk * BNW + 64 * g;
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            // columns 64 g + 8 jj + 2 q + {0, 1} (a) and the same + 32 (b) of the tile: fragment entries j, j + 4
+            const int ja = 8 * g + jj, jb = ja + 4;
+            const float a0 = acc[4 * ja + 2 * h], a1 = acc[4 * ja + 2 * h + 1];
+            const float b0 = acc[4 * jb + 2 * h], b1 = acc[4 * jb + 2 * h + 1];
+            if constexpr (EPI == EPI_ROPE) {
+              uint32_t oa, ob;
+              if (rotate && col0 < p.rope_cols) {   // q and k heads: rotate-half over the 64-wide head
+                oa = pack_half2(a0 * c[2 * jj] - b0 * sv[2 * jj], a1 * c[2 * jj + 1] - b1 * sv[2 * jj + 1]);
+                ob = pack_half2(a0 * sv[2 * jj] + b0 * c[2 * jj], a1 * sv[2 * jj + 1] + b1 * c[2 * jj + 1]);
+              } else if (fold) {   // v columns: no rotation to carry rstd
+                oa = pack_half2(a0 * rstd[h], a1 * rstd[h]);
+                ob = pack_half2(b0 * rstd[h], b1 * rstd[h]);
+              } else {
+                oa = pack_half2(a0, a1);
+                ob = pack_half2(b0, b1);
+              }
+              sts_b32(box + br * 128 + ((jj ^ (br & 7)) << 4) + 4 * q, oa);
+              sts_b32(box + br * 128 + (((jj + 4) ^ (br & 7)) << 4) + 4 * q, ob);
+            } else {
+              const float rs = fold ? rstd[h] : 1.0f;
+              const float kz = rs * 0.70710678118654752440f, kh = 0.5f * rs * rs;
+              const float g0 = geglu_fold_f(a0, b0, kz, kh);
+              const float g1 = geglu_fold_f(a1, b1, kz, kh);
+              sts_b32(box + br * 64 + ((jj ^ ((br >> 1) & 3)) << 4) + 4 * q, pack_half2(g0, g1));
+            }
+          }
+        }
+      }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) {
+#pragma unroll
+        for (int g = 0; g < 3; ++g) {
+          // output columns of the group; a group wholly past N (a partial last tile) is not stored, rows >= M and
+          // columns >= n_out inside a box are clipped by the TMA unit
+          const int ocol0 = EPI == EPI_GEGLU ? n_blk * (BNW / 2) + 32 * g : n_blk * BNW + 64 * g;
+          if (ocol0 < n_out) tma_store_2d(&tmap_out, my_boxes + g * Cfg::kBoxBytes, ocol0, row0);
+        }
+        bulk_commit();
+      }
+    }
+    if (lane == 0) bulk_wait_read<0>();   // smem must outlive the last stores' reads
+    __syncwarp();
+  }
+  if constexpr (CN > 1) cluster_sync();
+  else __syncthreads();
+}
+
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
@@ -752,20 +1034,34 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// Clusters of CN CTAs of gemm_kernel<EPI, CN> that are co-resident on the device.  A GPC holds a whole number of
-// clusters, so this is the occupancy query's answer, not num_sms / CN.  Asked once per epilogue and cluster size
+// The kernel gemm_f16 launches for an epilogue, cluster size and tile width (WIDE: gemm_wide_kernel), with its shared
+// memory and block size.
+template <int EPI, int CN, bool WIDE>
+struct Kernel {
+  static constexpr auto fn() {
+    if constexpr (WIDE) return gemm_wide_kernel<EPI, CN>;
+    else return gemm_kernel<EPI, CN>;
+  }
+  static constexpr int kSmem = WIDE ? WideCfg<EPI>::kSmemBytes : GemmCfg<EPI>::kSmemBytes;
+  static constexpr int kThreads = WIDE ? kWideThreads : kGemmThreads;
+  static constexpr int kBN = WIDE ? BNW : BN;
+};
+
+// Clusters of CN CTAs of the kernel that are co-resident on the device.  A GPC holds a whole number of
+// clusters, so this is the occupancy query's answer, not num_sms / CN.  Asked once per kernel and cluster size
 // (all devices of one box are the same part).
-template <int EPI, int CN>
+template <int EPI, int CN, bool WIDE = false>
 int max_clusters(int num_sms) {
+  using Kn = Kernel<EPI, CN, WIDE>;
   constexpr int csize = CN;
   static std::atomic<int> cached{0};
   int n = cached.load(std::memory_order_relaxed);
   if (n > 0) return n;
-  SRB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<EPI, CN>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<EPI>::kSmemBytes));
+  SRB_CUDA_CHECK(cudaFuncSetAttribute(Kn::fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::kSmem));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(csize * num_sms);
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = GemmCfg<EPI>::kSmemBytes;
+  cfg.blockDim = dim3(Kn::kThreads);
+  cfg.dynamicSmemBytes = Kn::kSmem;
   cudaLaunchAttribute attr;
   attr.id = cudaLaunchAttributeClusterDimension;
   attr.val.clusterDim.x = csize;
@@ -773,7 +1069,7 @@ int max_clusters(int num_sms) {
   attr.val.clusterDim.z = 1;
   cfg.attrs = &attr;
   cfg.numAttrs = 1;
-  SRB_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&n, gemm_kernel<EPI, CN>, &cfg));
+  SRB_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&n, Kn::fn(), &cfg));
   if (n <= 0) {
     fprintf(stderr, "[srb200] gemm_f16: no %d-CTA cluster of this kernel fits the device\n", csize);
     return -1;
@@ -782,17 +1078,17 @@ int max_clusters(int num_sms) {
   return n;
 }
 
-template <int EPI, int CN = 1>
+template <int EPI, int CN = 1, bool WIDE = false>
 int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
            const CUtensorMap& tx, const KArgs& ka, int num_sms, int grid_override = 0) {
-  using Cfg = GemmCfg<EPI>;
+  using Kn = Kernel<EPI, CN, WIDE>;
   // per-device attribute; cheap enough to set on every launch (multi-GPU processes switch devices)
-  SRB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<EPI, CN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+  SRB_CUDA_CHECK(cudaFuncSetAttribute(Kn::fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::kSmem));
   constexpr int csize = CN;
-  const int tiles = ((ka.M + BM - 1) / BM) * ((ka.N + BN * csize - 1) / (BN * csize));   // cluster tiles
+  const int tiles = ((ka.M + BM - 1) / BM) * ((ka.N + Kn::kBN * csize - 1) / (Kn::kBN * csize));   // cluster tiles
   cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.blockDim = dim3(Kn::kThreads);
+  cfg.dynamicSmemBytes = Kn::kSmem;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   int nattr = 0;
@@ -807,14 +1103,14 @@ int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, co
     attr[nattr].val.clusterDim.x = csize;
     attr[nattr].val.clusterDim.y = 1;
     attr[nattr++].val.clusterDim.z = 1;
-    workers = max_clusters<EPI, CN>(num_sms);
+    workers = max_clusters<EPI, CN, WIDE>(num_sms);
     if (workers <= 0) return -1;
   }
   const int grid = grid_override > 0 ? grid_override : csize * (tiles < workers ? tiles : workers);
   cfg.gridDim = dim3(grid);
   cfg.attrs = attr;
   cfg.numAttrs = nattr;
-  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<EPI, CN>, ta, tb, tc, tx, ka));
+  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, Kn::fn(), ta, tb, tc, tx, ka));
   note_launch();
   return 0;
 }
@@ -822,7 +1118,8 @@ int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, co
 }  // namespace
 
 static int make_tmap_2d(CUtensorMap* out, CUtensorMapDataType dt, int elem_bytes, const void* ptr, uint64_t cols,
-                        uint64_t rows, uint64_t ld_elems, uint32_t box_cols, uint32_t box_rows) {
+                        uint64_t rows, uint64_t ld_elems, uint32_t box_cols, uint32_t box_rows,
+                        CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
     fprintf(stderr, "[srb200] cuTensorMapEncodeTiled entry point unavailable\n");
@@ -833,7 +1130,7 @@ static int make_tmap_2d(CUtensorMap* out, CUtensorMapDataType dt, int elem_bytes
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, dt, 2, const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     fprintf(stderr, "[srb200] cuTensorMapEncodeTiled failed: %d (cols=%llu rows=%llu ld=%llu box=%ux%u)\n", (int)r,
             (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)ld_elems, box_cols, box_rows);
@@ -860,11 +1157,21 @@ int make_tmap_f16_kmajor(CUtensorMap* out, const void* ptr, uint64_t rows, uint6
 // projections use them.  The residual GEMMs, whose time goes to the fp16-pair epilogue rather than the operand feed,
 // run without clusters; so do the epilogues not measured here (EPI_F16, EPI_GELU, EPI_RESID) and EPI_TOPK, whose
 // grouped schedule gives each worker its own query block.  A pair is only formed when the column tiles pair up
-// exactly: with an odd N / 128 every other cluster would carry a CTA that computes a tile wholly past N.
+// exactly, in both tile widths these projections can run at (128: gemm_kernel, 192: gemm_wide_kernel): with an odd
+// tile count every other cluster would carry a CTA that computes a tile wholly past N.
 int gemm_cluster_size(int epi, int N, int K) {
   (void)K;
   const bool share_a = epi == EPI_ROPE || epi == EPI_GEGLU;
-  return share_a && ((N + BN - 1) / BN) % 2 == 0 ? 2 : 1;
+  return share_a && ((N + BN - 1) / BN) % 2 == 0 && ((N + BNW - 1) / BNW) % 2 == 0 ? 2 : 1;
+}
+
+// EPI_ROPE and EPI_GEGLU run on gemm_wide_kernel; SRB_GEMM_WIDE=0 puts them back on gemm_kernel (A/B measurements and
+// the bitwise comparison of the two kernels).  Read once per process.  gemm_cluster_size does not look at it: at an N
+// whose 128-wide tiles pair but 192-wide ones do not (512, 1280, ...) the 128 x 128 kernel then runs unclustered --
+// another schedule than it had on its own, the same results.
+static bool gemm_wide() {
+  static const bool on = [] { const char* e = getenv("SRB_GEMM_WIDE"); return !(e && e[0] == '0'); }();
+  return on;
 }
 
 static int device_sms() {
@@ -883,8 +1190,8 @@ int gemm_cluster_workers(int epi, int N, int K) {
   const int num_sms = device_sms();
   if (num_sms <= 0 || cn == 1) return num_sms;
   // gemm_cluster_size forms pairs for these two epilogues only
-  if (epi == EPI_ROPE) return max_clusters<EPI_ROPE, 2>(num_sms);
-  if (epi == EPI_GEGLU) return max_clusters<EPI_GEGLU, 2>(num_sms);
+  if (epi == EPI_ROPE) return gemm_wide() ? max_clusters<EPI_ROPE, 2, true>(num_sms) : max_clusters<EPI_ROPE, 2>(num_sms);
+  if (epi == EPI_GEGLU) return gemm_wide() ? max_clusters<EPI_GEGLU, 2, true>(num_sms) : max_clusters<EPI_GEGLU, 2>(num_sms);
   return -1;
 }
 
@@ -916,6 +1223,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   const int num_sms = device_sms();
   if (num_sms <= 0) return -1;
   const int cn = gemm_cluster_size(g.epi, g.N, g.K);
+  const bool wide = (g.epi == EPI_ROPE || g.epi == EPI_GEGLU) && gemm_wide();
   // operand boxes: each CTA of a cluster loads 1/cn of the A box (kernel: TMA producer)
   CUtensorMap ta, tb, tc;
   if (make_tmap_f16_kmajor(&ta, g.A, static_cast<uint64_t>(g.a_rows > 0 ? g.a_rows : g.M), g.K, BM / cn)) return -1;
@@ -924,7 +1232,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
     fprintf(stderr, "[srb200] gemm_f16: grouped weights need w_group_rows %% %d == 0 and whole column tiles\n", BM);
     return -1;
   }
-  if (make_tmap_f16_kmajor(&tb, g.W, static_cast<uint64_t>(g.N) * w_groups, g.K, BN)) return -1;
+  if (make_tmap_f16_kmajor(&tb, g.W, static_cast<uint64_t>(g.N) * w_groups, g.K, wide ? BNW : BN)) return -1;
   // output boxes: 32 rows x 128 bytes (64 fp16 or 32 fp32 columns), clipped at M rows / n_out columns
   if (g.epi == EPI_TOPK) {
     tc = ta;   // no matrix output
@@ -932,6 +1240,12 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
     if (make_tmap_2d(&tc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.out, g.N, g.M, g.ldo, 32, 32)) return -1;
   } else if (is_hl) {
     if (make_tmap_2d(&tc, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.out, g.N, g.M, g.N, 64, 32)) return -1;
+  } else if (wide) {
+    // gemm_wide_kernel: one box per warp (16 rows) and 64-column accumulator group (see WideCfg)
+    const bool geglu = g.epi == EPI_GEGLU;
+    if (make_tmap_2d(&tc, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.out, geglu ? g.N / 2 : g.N, g.M, g.ldo, geglu ? 32 : 64, 16,
+                     geglu ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B))
+      return -1;
   } else {
     const uint64_t n_out = g.epi == EPI_GEGLU ? g.N / 2 : g.N;
     if (make_tmap_2d(&tc, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.out, n_out, g.M, g.ldo, 64, 32)) return -1;
@@ -966,11 +1280,17 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   switch (g.epi) {
     case EPI_F16: return launch<EPI_F16>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_ROPE:
+      if (wide)
+        return cn == 2 ? launch<EPI_ROPE, 2, true>(stream, ta, tb, tc, tx, ka, num_sms)
+                       : launch<EPI_ROPE, 1, true>(stream, ta, tb, tc, tx, ka, num_sms);
       return cn == 2 ? launch<EPI_ROPE, 2>(stream, ta, tb, tc, tx, ka, num_sms)
                      : launch<EPI_ROPE>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_RESID: return launch<EPI_RESID>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_RESID_HL: return launch<EPI_RESID_HL>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_GEGLU:
+      if (wide)
+        return cn == 2 ? launch<EPI_GEGLU, 2, true>(stream, ta, tb, tc, tx, ka, num_sms)
+                       : launch<EPI_GEGLU, 1, true>(stream, ta, tb, tc, tx, ka, num_sms);
       return cn == 2 ? launch<EPI_GEGLU, 2>(stream, ta, tb, tc, tx, ka, num_sms)
                      : launch<EPI_GEGLU>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_GELU: return launch<EPI_GELU>(stream, ta, tb, tc, tx, ka, num_sms);
