@@ -4,19 +4,22 @@
 //
 // Replaces the dense f32 `gemm`+rayon matmuls behind candle's Linear on the reference's hot loop
 // (candle-binding/src/model_architectures/traditional/candle_models/modernbert.rs
-//  :123 Wqkv, :196 Wo, :236-238 Wi/GeGLU/Wo) with one kernel family on 128 x 128 tiles:
-//   * warp 8      : TMA producer  (cp.async.bulk.tensor 2D, 128B swizzle, mbarrier complete_tx)
-//   * warps 4..7  : one MMA warpgroup -- wgmma.mma_async m64n128k16 twice per k-step (rows 0-63, 64-127), fp32
-//                   accumulators in registers; at the end of a tile they go to a swizzled fp32 tile in shared memory
-//   * warps 0..3  : epilogue (shared fp32 tile -> registers, one row per lane -> fused math -> swizzled box -> TMA store)
-//   * the accumulator tile in shared memory is the hand-off: the epilogue of tile i overlaps the mainloop of tile i+1,
-//     whose accumulators live in the MMA warpgroup's registers until the epilogue has released the shared tile.
-//   * thread-block clusters (gemm_cluster_size): the cn CTAs of a cluster compute neighbouring column tiles of one row
-//     block; each loads a 1/cn slice of the shared A box and multicasts it (TMA .multicast::cluster), and frees a
-//     stage by arriving on the empty barrier of every CTA that wrote into it.  Tiles, the wgmma sequence,
-//     the accumulation order and the epilogues are the same as without clusters: results are bitwise identical.
-// Fused epilogues: bias, RoPE (rotate-half, modernbert.rs:61-85), fp32 residual add (:300-303),
-// GeGLU = gelu_erf(a)*b (:238), erf-GELU (BERT intermediate).
+//  :123 Wqkv, :196 Wo, :236-238 Wi/GeGLU/Wo) with two persistent kernels:
+//   * gemm_kernel, 128 x 128 tiles: EPI_F16 (bias), EPI_RESID (fp32 residual add, :300-303), EPI_GELU (erf-GELU, BERT
+//     intermediate), EPI_TOPK (the cache scan) and EPI_RESID_HL (the fp16-pair residual stream)
+//     - warp 8      : TMA producer  (cp.async.bulk.tensor 2D, 128B swizzle, mbarrier complete_tx)
+//     - warps 4..7  : one MMA warpgroup -- wgmma.mma_async m64n128k16 twice per k-step (rows 0-63, 64-127), fp32
+//                     accumulators in registers; at the end of a tile they go to a swizzled fp32 tile in shared memory
+//     - warps 0..3  : epilogue (shared fp32 tile -> registers, one row per lane -> fused math -> swizzled box -> TMA store)
+//     - the accumulator tile in shared memory is the hand-off: the epilogue of tile i overlaps the mainloop of tile i+1,
+//       whose accumulators live in the MMA warpgroup's registers until the epilogue has released the shared tile.
+//   * gemm_wide_kernel, 128 x 192 tiles: the LayerNorm-fold projections, EPI_ROPE (rotate-half, modernbert.rs:61-85)
+//     and EPI_GEGLU (gelu_erf(a)*b, :238), with two MMA warpgroups and the epilogue from their registers (see there).
+//     It is the only kernel that runs in thread-block clusters (gemm_cluster_size): the cn CTAs of a cluster compute
+//     neighbouring column tiles of one row block; each loads a 1/cn slice of the shared A box and multicasts it (TMA
+//     .multicast::cluster), and frees a stage by arriving on the empty barrier of every CTA that wrote into it.  Tiles,
+//     the wgmma sequence, the accumulation order and the epilogues are the same as without clusters: results are
+//     bitwise identical.
 #include "gemm.h"
 
 #include <atomic>
@@ -161,24 +164,11 @@ __device__ __forceinline__ uint32_t acc_off(int row, int col) {
   return static_cast<uint32_t>(row * (BN * 4) + (((u & ~7) | ((u & 7) ^ (row & 7))) << 4) + (col & 3) * 4);
 }
 
-// LayerNorm fold, consumer side.  W'' = (W diag(gamma)) with every row re-centred to sum zero, so that
-// sum_k x[r,k] W''[n,k] = sum_k (x[r,k] - mean_r) W'[n,k]: the mean subtraction of the LayerNorm happens inside the GEMM
-// (the centring matrix I - 11^T/H commutes into the weights) and the epilogue is left with the per-row rstd factor --
-// which the RoPE epilogue folds into the row's cos / sin registers (the rotation is linear), so q and k cost nothing.
-__device__ __forceinline__ void fold_scale(float rstd, uint32_t* a, uint32_t* b) {
-#pragma unroll
-  for (int i = 0; i < 32; ++i) {
-    a[i] = __float_as_uint(__uint_as_float(a[i]) * rstd);
-    b[i] = __float_as_uint(__uint_as_float(b[i]) * rstd);
-  }
-}
-
-// CN: thread-block cluster size -- CN neighbouring column tiles of one row block share A (1: no clusters; a compile-time
-// constant, so that the unclustered instantiations carry none of the cluster arithmetic)
-template <int EPI, int CN>
+template <int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_aux, const KArgs p) {
+  static_assert(EPI != EPI_ROPE && EPI != EPI_GEGLU, "the LayerNorm-fold projections run on gemm_wide_kernel");
   using Cfg = GemmCfg<EPI>;
   static_assert(Cfg::kSmemBytes <= kSmemLimit, "over the 227 KB shared-memory opt-in limit");
   constexpr bool kHL = EPI == EPI_RESID_HL;
@@ -203,34 +193,25 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int m_blocks = (p.M + BM - 1) / BM;
   const int n_blocks = (p.N + BN - 1) / BN;
   const int k_blocks = (p.K + BK - 1) / BK;
-  // Thread-block clusters of cn CTAs along N (1: none).  The schedule below hands out CLUSTER tiles -- cn neighbouring
-  // 128 x 128 tiles of one row block -- and CTA rn of the cluster computes tile (m_c, cn n_c + rn) of cluster tile
-  // (m_c, n_c).  The cn CTAs share the A row block: each loads a 1/cn slice of the A box and multicasts it to all of
-  // them, so an A k-block is read out of L2 once per cluster instead of once per CTA.  All CTAs of a cluster walk the
-  // same cluster tiles and k-blocks in lockstep; a tile past N is still loaded (TMA zero-fills) and computed, and its
-  // stores are skipped.  (Sharing W across row blocks as well was measured slower at every projection shape.)
-  constexpr int cn = CN;
-  const int rn = blockIdx.x % cn;
-  const int n_cblocks = (n_blocks + cn - 1) / cn;
-  const int num_tiles = m_blocks * n_cblocks;   // cluster tiles (= tiles without clusters)
-  auto tile_m = [&](int t) { return t / n_cblocks; };
-  auto tile_n = [&](int t) { return (t % n_cblocks) * cn + rn; };
+  const int num_tiles = m_blocks * n_blocks;
+  auto tile_m = [&](int t) { return t / n_blocks; };
+  auto tile_n = [&](int t) { return t % n_blocks; };
   auto row_base = [&](int m_blk) { return m_blk * BM; };
-  // contiguous tile range per cluster (n fastest): one cluster walks all N tiles of its M blocks back to back, so the
-  // A row-block stays hot in L2 and per-row epilogue state (RoPE cos/sin) is reused across tiles
-  const int num_workers = gridDim.x / cn;
+  // contiguous tile range per worker (n fastest): one worker walks all N tiles of its M blocks back to back, so the
+  // A row-block stays hot in L2 and per-row epilogue state (pivots, top-8 lists) is reused across tiles
+  const int num_workers = gridDim.x;
   const int base = num_tiles / num_workers, rem = num_tiles % num_workers;
-  const int bid = blockIdx.x / cn;   // worker = cluster
+  const int bid = blockIdx.x;
   int t_begin = bid * base + (bid < rem ? bid : rem);
   int t_end = t_begin + base + (bid < rem ? 1 : 0);
   // EPI_TOPK, grouped schedule (p.grouped): worker w owns query block w % m_blocks for its whole life (its running
   // top-8 lists live in registers) and walks the stored-row tiles g, g + G, g + 2G, ... with g = w / m_blocks,
   // G = workers / m_blocks.  The m_blocks workers of a group therefore ask for the SAME stored-row tile at about the
   // same time: one HBM read, the rest L2 hits -- the store streams once per batch instead of once per query block.
-  // Tiles are numbered t = m_blk * n_blocks + n_blk as everywhere else (EPI_TOPK runs without clusters: cluster tiles
-  // are tiles); `t_step` is the distance between two tiles of this worker (1 for the contiguous ranges).
+  // Tiles are numbered t = m_blk * n_blocks + n_blk as everywhere else; `t_step` is the distance between two tiles of
+  // this worker (1 for the contiguous ranges).
   int t_step = 1;
-  // Interleaved schedule (p.interleave; the residual GEMMs): worker (cluster) w takes tiles w, w + W, w + 2W, ...  With
+  // Interleaved schedule (p.interleave; the residual GEMMs): worker w takes tiles w, w + W, w + 2W, ...  With
   // n fastest in the tile numbering the N / BN tiles of one row block run AT THE SAME TIME on neighbouring workers, so
   // each A k-block is pulled from HBM once and hit in L2 by the others, where the contiguous ranges could lose the row
   // block from L2 to the residual stream passing through between two tiles of one worker.
@@ -257,17 +238,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      // one arrival per MMA warp of every CTA this CTA's producer multicasts into: the cn CTAs of its cluster
-      mbar_init(&empty_bar[s], 4 * cn);
+      mbar_init(&empty_bar[s], 4);   // one arrival per MMA warp
     }
     mbar_init(tfull_bar, 128);            // every thread of the MMA warpgroup, after its fragment stores
     mbar_init(tempty_bar, kEpiWarps);
     for (int i = 0; i < kEpiWarps * kStageBufs; ++i) mbar_init(&resid_bar[i], 1);
     mbar_fence_init();
   }
-  // no CTA of the cluster multicasts into another or arrives on its barriers before those barriers exist
-  if constexpr (CN > 1) cluster_sync();
-  else __syncthreads();
+  __syncthreads();
   // PDL: everything above overlapped the previous kernel's tail; nothing below may start before its writes are visible
   griddep_launch_dependents();
   griddep_wait();
@@ -277,10 +255,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     if (lane == 0) {
       int s = 0;
       uint32_t ph = 0;
-      // this CTA's slice of the shared A box (tensor-map box height BM / cn rows, a multiple of the 8-row swizzle atom,
-      // so the slices assemble into exactly the tile layout one full-box load would give), multicast to the whole cluster
-      const int a_rows = BM / cn;
-      const uint16_t a_mask = static_cast<uint16_t>((1u << cn) - 1);
       for (int t = t_begin; t < t_end; t += t_step) {
         const int m_blk = tile_m(t), n_blk = tile_n(t);
         // grouped weights (one matrix per task, stacked along N): the row block picks its matrix; blocks never straddle
@@ -289,12 +263,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         for (int kb = 0; kb < k_blocks; ++kb) {
           mbar_wait(&empty_bar[s], ph ^ 1);
           const int kc = kb * BK;
-          // the stage fills with the A slices of every CTA of the cluster and this CTA's own W box: the whole stage
           mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
-          uint8_t* da = smem_a + s * Cfg::kABytes + rn * a_rows * (BK * 2);
-          const int ya = m_blk * BM + rn * a_rows;
-          if (cn > 1) tma_load_2d_multicast(da, &tmap_a, &full_bar[s], kc, ya, a_mask);
-          else tma_load_2d(da, &tmap_a, &full_bar[s], kc, ya);
+          tma_load_2d(smem_a + s * Cfg::kABytes, &tmap_a, &full_bar[s], kc, m_blk * BM);
           tma_load_2d(smem_b + s * Cfg::kBBytes, &tmap_b, &full_bar[s], kc, w_row0 + n_blk * BN);
           if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
         }
@@ -307,16 +277,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     int s = 0;
     uint32_t ph = 0;
     uint32_t eph = 0;   // tempty phase
-    // a stage of this CTA is written by the producers of every CTA of its cluster (A slices): freeing it is one
-    // arrival on the empty barrier of each of them, lane i for CTA i, so that the arrivals go out side by side on the
-    // MMA warp's critical path
-    auto release = [&](int st) {
-      if (cn == 1) {
-        if (lane == 0) mbar_arrive(&empty_bar[st]);
-      } else if (lane < cn) {
-        mbar_arrive_cluster(&empty_bar[st], lane);
-      }
-    };
     for (int t = t_begin; t < t_end; t += t_step) {
       int prev = -1;
       for (int kb = 0; kb < k_blocks; ++kb) {
@@ -336,13 +296,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         // the previous stage's MMAs have completed once at most this stage's group is pending: free that stage
         wgmma_wait<1>();
         __syncwarp();
-        if (prev >= 0) release(prev);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
         prev = s;
         if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
       }
       wgmma_wait<0>();
       __syncwarp();
-      if (prev >= 0) release(prev);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       // hand the tile to the epilogue once it has read out the previous one
       mbar_wait(tempty_bar, eph ^ 1);
       eph ^= 1;
@@ -362,12 +322,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     // ================= epilogue warps: shared fp32 tile -> registers -> swizzled smem box -> TMA store =================
     const int quad = warp;  // 32-row quarter of the tile this warp owns (one row per lane)
     uint8_t* my_bufs = smem_epi + warp * (kStageBufs * kStageBufBytes);
-    const bool fold = (EPI == EPI_ROPE || EPI == EPI_GEGLU) && p.fold_stats != nullptr;
-    float f_rstd = 1.f;   // fold: rstd of this thread's row
     float pv = 0.f;       // EPI_RESID_HL: the pivot SHIFT of this GEMM for this thread's row
     float pv_prev = 0.f;  // EPI_RESID_HL: the pivot the stored pair is relative to
     int pv_mblk = -1;
-    int fold_mblk = -1;
     uint64_t* my_rbar = resid_bar + warp * kStageBufs;
     uint32_t aph = 0;
     int cb = 0;                 // staging buffer to use next
@@ -382,16 +339,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       }
     };
     // chunk geometry: a chunk is one 32-row x 128-byte output box of this warp
-    constexpr int kAccPerChunk = (EPI == EPI_RESID || EPI == EPI_TOPK) ? 32 : (EPI == EPI_GEGLU ? 128 : 64);  // accumulator columns
-    constexpr int kOutPerChunk = (EPI == EPI_RESID || EPI == EPI_TOPK) ? 32 : 64;                                // output columns
-    constexpr int kChunks = BN / kAccPerChunk;
+    constexpr int kChunkCols = (EPI == EPI_RESID || EPI == EPI_TOPK) ? 32 : 64;   // accumulator = output columns
+    constexpr int kChunks = BN / kChunkCols;
     constexpr int kPairs = kStageBufs / 2;   // EPI_RESID_HL: (hi, lo) box pairs of this warp
-    const int n_out = (EPI == EPI_GEGLU) ? p.N / 2 : p.N;
     const bool use_resid = (EPI == EPI_RESID) && p.has_resid;
 
     // EPI_RESID: residual boxes are TMA-loaded one chunk ahead (flat over (tile, chunk) of this CTA)
-    auto out_col = [&](int t, int c) { return tile_n(t) * (BN / kAccPerChunk * kOutPerChunk) + c * kOutPerChunk; };
-    auto chunk_valid = [&](int t, int c) { return t < t_end && out_col(t, c) < n_out; };
+    auto out_col = [&](int t, int c) { return tile_n(t) * BN + c * kChunkCols; };
+    auto chunk_valid = [&](int t, int c) { return t < t_end && out_col(t, c) < p.N; };
     auto issue_resid = [&](int t, int c, int buf) {  // lane 0 only
       if constexpr (kHL) {   // buf = pair index: hi box, then lo box, one barrier for both
         uint8_t* pb = my_bufs + buf * 2 * kStageBufBytes;
@@ -409,24 +364,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     constexpr int kRing = kHL ? kPairs : kStageBufs;   // residual-load ring: boxes, or box pairs
     constexpr int kAhead = kHL ? 1 : (kStageBufs - 2 > 0 ? kStageBufs - 2 : 1);
     int pf_t = t_begin, pf_c = 0, pf_buf = 0;
-    // a tile wholly past N (the second CTA of a cluster on an odd last column) has no chunk: the epilogue skips it,
-    // and so must the cursor, or it would wait on that tile for good and starve every later tile of its residual
-    auto pf_skip = [&]() { while (pf_t < t_end && out_col(pf_t, 0) >= n_out) pf_t += t_step; };
-    pf_skip();
     auto pf_issue = [&]() {  // lane 0 only
       if (!chunk_valid(pf_t, pf_c)) return;
       issue_resid(pf_t, pf_c, pf_buf);
       if (++pf_buf == kRing) pf_buf = 0;
-      if (++pf_c >= kChunks || !chunk_valid(pf_t, pf_c)) { pf_t += t_step; pf_c = 0; pf_skip(); }
+      if (++pf_c >= kChunks || !chunk_valid(pf_t, pf_c)) { pf_t += t_step; pf_c = 0; }
     };
     if ((use_resid || kHL) && lane == 0) {
 #pragma unroll
       for (int i = 0; i < kAhead; ++i) pf_issue();
     }
-
-    // EPI_ROPE: this thread's cos/sin row, reloaded only when the M block changes
-    float cs[EPI == EPI_ROPE ? 32 : 1], sn[EPI == EPI_ROPE ? 32 : 1];
-    int rope_mblk = -1;
 
     // EPI_TOPK: this thread's running top-8 (descending) over the columns this CTA walks for its current row
     float tk_v[EPI == EPI_TOPK ? kTopK : 1];
@@ -445,48 +392,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       }
     };
     for (int t = t_begin; t < t_end; t += t_step) {
-      const int m_blk = tile_m(t), n_blk = tile_n(t);
+      const int m_blk = tile_m(t);
       const int row0 = row_base(m_blk) + quad * 32;
       if constexpr (EPI == EPI_TOPK) {
         if (m_blk != tk_mblk) {
           if (tk_mblk >= 0) tk_flush(tk_mblk);
           tk_reset();
           tk_mblk = m_blk;
-        }
-      }
-      if constexpr (EPI == EPI_ROPE || EPI == EPI_GEGLU) {
-        if (fold && m_blk != fold_mblk) {
-          const int row = row0 + lane < p.M ? row0 + lane : p.M - 1;
-          float s1 = 0.f, s2 = 0.f;
-          for (int k = 0; k < p.fold_parts; ++k) {   // fixed slice order: reproducible
-            const float2 st = __ldg(reinterpret_cast<const float2*>(p.fold_stats) + static_cast<size_t>(k) * p.M + row);
-            s1 += st.x;
-            s2 += st.y;
-          }
-          const float mean = s1 * p.fold_inv_h;
-          const float var = fmaxf(s2 * p.fold_inv_h - mean * mean, 0.f);
-          f_rstd = rsqrtf(var + p.fold_eps);
-          fold_mblk = m_blk;
-          rope_mblk = -1;   // the row's cos / sin registers carry rstd: reload them for this M block
-        }
-      }
-      if constexpr (EPI == EPI_ROPE) {
-        if (m_blk != rope_mblk && n_blk * BN < p.rope_cols) {
-          const int row = row0 + lane;
-          const int pos = __ldg(p.pos + (row < p.M ? row : p.M - 1));   // rows past M: any valid table row (never stored)
-          const float4* c4 = reinterpret_cast<const float4*>(p.rope_cos + static_cast<size_t>(pos) * 32);
-          const float4* s4 = reinterpret_cast<const float4*>(p.rope_sin + static_cast<size_t>(pos) * 32);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 a = __ldg(c4 + i), b = __ldg(s4 + i);
-            cs[4 * i] = a.x; cs[4 * i + 1] = a.y; cs[4 * i + 2] = a.z; cs[4 * i + 3] = a.w;
-            sn[4 * i] = b.x; sn[4 * i + 1] = b.y; sn[4 * i + 2] = b.z; sn[4 * i + 3] = b.w;
-          }
-          if (fold) {   // LayerNorm fold: the rstd factor of the row rides on the (linear) rotation
-#pragma unroll
-            for (int i = 0; i < 32; ++i) { cs[i] *= f_rstd; sn[i] *= f_rstd; }
-          }
-          rope_mblk = m_blk;
         }
       }
       float st1 = 0.f, st2 = 0.f;   // EPI_RESID_HL: this row's (sum, sum of squares) over the current 128-column slice
@@ -574,7 +486,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll 1
         for (int c = 0; c < kChunks; ++c) {
           const int ocol0 = out_col(t, c);
-          if (ocol0 >= n_out) break;
+          if (ocol0 >= p.N) break;
           uint8_t* hb = my_bufs + cb * 2 * kStageBufBytes;
           uint8_t* lb = hb + kStageBufBytes;
           if (lane == 0) {
@@ -637,7 +549,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll 1
       for (int c = 0; c < ((EPI == EPI_TOPK || kHL) ? 0 : kChunks); ++c) {
         const int ocol0 = out_col(t, c);
-        if (ocol0 >= n_out) break;
+        if (ocol0 >= p.N) break;   // the last column tile of an N % 128 == 64 output is half empty
         uint8_t* buf = my_bufs + cb * kStageBufBytes;
         uint8_t* my_row = buf;  // + box_off(lane, chunk16)
         if (use_resid) {
@@ -691,51 +603,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             for (int i = 0; i < 4; ++i)
               sts16(my_row + box_off(lane, hf * 4 + i), h[4 * i], h[4 * i + 1], h[4 * i + 2], h[4 * i + 3]);
           }
-        } else if constexpr (EPI == EPI_ROPE) {
-          uint32_t r1[32], r2[32];
-          acc_ld32(c * 64, r1);
-          acc_ld32(c * 64 + 32, r2);
-          if (fold && ocol0 >= p.rope_cols) fold_scale(f_rstd, r1, r2);   // v columns: no rotation to carry rstd
-          if (ocol0 < p.rope_cols) {  // q and k heads: rotate-half over the 64-wide head (in place, packed)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float a0 = __uint_as_float(r1[2 * i]), a1 = __uint_as_float(r1[2 * i + 1]);
-              const float b0 = __uint_as_float(r2[2 * i]), b1 = __uint_as_float(r2[2 * i + 1]);
-              r1[i] = pack_half2(a0 * cs[2 * i] - b0 * sn[2 * i], a1 * cs[2 * i + 1] - b1 * sn[2 * i + 1]);
-              r2[i] = pack_half2(a0 * sn[2 * i] + b0 * cs[2 * i], a1 * sn[2 * i + 1] + b1 * cs[2 * i + 1]);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              r1[i] = pack_half2(__uint_as_float(r1[2 * i]), __uint_as_float(r1[2 * i + 1]));
-              r2[i] = pack_half2(__uint_as_float(r2[2 * i]), __uint_as_float(r2[2 * i + 1]));
-            }
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            sts16(my_row + box_off(lane, i), r1[4 * i], r1[4 * i + 1], r1[4 * i + 2], r1[4 * i + 3]);
-            sts16(my_row + box_off(lane, 4 + i), r2[4 * i], r2[4 * i + 1], r2[4 * i + 2], r2[4 * i + 3]);
-          }
-        } else if constexpr (EPI == EPI_GEGLU) {
-          // W rows are pre-interleaved in 32-row groups [a(32j..32j+31) | b(32j..32j+31)]: accumulator columns
-          // [64j, 64j+32) hold `a`, [64j+32, 64j+64) the matching `b`; one output chunk = two such groups
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            uint32_t ra[32], rb[32];
-            acc_ld32(c * 128 + hf * 64, ra);
-            acc_ld32(c * 128 + hf * 64 + 32, rb);
-            const float rs = fold ? f_rstd : 1.0f;
-            const float kz = rs * 0.70710678118654752440f, kh = 0.5f * rs * rs;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float g0 = geglu_fold_f(__uint_as_float(ra[2 * i]), __uint_as_float(rb[2 * i]), kz, kh);
-              const float g1 = geglu_fold_f(__uint_as_float(ra[2 * i + 1]), __uint_as_float(rb[2 * i + 1]), kz, kh);
-              ra[i] = pack_half2(g0, g1);
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              sts16(my_row + box_off(lane, hf * 4 + i), ra[4 * i], ra[4 * i + 1], ra[4 * i + 2], ra[4 * i + 3]);
-          }
         }
         fence_proxy_async_smem();
         __syncwarp();
@@ -755,25 +622,32 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     if (lane == 0) bulk_wait_read<0>();  // smem must outlive the last stores' reads
     __syncwarp();
   }
-  // no CTA leaves while another of its cluster may still arrive on its barriers
-  if constexpr (CN > 1) cluster_sync();
-  else __syncthreads();
+  __syncthreads();
 }
 
 // ================= the LayerNorm-fold projections (EPI_ROPE, EPI_GEGLU) on 128 x 192 tiles =================
-// gemm_kernel hands every 128 x 128 accumulator tile through 64 KB of shared memory to separate epilogue warps; for the
-// two large projections that hand-off, and the single MMA warpgroup that stalls on it, cost about a quarter of the
-// GEMM.  gemm_wide_kernel instead runs
+// gemm_wide_kernel runs
 //   * warps 0..7 : two MMA warpgroups; warpgroup w owns rows 64 w .. 64 w + 63 of the tile: m64n192k16 per k-step,
 //     then the epilogue straight from its accumulator fragment (fold rstd, RoPE or GeGLU, fp16 pack) into a swizzled
-//     16-row box per warp, stored by TMA.
+//     16-row box per warp, stored by TMA.  There is no fp32 hand-off through shared memory to separate epilogue warps:
+//     for these two large projections that hand-off, and the single MMA warpgroup stalling on it, cost about a quarter
+//     of the GEMM.
 //   * warp 8     : TMA producer; it fills the ring for the next tile while the warpgroups run the epilogue.
 // 288 threads: nine warps, three on one SM sub-partition, so ptxas allocates at most 16384 / 96 -> 168 registers per
 // thread.  The 96 accumulators and the epilogue fit in that without spilling (-Xptxas -v: 166-168).
-// The schedule (persistent contiguous ranges, 1 x cn clusters multicasting A, grouped weights, PDL), the per-element
-// accumulation over K and the epilogue expressions are those of gemm_kernel: the results are bitwise the same.
 // 192 = three 64-wide heads, and in the fragment columns c and c + 32 sit in the same thread, which is the pairing of
 // both rotate-half RoPE and the 32-row (a | b) interleave of the GeGLU weights.
+// Schedule: persistent, one contiguous range of tiles per worker (n fastest), so that a worker walks all N tiles of its
+// row blocks back to back, the A row block stays hot in L2 and the per-row state (rstd, positions) is reused.
+// Thread-block clusters of CN CTAs along N (1: none): the schedule hands out CLUSTER tiles -- cn neighbouring tiles of
+// one row block -- and CTA rn of the cluster computes tile (m_c, cn n_c + rn) of cluster tile (m_c, n_c).  The cn CTAs
+// share the A row block: each loads a 1/cn slice of the A box and multicasts it to all of them, so an A k-block is read
+// out of L2 once per cluster instead of once per CTA.  All CTAs of a cluster walk the same cluster tiles and k-blocks in
+// lockstep.  (Sharing W across row blocks as well was measured slower at every projection shape.)
+// LayerNorm fold, consumer side.  W'' = (W diag(gamma)) with every row re-centred to sum zero, so that
+// sum_k x[r,k] W''[n,k] = sum_k (x[r,k] - mean_r) W'[n,k]: the mean subtraction of the LayerNorm happens inside the GEMM
+// (the centring matrix I - 11^T/H commutes into the weights) and the epilogue is left with the per-row rstd factor --
+// which the RoPE epilogue folds into the row's cos / sin (the rotation is linear), so q and k cost nothing.
 constexpr int BNW = 192;
 constexpr int kWideThreads = 32 * 9;
 
@@ -815,7 +689,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int m_blocks = (p.M + BM - 1) / BM;
   const int n_blocks = (p.N + BNW - 1) / BNW;
   const int k_blocks = (p.K + BK - 1) / BK;
-  // cluster tiles and contiguous ranges exactly as gemm_kernel (see there)
+  // cluster tiles and contiguous ranges (see above)
   constexpr int cn = CN;
   const int rn = blockIdx.x % cn;
   const int n_cblocks = (n_blocks + cn - 1) / cn;
@@ -837,6 +711,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     }
     mbar_fence_init();
   }
+  // no CTA of the cluster multicasts into another or arrives on its barriers before those barriers exist
   if constexpr (CN > 1) cluster_sync();
   else __syncthreads();
   griddep_launch_dependents();
@@ -847,14 +722,19 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (lane == 0) {
       int s = 0;
       uint32_t ph = 0;
+      // this CTA's slice of the shared A box (tensor-map box height BM / cn rows, a multiple of the 8-row swizzle atom,
+      // so the slices assemble into exactly the tile layout one full-box load would give), multicast to the whole cluster
       const int a_rows = BM / cn;
       const uint16_t a_mask = static_cast<uint16_t>((1u << cn) - 1);
       for (int t = t_begin; t < t_end; ++t) {
         const int m_blk = t / n_cblocks, n_blk = (t % n_cblocks) * cn + rn;
+        // grouped weights (one matrix per task, stacked along N): the row block picks its matrix; blocks never straddle
+        // two groups (grp_rows is a multiple of the block height, checked on the host)
         const int w_row0 = p.grp_rows > 0 ? ((m_blk * BM) / p.grp_rows) * p.N : 0;
         for (int kb = 0; kb < k_blocks; ++kb) {
           mbar_wait(&empty_bar[s], ph ^ 1);
           const int kc = kb * BK;
+          // the stage fills with the A slices of every CTA of the cluster and this CTA's own W box: the whole stage
           mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
           uint8_t* da = smem_a + s * Cfg::kABytes + rn * a_rows * (BK * 2);
           const int ya = m_blk * BM + rn * a_rows;
@@ -880,6 +760,9 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     int row_mblk = -1;
     int s = 0;
     uint32_t ph = 0;
+    // a stage of this CTA is written by the producers of every CTA of its cluster (A slices): freeing it is one
+    // arrival on the empty barrier of each of them, lane i for CTA i, so that the arrivals go out side by side on the
+    // MMA warp's critical path
     auto release = [&](int st) {
       if (cn == 1) {
         if (lane == 0) mbar_arrive(&empty_bar[st]);
@@ -890,7 +773,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     for (int t = t_begin; t < t_end; ++t) {
       const int m_blk = t / n_cblocks, n_blk = (t % n_cblocks) * cn + rn;
       const int row0 = m_blk * BM + 64 * wg + 16 * wq;   // first row of this warp's boxes
-      if (m_blk != row_mblk) {   // per-row state (the same expressions as gemm_kernel)
+      if (m_blk != row_mblk) {   // per-row state, reloaded only when the row block changes
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = row0 + fr + 8 * h < p.M ? row0 + fr + 8 * h : p.M - 1;   // rows past M: never stored
@@ -1009,6 +892,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (lane == 0) bulk_wait_read<0>();   // smem must outlive the last stores' reads
     __syncwarp();
   }
+  // no CTA leaves while another of its cluster may still arrive on its barriers
   if constexpr (CN > 1) cluster_sync();
   else __syncthreads();
 }
@@ -1034,30 +918,37 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// The kernel gemm_f16 launches for an epilogue, cluster size and tile width (WIDE: gemm_wide_kernel), with its shared
-// memory and block size.
-template <int EPI, int CN, bool WIDE>
+// The kernel gemm_f16 launches for an epilogue, with its shared memory, block size and tile width: gemm_wide_kernel for
+// the LayerNorm-fold projections, in clusters of CN CTAs; gemm_kernel, which has no clusters, for every other epilogue.
+template <int EPI>
 struct Kernel {
+  static constexpr bool kWide = EPI == EPI_ROPE || EPI == EPI_GEGLU;
+  template <int CN>
   static constexpr auto fn() {
-    if constexpr (WIDE) return gemm_wide_kernel<EPI, CN>;
-    else return gemm_kernel<EPI, CN>;
+    if constexpr (kWide) {
+      return gemm_wide_kernel<EPI, CN>;
+    } else {
+      static_assert(CN == 1, "gemm_kernel runs without clusters");
+      return gemm_kernel<EPI>;
+    }
   }
-  static constexpr int kSmem = WIDE ? WideCfg<EPI>::kSmemBytes : GemmCfg<EPI>::kSmemBytes;
-  static constexpr int kThreads = WIDE ? kWideThreads : kGemmThreads;
-  static constexpr int kBN = WIDE ? BNW : BN;
+  static constexpr int kSmem = kWide ? WideCfg<EPI>::kSmemBytes : GemmCfg<EPI>::kSmemBytes;
+  static constexpr int kThreads = kWide ? kWideThreads : kGemmThreads;
+  static constexpr int kBN = kWide ? BNW : BN;
 };
 
 // Clusters of CN CTAs of the kernel that are co-resident on the device.  A GPC holds a whole number of
 // clusters, so this is the occupancy query's answer, not num_sms / CN.  Asked once per kernel and cluster size
 // (all devices of one box are the same part).
-template <int EPI, int CN, bool WIDE = false>
+template <int EPI, int CN>
 int max_clusters(int num_sms) {
-  using Kn = Kernel<EPI, CN, WIDE>;
+  using Kn = Kernel<EPI>;
+  const auto fn = Kn::template fn<CN>();
   constexpr int csize = CN;
   static std::atomic<int> cached{0};
   int n = cached.load(std::memory_order_relaxed);
   if (n > 0) return n;
-  SRB_CUDA_CHECK(cudaFuncSetAttribute(Kn::fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::kSmem));
+  SRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::kSmem));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(csize * num_sms);
   cfg.blockDim = dim3(Kn::kThreads);
@@ -1069,7 +960,7 @@ int max_clusters(int num_sms) {
   attr.val.clusterDim.z = 1;
   cfg.attrs = &attr;
   cfg.numAttrs = 1;
-  SRB_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&n, Kn::fn(), &cfg));
+  SRB_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&n, fn, &cfg));
   if (n <= 0) {
     fprintf(stderr, "[srb200] gemm_f16: no %d-CTA cluster of this kernel fits the device\n", csize);
     return -1;
@@ -1078,12 +969,13 @@ int max_clusters(int num_sms) {
   return n;
 }
 
-template <int EPI, int CN = 1, bool WIDE = false>
+template <int EPI, int CN = 1>
 int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
            const CUtensorMap& tx, const KArgs& ka, int num_sms, int grid_override = 0) {
-  using Kn = Kernel<EPI, CN, WIDE>;
+  using Kn = Kernel<EPI>;
+  const auto fn = Kn::template fn<CN>();
   // per-device attribute; cheap enough to set on every launch (multi-GPU processes switch devices)
-  SRB_CUDA_CHECK(cudaFuncSetAttribute(Kn::fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::kSmem));
+  SRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::kSmem));
   constexpr int csize = CN;
   const int tiles = ((ka.M + BM - 1) / BM) * ((ka.N + Kn::kBN * csize - 1) / (Kn::kBN * csize));   // cluster tiles
   cudaLaunchConfig_t cfg = {};
@@ -1103,14 +995,14 @@ int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, co
     attr[nattr].val.clusterDim.x = csize;
     attr[nattr].val.clusterDim.y = 1;
     attr[nattr++].val.clusterDim.z = 1;
-    workers = max_clusters<EPI, CN, WIDE>(num_sms);
+    workers = max_clusters<EPI, CN>(num_sms);
     if (workers <= 0) return -1;
   }
   const int grid = grid_override > 0 ? grid_override : csize * (tiles < workers ? tiles : workers);
   cfg.gridDim = dim3(grid);
   cfg.attrs = attr;
   cfg.numAttrs = nattr;
-  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, Kn::fn(), ta, tb, tc, tx, ka));
+  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, fn, ta, tb, tc, tx, ka));
   note_launch();
   return 0;
 }
@@ -1148,30 +1040,24 @@ int make_tmap_f16_kmajor(CUtensorMap* out, const void* ptr, uint64_t rows, uint6
   return make_tmap_2d(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, k, rows, k, BK, box_rows);
 }
 
-// Measured at T = 131072 (ModernBERT-base, tools/gemm_prof.py), ms per GEMM.  H100 80GB HBM3 at a 400 W power limit
-// (power-capped SM clock), clusters of 1 x 1 / 2 x 1 (two row blocks share W) / 1 x 2 (two column tiles share A) /
-// 2 x 2:  Wqkv (EPI_ROPE, N 2304, K 768) 1.46 / 1.52 / 1.31 / 1.29;  Wi (EPI_GEGLU, N 2304) 1.39 / 1.39 / 1.28 / 1.46;
-// Wo2 (EPI_RESID_HL, N 768, K 1152) 0.93 / 1.00 / 0.89 / 0.98;  Wo (EPI_RESID_HL, K 768) 0.59 / 0.63 / 0.64 / 0.67.
-// The same card at 700 W, 1 x 1 / 1 x 2:  Wqkv 1.08 / 0.96;  Wi 1.00 / 0.94;  Wo2 0.69 / 0.74.
-// Only sharing A helps, so the kernel implements 1 x cn clusters alone, and only the two large LayerNorm-fold
-// projections use them.  The residual GEMMs, whose time goes to the fp16-pair epilogue rather than the operand feed,
-// run without clusters; so do the epilogues not measured here (EPI_F16, EPI_GELU, EPI_RESID) and EPI_TOPK, whose
-// grouped schedule gives each worker its own query block.  A pair is only formed when the column tiles pair up
-// exactly, in both tile widths these projections can run at (128: gemm_kernel, 192: gemm_wide_kernel): with an odd
-// tile count every other cluster would carry a CTA that computes a tile wholly past N.
+// Measured at T = 131072 (ModernBERT-base, tools/gemm_prof.py), ms per GEMM, every GEMM on 128 x 128 tiles.  H100 80GB
+// HBM3 at a 400 W power limit (power-capped SM clock), clusters of 1 x 1 / 2 x 1 (two row blocks share W) / 1 x 2 (two
+// column tiles share A) / 2 x 2:  Wqkv (EPI_ROPE, N 2304, K 768) 1.46 / 1.52 / 1.31 / 1.29;  Wi (EPI_GEGLU, N 2304)
+// 1.39 / 1.39 / 1.28 / 1.46;  Wo2 (EPI_RESID_HL, N 768, K 1152) 0.93 / 1.00 / 0.89 / 0.98;  Wo (EPI_RESID_HL, K 768)
+// 0.59 / 0.63 / 0.64 / 0.67.  The same card at 700 W, 1 x 1 / 1 x 2:  Wqkv 1.08 / 0.96;  Wi 1.00 / 0.94;  Wo2 0.69 / 0.74.
+// Only sharing A helps, so clusters are 1 x cn only, and only the two large LayerNorm-fold projections
+// (gemm_wide_kernel) use them.  The residual GEMMs, whose time goes to the fp16-pair epilogue rather than the operand
+// feed, run without clusters; so do the epilogues not measured here (EPI_F16, EPI_GELU, EPI_RESID) and EPI_TOPK, whose
+// grouped schedule gives each worker its own query block.
+// A pair forms only where N's column-tile count is even both in 128-wide and in 192-wide tiles.  The 192-wide kernel
+// needs the second condition: with an odd count, every other cluster would carry a CTA that computes a tile wholly past
+// N.  The first condition is kept because this rule is the configuration the clustered 192-wide kernel was measured in.
+// A rule on 192-wide tiles alone would pair shapes that run unpaired today (ModernBERT-large's Wi at N = 5248: 41 tiles
+// of 128, 28 of 192), and its speed there has not been measured.
 int gemm_cluster_size(int epi, int N, int K) {
   (void)K;
   const bool share_a = epi == EPI_ROPE || epi == EPI_GEGLU;
   return share_a && ((N + BN - 1) / BN) % 2 == 0 && ((N + BNW - 1) / BNW) % 2 == 0 ? 2 : 1;
-}
-
-// EPI_ROPE and EPI_GEGLU run on gemm_wide_kernel; SRB_GEMM_WIDE=0 puts them back on gemm_kernel (A/B measurements and
-// the bitwise comparison of the two kernels).  Read once per process.  gemm_cluster_size does not look at it: at an N
-// whose 128-wide tiles pair but 192-wide ones do not (512, 1280, ...) the 128 x 128 kernel then runs unclustered --
-// another schedule than it had on its own, the same results.
-static bool gemm_wide() {
-  static const bool on = [] { const char* e = getenv("SRB_GEMM_WIDE"); return !(e && e[0] == '0'); }();
-  return on;
 }
 
 static int device_sms() {
@@ -1190,8 +1076,8 @@ int gemm_cluster_workers(int epi, int N, int K) {
   const int num_sms = device_sms();
   if (num_sms <= 0 || cn == 1) return num_sms;
   // gemm_cluster_size forms pairs for these two epilogues only
-  if (epi == EPI_ROPE) return gemm_wide() ? max_clusters<EPI_ROPE, 2, true>(num_sms) : max_clusters<EPI_ROPE, 2>(num_sms);
-  if (epi == EPI_GEGLU) return gemm_wide() ? max_clusters<EPI_GEGLU, 2, true>(num_sms) : max_clusters<EPI_GEGLU, 2>(num_sms);
+  if (epi == EPI_ROPE) return max_clusters<EPI_ROPE, 2>(num_sms);
+  if (epi == EPI_GEGLU) return max_clusters<EPI_GEGLU, 2>(num_sms);
   return -1;
 }
 
@@ -1223,7 +1109,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   const int num_sms = device_sms();
   if (num_sms <= 0) return -1;
   const int cn = gemm_cluster_size(g.epi, g.N, g.K);
-  const bool wide = (g.epi == EPI_ROPE || g.epi == EPI_GEGLU) && gemm_wide();
+  const bool wide = g.epi == EPI_ROPE || g.epi == EPI_GEGLU;   // gemm_wide_kernel
   // operand boxes: each CTA of a cluster loads 1/cn of the A box (kernel: TMA producer)
   CUtensorMap ta, tb, tc;
   if (make_tmap_f16_kmajor(&ta, g.A, static_cast<uint64_t>(g.a_rows > 0 ? g.a_rows : g.M), g.K, BM / cn)) return -1;
@@ -1233,7 +1119,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
     return -1;
   }
   if (make_tmap_f16_kmajor(&tb, g.W, static_cast<uint64_t>(g.N) * w_groups, g.K, wide ? BNW : BN)) return -1;
-  // output boxes: 32 rows x 128 bytes (64 fp16 or 32 fp32 columns), clipped at M rows / n_out columns
+  // output boxes, clipped at M rows / n_out columns.  gemm_kernel: 32 rows x 128 bytes (64 fp16 or 32 fp32 columns)
   if (g.epi == EPI_TOPK) {
     tc = ta;   // no matrix output
   } else if (g.epi == EPI_RESID) {
@@ -1247,8 +1133,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
                      geglu ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B))
       return -1;
   } else {
-    const uint64_t n_out = g.epi == EPI_GEGLU ? g.N / 2 : g.N;
-    if (make_tmap_2d(&tc, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.out, n_out, g.M, g.ldo, 64, 32)) return -1;
+    if (make_tmap_2d(&tc, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.out, g.N, g.M, g.ldo, 64, 32)) return -1;
   }
   KArgs ka;
   ka.M = g.M; ka.N = g.N; ka.K = g.K;
@@ -1280,17 +1165,11 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   switch (g.epi) {
     case EPI_F16: return launch<EPI_F16>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_ROPE:
-      if (wide)
-        return cn == 2 ? launch<EPI_ROPE, 2, true>(stream, ta, tb, tc, tx, ka, num_sms)
-                       : launch<EPI_ROPE, 1, true>(stream, ta, tb, tc, tx, ka, num_sms);
       return cn == 2 ? launch<EPI_ROPE, 2>(stream, ta, tb, tc, tx, ka, num_sms)
                      : launch<EPI_ROPE>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_RESID: return launch<EPI_RESID>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_RESID_HL: return launch<EPI_RESID_HL>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_GEGLU:
-      if (wide)
-        return cn == 2 ? launch<EPI_GEGLU, 2, true>(stream, ta, tb, tc, tx, ka, num_sms)
-                       : launch<EPI_GEGLU, 1, true>(stream, ta, tb, tc, tx, ka, num_sms);
       return cn == 2 ? launch<EPI_GEGLU, 2>(stream, ta, tb, tc, tx, ka, num_sms)
                      : launch<EPI_GEGLU>(stream, ta, tb, tc, tx, ka, num_sms);
     case EPI_GELU: return launch<EPI_GELU>(stream, ta, tb, tc, tx, ka, num_sms);

@@ -65,6 +65,18 @@ def _cluster(lib, epi, n, k):
     return cn.value
 
 
+def test_wide_cluster_workers(lib):
+    """The pair count of the kernel each clustered shape launches fits the device."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    f = lib.sr_test_gemm_cluster
+    f.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    for epi in (EPI_ROPE, EPI_GEGLU):
+        for n in (512, 1152, 1280, 1536, 2304, 3072):
+            cn, workers = C.c_int(0), C.c_int(0)
+            assert f(epi, n, 768, C.byref(cn), C.byref(workers)) == 0
+            assert 0 < workers.value * cn.value <= sms, (epi, n)
+
+
 def _up(x, a):
     return (x + a - 1) // a * a
 
@@ -207,7 +219,7 @@ MS = [1, 40, 64, 65, 127, 129, 2333, 16897]   # 16897 = 132 * 128 + 1: several t
 NS = [64, 192, 320, 2304]                      # 192: two column tiles (a 2-CTA cluster for RoPE), the second half empty
 NS_128 = [128, 640, 2304]                      # GeGLU and the fp16 pair need N % 128 == 0
 KS = [8, 72, 200, 768, 1160]                   # all but 768 end in a partial k-block
-ROPE_COLS = {64: 64, 192: 128, 320: 192, 2304: 1536}
+ROPE_COLS = {64: 64, 192: 128, 320: 192, 1152: 768, 2304: 1536}
 EPIS = [EPI_F16, EPI_ROPE, EPI_RESID, EPI_GEGLU, EPI_GELU, EPI_RESID_HL]
 
 
@@ -229,22 +241,29 @@ def test_shape_edges(lib, epi, M, N, K, i):
 
 
 @pytest.mark.parametrize("epi,N,M", [(EPI_ROPE, 2304, 2333), (EPI_ROPE, 320, 127), (EPI_GEGLU, 2304, 65),
-                                     (EPI_GEGLU, 640, 2333)])
+                                     (EPI_GEGLU, 640, 2333), (EPI_ROPE, 1152, 20000), (EPI_GEGLU, 2304, 20000)])
 def test_layernorm_fold(lib, epi, N, M):
     """The fold scales the whole accumulator by the row's rstd, which depends on the LayerNorm epsilon for rows of small
-    variance."""
+    variance.  M = 20000 gives every worker several row blocks, unclustered (N = 1152) and in pairs (N = 2304)."""
     p = problem(epi, M, N, 768, seed=31 * M, fold=True, rope_cols=ROPE_COLS.get(N, 0), w_scale=0.01)
     check_parity(p, tag=go.EPI_NAMES[epi] + "+fold")
 
 
+GROUPED = [(EPI_F16, 384, 200, False), (EPI_ROPE, 2304, 768, False), (EPI_ROPE, 2304, 768, True),
+           (EPI_ROPE, 1152, 768, False), (EPI_ROPE, 1152, 768, True), (EPI_GEGLU, 2304, 768, False),
+           (EPI_GEGLU, 2304, 768, True), (EPI_RESID_HL, 768, 768, False)]
+
+
 @pytest.mark.parametrize("rows", [128, 256])
-@pytest.mark.parametrize("epi,N,K", [(EPI_F16, 384, 200), (EPI_ROPE, 2304, 768), (EPI_RESID_HL, 768, 768)])
-def test_grouped_weights(lib, epi, N, K, rows):
+@pytest.mark.parametrize("epi,N,K,fold", GROUPED,
+                         ids=[f"{e}-{n}-{k}" + ("-fold" if f else "") for e, n, k, f in GROUPED])
+def test_grouped_weights(lib, epi, N, K, fold, rows):
     """w_groups = 3 stacked matrices; the last group is partly empty.  Row blocks of 128 never straddle two groups
-    when w_group_rows is a multiple of 128, which is what gemm_f16 accepts."""
+    when w_group_rows is a multiple of 128, which is what gemm_f16 accepts.  The LayerNorm-fold projections run in
+    pairs at N = 2304 and unclustered at N = 1152 (the shared-LoRA serving shapes)."""
     p = problem(epi, 3 * rows - 5, N, K, seed=rows + epi, w_groups=3, w_group_rows=rows, rope_cols=ROPE_COLS.get(N, 0),
-                bias=epi == EPI_F16)
-    check_parity(p, tag=go.EPI_NAMES[epi] + "+grp")
+                bias=epi == EPI_F16, fold=fold, w_scale=0.01 if fold else 0.05)
+    check_parity(p, tag=go.EPI_NAMES[epi] + ("+grp+fold" if fold else "+grp"))
 
 
 # ---- the cache scan: GEMV (B <= 4), fused top-8 epilogue (one row block, and the grouped schedule), two-pass (k > 8)

@@ -1,6 +1,7 @@
 """The thread-block cluster rule of the LayerNorm-fold projections (gemm_cluster_size), host side only: a pair of CTAs
-shares A only where the column tiles pair up at both tile widths these GEMMs can run at (128: gemm_kernel, 192:
-gemm_wide_kernel), so that no cluster carries a tile wholly past N; every other epilogue runs unclustered."""
+shares A only where N's column-tile count is even both in 128-wide and in 192-wide tiles.  The even count at 192 keeps
+every cluster free of a tile wholly past N; the even count at 128 keeps the schedule the clustered kernel was measured
+with.  Every other epilogue runs unclustered."""
 import ctypes as C
 
 import pytest

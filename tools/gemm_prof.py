@@ -12,12 +12,9 @@ loads 1/cluster_n of the shared A box and multicasts it to the others; W boxes a
 co-resident clusters (workers of the persistent grid), and torch.mm on the same fp16 M, N, K as a cuBLAS reference point (no epilogue: a
 reference, not a target).  The GPU name, power limit and maximum SM clock are read in the same run.
 
-  python tools/gemm_prof.py [--root TREE] [--iters N] [--json OUT] [--only Wqkv,Wi] [--ab ROUNDS]
+  python tools/gemm_prof.py [--root TREE] [--iters N] [--json OUT] [--only Wqkv,Wi]
 
 --root loads the library built in another checkout of this project (to compare two builds in one run).
---ab times Wqkv and Wi on both kernels the library has for them -- 128 x 192 tiles (gemm_wide_kernel, the default)
-and 128 x 128 (SRB_GEMM_WIDE=0) -- in ROUNDS alternating child processes (the switch is read once per process), and
-prints every round and the median ratio.
 """
 import argparse
 import ctypes as C
@@ -32,32 +29,7 @@ ap.add_argument("--m", type=int, default=131072)
 ap.add_argument("--iters", type=int, default=20)
 ap.add_argument("--json", default=None, help="also write the rows as JSON here")
 ap.add_argument("--only", default=None, help="comma-separated GEMM names to time")
-ap.add_argument("--ab", type=int, default=0, help="rounds of the 128 x 192 / 128 x 128 A/B on Wqkv and Wi")
 args = ap.parse_args()
-
-if args.ab:
-    import statistics
-    import tempfile
-    times = {"wide": [], "narrow": []}
-    with tempfile.TemporaryDirectory() as d:
-        for r in range(args.ab):
-            for name, flag in (("narrow", "0"), ("wide", "1")):
-                out = os.path.join(d, f"{name}{r}.json")
-                cmd = [sys.executable, os.path.abspath(__file__), "--root", args.root, "--m", str(args.m), "--iters",
-                       str(args.iters), "--only", "Wqkv,Wi", "--json", out]
-                subprocess.run(cmd, env=dict(os.environ, SRB_GEMM_WIDE=flag), check=True, stdout=subprocess.DEVNULL)
-                res = json.load(open(out))
-                times[name].append({row["gemm"]: row["ms"] for row in res["rows"]})
-                print(f"# round {r} {name:6s} " + "  ".join(f"{k} {v:.3f} ms" for k, v in times[name][-1].items()),
-                      flush=True)
-    print(f"# {res['gpu']}   M={args.m}")
-    for g in ("Wqkv", "Wi"):
-        w = [t[g] for t in times["wide"]]
-        n = [t[g] for t in times["narrow"]]
-        print(f"  {g:5s} 128x128 median {statistics.median(n):.3f} ms (spread {min(n):.3f}-{max(n):.3f})   "
-              f"128x192 median {statistics.median(w):.3f} ms (spread {min(w):.3f}-{max(w):.3f})   "
-              f"{100 * (1 - statistics.median(w) / statistics.median(n)):.1f} % faster")
-    sys.exit(0)
 sys.path.insert(0, os.path.abspath(args.root))
 
 import torch  # noqa: E402
@@ -166,8 +138,8 @@ if args.only:
 for name, epi_name, epi, n, k, fn, hbm in gemms:
     ms = timed(fn, args.iters)
     cn, workers = cluster_shape(epi, n, k)
-    # tile width of the kernel this GEMM runs on: 192 for the LayerNorm-fold projections unless SRB_GEMM_WIDE=0
-    bn = 192 if epi in (EPI_ROPE, EPI_GEGLU) and os.environ.get("SRB_GEMM_WIDE", "1")[:1] != "0" else BN
+    # tile width of the kernel this GEMM runs on: 192 for the LayerNorm-fold projections (gemm_wide_kernel)
+    bn = 192 if epi in (EPI_ROPE, EPI_GEGLU) else BN
     tiles = ((M + BM - 1) // BM) * ((n + bn - 1) // bn)
     l2_bytes = tiles * k * 2 * (BM / cn + bn)
     a = x_i if k == I else x_h
