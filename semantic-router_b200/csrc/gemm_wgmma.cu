@@ -45,13 +45,16 @@ constexpr int kBarrierBytes = 512;
 constexpr int kSmemLimit = 232448;     // 227 KB opt-in limit per CTA (sm_90)
 constexpr int kAccBytes = BM * BN * 4; // fp32 accumulator tile handed from the MMA warpgroup to the epilogue
 // staging boxes per epilogue warp.  The fp32-residual epilogue keeps one residual load in flight next to the box being
-// computed; the fp16-pair residual epilogue keeps two (hi, lo) box pairs (one loading while the other computes).
-// Shared memory is what limits this on sm_90: the 64 KB accumulator tile plus these boxes leave 3-4 mainloop stages.
-__host__ __device__ constexpr int stage_bufs(int epi) { return epi == EPI_RESID_HL ? 4 : 2; }
+// computed; the fp16-pair residual epilogue has one (hi, lo) box pair, loaded at the start of the chunk that uses it.
+// Shared memory is what limits this on sm_90: the 64 KB accumulator tile plus these boxes leave 4 mainloop stages.  A
+// second pair (to load a chunk ahead) costs the fourth stage, and the residual GEMMs are bound by their operand feed,
+// not by the epilogue's load latency: at T = 131072 on an H100 80GB HBM3 (700 W), two pairs and 3 stages ran Wo in
+// 0.518 ms and Wo2 in 0.651-0.662 ms, one pair and 4 stages 0.443-0.444 and 0.528-0.536 ms (tools/gemm_prof.py).
+constexpr int kStageBufs = 2;
 
 template <int EPI>
 struct GemmCfg {
-  static constexpr int kBufs = stage_bufs(EPI);
+  static constexpr int kBufs = kStageBufs;
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
@@ -172,7 +175,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   using Cfg = GemmCfg<EPI>;
   static_assert(Cfg::kSmemBytes <= kSmemLimit, "over the 227 KB shared-memory opt-in limit");
   constexpr bool kHL = EPI == EPI_RESID_HL;
-  constexpr int kStageBufs = Cfg::kBufs;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -341,7 +343,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     // chunk geometry: a chunk is one 32-row x 128-byte output box of this warp
     constexpr int kChunkCols = (EPI == EPI_RESID || EPI == EPI_TOPK) ? 32 : 64;   // accumulator = output columns
     constexpr int kChunks = BN / kChunkCols;
-    constexpr int kPairs = kStageBufs / 2;   // EPI_RESID_HL: (hi, lo) box pairs of this warp
+    constexpr int kPairs = kStageBufs / 2;   // EPI_RESID_HL: (hi, lo) box pairs of this warp (one)
     const bool use_resid = (EPI == EPI_RESID) && p.has_resid;
 
     // EPI_RESID: residual boxes are TMA-loaded one chunk ahead (flat over (tile, chunk) of this CTA)
@@ -360,9 +362,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       }
     };
     // residual prefetch cursor: runs kAhead chunks in front of the chunk being processed (flat over this CTA's
-    // (tile, chunk) sequence)
+    // (tile, chunk) sequence); EPI_RESID_HL: 0, the single pair is loaded at the start of its own chunk
     constexpr int kRing = kHL ? kPairs : kStageBufs;   // residual-load ring: boxes, or box pairs
-    constexpr int kAhead = kHL ? 1 : (kStageBufs - 2 > 0 ? kStageBufs - 2 : 1);
+    constexpr int kAhead = kHL ? kPairs - 1 : (kStageBufs - 2 > 0 ? kStageBufs - 2 : 1);
     int pf_t = t_begin, pf_c = 0, pf_buf = 0;
     auto pf_issue = [&]() {  // lane 0 only
       if (!chunk_valid(pf_t, pf_c)) return;
@@ -481,8 +483,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         }
       }
       if constexpr (kHL) {
-        // 64-column chunks: the (hi, lo) boxes of the chunk arrive by TMA one chunk ahead, are updated in place in
-        // shared memory and leave by TMA; statistics go out per 128-column slice
+        // 64-column chunks: the (hi, lo) boxes of the chunk arrive by TMA, are updated in place in shared memory and
+        // leave by TMA; statistics go out per 128-column slice
 #pragma unroll 1
         for (int c = 0; c < kChunks; ++c) {
           const int ocol0 = out_col(t, c);
@@ -490,7 +492,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           uint8_t* hb = my_bufs + cb * 2 * kStageBufBytes;
           uint8_t* lb = hb + kStageBufBytes;
           if (lane == 0) {
-            // the pair the prefetch cursor points at was stored kPairs - 1 chunks ago: all but the newest store group read out
+            // the pair the prefetch cursor points at was last stored kPairs - kAhead chunks ago: read out by now
             bulk_wait_read<kPairs - kAhead - 1>();
             pf_issue();
           }
@@ -1046,8 +1048,8 @@ int make_tmap_f16_kmajor(CUtensorMap* out, const void* ptr, uint64_t rows, uint6
 // 1.39 / 1.39 / 1.28 / 1.46;  Wo2 (EPI_RESID_HL, N 768, K 1152) 0.93 / 1.00 / 0.89 / 0.98;  Wo (EPI_RESID_HL, K 768)
 // 0.59 / 0.63 / 0.64 / 0.67.  The same card at 700 W, 1 x 1 / 1 x 2:  Wqkv 1.08 / 0.96;  Wi 1.00 / 0.94;  Wo2 0.69 / 0.74.
 // Only sharing A helps, so clusters are 1 x cn only, and only the two large LayerNorm-fold projections
-// (gemm_wide_kernel) use them.  The residual GEMMs, whose time goes to the fp16-pair epilogue rather than the operand
-// feed, run without clusters; so do the epilogues not measured here (EPI_F16, EPI_GELU, EPI_RESID) and EPI_TOPK, whose
+// (gemm_wide_kernel) use them.  The residual GEMMs run without clusters (a deeper operand ring sped them up instead:
+// GemmCfg, Wo 0.52 -> 0.44 ms, Wo2 0.66 -> 0.53 ms at 700 W); so do the epilogues not measured here (EPI_F16, EPI_GELU, EPI_RESID) and EPI_TOPK, whose
 // grouped schedule gives each worker its own query block.
 // A pair forms only where N's column-tile count is even both in 128-wide and in 192-wide tiles.  The 192-wide kernel
 // needs the second condition: with an odd count, every other cluster would carry a CTA that computes a tile wholly past
