@@ -206,10 +206,11 @@ def modernbert_forward(weights: Dict[str, torch.Tensor], cfg: ModernBertConfig,
     B, S = ids.shape
     nH, D = cfg.num_attention_heads, cfg.head_dim
     L = cfg.num_hidden_layers if num_layers is None else min(num_layers, cfg.num_hidden_layers)
+    dev = ids.device
     gmask = global_mask_4d(mask)
-    lmask = local_mask(S, cfg.local_attention // 2)
-    cos_g, sin_g = rope_tables(D, cfg.global_rope_theta, S)
-    cos_l, sin_l = rope_tables(D, cfg.local_rope_theta, S)
+    lmask = local_mask(S, cfg.local_attention // 2).to(dev)
+    cos_g, sin_g = (t.to(dev) for t in rope_tables(D, cfg.global_rope_theta, S))
+    cos_l, sin_l = (t.to(dev) for t in rope_tables(D, cfg.local_rope_theta, S))
 
     x = F.embedding(ids.long(), _w(weights, "embeddings.tok_embeddings.weight", P))
     x = layer_norm(x, _w(weights, "embeddings.norm.weight", P), None, cfg.layer_norm_eps)
@@ -410,9 +411,11 @@ def mmbert_embed(weights, cfg: ModernBertConfig, ids: torch.Tensor, mask: torch.
 # BERT (candle-transformers models/bert.rs semantics)
 # --------------------------------------------------------------------------------------
 def bert_forward(weights: Dict[str, torch.Tensor], cfg: BertConfig, ids: torch.Tensor,
-                 mask: torch.Tensor, prefix: str = "bert") -> torch.Tensor:
+                 mask: torch.Tensor, prefix: str = "bert",
+                 collect: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
     """candle BertModel::forward(input_ids, token_type_ids=0, Some(mask)) used at
-    traditional/bert.rs:230-234, core/similarity.rs:213-217, lora/bert_lora.rs:569."""
+    traditional/bert.rs:230-234, core/similarity.rs:213-217, lora/bert_lora.rs:569.
+    `collect` (optional) receives the hidden states after every layer."""
     p = (prefix + ".") if prefix else ""
     B, S = ids.shape
     nH, D = cfg.num_attention_heads, cfg.head_dim
@@ -439,6 +442,8 @@ def bert_forward(weights: Dict[str, torch.Tensor], cfg: BertConfig, ids: torch.T
         x = layer_norm(lin(inter, "output.dense") + x,
                        weights[Lp + "output.LayerNorm.weight"],
                        weights[Lp + "output.LayerNorm.bias"], cfg.layer_norm_eps)
+        if collect is not None:
+            collect.append(x.clone())
     return x
 
 
