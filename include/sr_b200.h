@@ -82,25 +82,41 @@ SR_API int sr_embed_ids_padded(sr_model* m, const int32_t* ids, const int32_t* c
 SR_API int sr_classify_multi_ids(sr_model* m, const int* heads, int n_heads, const int32_t* ids,
                           const int32_t* cu_seqlens, int batch, float** probs_out, int32_t** cls_out);
 
-/* ---- shared-base multi-task serving from UNMERGED LoRA checkpoints (SURVEY section 8 f3) ----------------
- * The reference's LoRA path computes x W^T + (alpha / r) (x A^T) B^T per adapted Linear (candle-binding/src/
- * model_architectures/lora/lora_adapter.rs:136-144) and its stated direction is one shared encoder for the intent / PII /
- * security tasks (src/semantic-router/pkg/classification/unified_classifier.go:113).  task_dirs[t] is a complete checkpoint
- * of task t: the SAME base tensors in every directory (checked bit for bit), `X.lora_A.weight` / `X.lora_B.weight` next to
- * the adapted `X.weight`s, its own classifier head, lora_config.json {"rank", "alpha"}.  Every task's adapters are folded
- * into its own copy of the projection weights at load and the copies are stacked.  A batch then runs ONCE through the
- * encoder as n_tasks copies of its rows, and each 256-row block of a projection GEMM picks its task's matrix in the TMA
- * producer, instead of n_tasks forwards over n_tasks merged models: the arithmetic of n_tasks separately loaded models.
- * token_level[t]: 1 token head, 0 sequence head, -1 from config.json. */
+/* ---- several task checkpoints of one encoder in ONE pass ---------------------------------------------------
+ * task_dirs[t] (1 <= n_tasks <= 8) is a complete checkpoint of task t with its own classifier head: merged LoRA models
+ * (the reference publishes its LoRA classifiers merged, lora_*_model), full fine-tunes of one base, or anything else of
+ * one encoder shape.  Every config.json field that shapes the encoder (architecture, hidden_size, num_hidden_layers,
+ * num_attention_heads, intermediate_size, vocab_size, max_position_embeddings, global_attn_every_n_layers,
+ * local_attention, both rope thetas, layer_norm_eps, classifier_pooling) must be equal, and padded-head (MiniLM) encoders
+ * are refused; these refusals name the field and the directory and come before any device is touched.  A tensor that
+ * is bitwise the same in every task is loaded once; one that differs gets a device copy per task.  Each task's
+ * projection weights (its own LayerNorm gamma folded in, adapters a checkpoint still carries merged as sr_model_load
+ * merges them) are stacked.  A batch then runs ONCE through the encoder as n_tasks copies of its rows: each 256-row block
+ * of a projection GEMM picks its task's matrix and bias, every embedding and LayerNorm row its task's weights, every
+ * task's head its task's final norm -- bitwise what n_tasks separately loaded models give.  The ordinary entries above
+ * run task 0's encoder on such a model; sr_model_set_precise refuses it.  token_level[t]: 1 token head, 0 sequence head, -1
+ * from config.json. */
+SR_API int sr_model_load_grouped(const char* const* task_dirs, const int* token_level, int n_tasks, int device,
+                                 sr_model** out);
+/* sr_model_load_grouped for UNMERGED LoRA checkpoints over one base (SURVEY section 8 f3): the reference's LoRA path
+ * computes x W^T + (alpha / r) (x A^T) B^T per adapted Linear (candle-binding/src/model_architectures/lora/
+ * lora_adapter.rs:136-144).  Every directory carries the SAME base tensors (checked bit for bit; refused otherwise),
+ * `X.lora_A.weight` / `X.lora_B.weight` next to the adapted `X.weight`s and lora_config.json {"rank", "alpha"}; a set
+ * without adapters is refused (load it with sr_model_load_grouped).  Each task's adapters are folded into its own copy
+ * of the projection weights at load. */
 SR_API int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_level, int n_tasks, int device,
                                      sr_model** out);
-SR_API int sr_lora_shared_tasks(const sr_model* m);   /* 0 for an ordinary model */
+/* tasks of a model from sr_model_load_grouped or sr_model_load_lora_shared; 0 for an ordinary model */
+SR_API int sr_lora_shared_tasks(const sr_model* m);
 /* 1: <model_dir>/model.safetensors carries lora_A / lora_B tensors, 0: it does not (a merged checkpoint), -1: unreadable */
 SR_API int sr_checkpoint_has_adapters(const char* model_dir);
-/* For each task t: sequence heads write probs_out[t] [batch, C_t], cls_out[t] / conf_out[t] [batch]; token heads write
+/* One pass of a grouped model (sr_model_load_grouped or sr_model_load_lora_shared) over a batch, every task's head.
+ * For each task t: sequence heads write probs_out[t] [batch, C_t], cls_out[t] / conf_out[t] [batch]; token heads write
  * probs_out[t] [T, C_t], cls_out[t] / conf_out[t] [T] (T = cu_seqlens[batch]).  Any of the pointers may be NULL. */
 SR_API int sr_classify_lora_shared_ids(sr_model* m, const int32_t* ids, const int32_t* cu_seqlens, int batch, int pooler_mode,
                                        float** probs_out, int32_t** cls_out, float** conf_out);
+/* device bytes of the tensors a model holds (weights, heads, rotary tables; not the per-call workspace) */
+SR_API long long sr_model_device_bytes(const sr_model* m);
 
 /* ---- device-resident entries (asynchronous on the model's stream; for kernel-only timing) ------------- */
 SR_API int sr_model_set_stream(sr_model* m, void* cuda_stream);   /* cudaStream_t; NULL restores the private stream */

@@ -49,6 +49,9 @@ def load_library(path: Optional[str] = None):
     L.sr_embed_ids_padded.argtypes = [vp, vp, vp, vp, C.c_int, vp]
     L.sr_classify_multi_ids.argtypes = [vp, vp, C.c_int, vp, vp, C.c_int, vp, vp]
     L.sr_model_load_lora_shared.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(vp)]
+    L.sr_model_load_grouped.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(vp)]
+    L.sr_model_device_bytes.argtypes = [vp]
+    L.sr_model_device_bytes.restype = C.c_longlong
     L.sr_lora_shared_tasks.argtypes = [vp]
     L.sr_checkpoint_has_adapters.argtypes = [C.c_char_p]
     L.sr_classify_lora_shared_ids.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp]
@@ -228,6 +231,10 @@ class Model:
     def num_classes(self, head: int = 0) -> int:
         return int(lib().sr_head_num_classes(self._h, head))
 
+    def device_bytes(self) -> int:
+        """Device bytes of the loaded tensors (not the per-call workspace)."""
+        return int(lib().sr_model_device_bytes(self._h))
+
     # ---- host-buffer entries (the e2e path: H2D + compute + D2H inside the call)
     def classify_ids(self, seqs: Sequence[np.ndarray], head: int = 0, pooler_mode: int = 0) -> Dict[str, np.ndarray]:
         ids, cu = pack(seqs)
@@ -295,13 +302,16 @@ class Model:
 class LoraSharedModel(Model):
     """ONE base encoder + the unmerged LoRA adapters and heads of several task checkpoints over it (sr_b200.h:
     sr_model_load_lora_shared); a batch runs once, every task's copy of the rows with that task's merged weights."""
+    _loader = "sr_model_load_lora_shared"
 
     def __init__(self, task_dirs: Sequence[str], token_level: Sequence[int], device: int = 0):
         self._h = C.c_void_p()
+        if len(token_level) != len(task_dirs):
+            raise SrError(f"{self._loader}: {len(token_level)} token_level values for {len(task_dirs)} task checkpoints")
         dirs = (C.c_char_p * len(task_dirs))(*[d.encode() for d in task_dirs])
         tl = np.asarray(token_level, dtype=np.int32)
-        if lib().sr_model_load_lora_shared(dirs, _p(tl), len(task_dirs), device, C.byref(self._h)) != 0:
-            raise _err("sr_model_load_lora_shared")
+        if getattr(lib(), self._loader)(dirs, _p(tl) if len(tl) else None, len(task_dirs), device, C.byref(self._h)) != 0:
+            raise _err(self._loader)
         info = ModelInfo()
         lib().sr_model_info(self._h, C.byref(info))
         self.info = info
@@ -322,6 +332,13 @@ class LoraSharedModel(Model):
         if lib().sr_classify_lora_shared_ids(self._h, _p(ids), _p(cu), B, pooler_mode, arr(probs), arr(cls), arr(conf)) != 0:
             raise _err("sr_classify_lora_shared_ids")
         return probs, cls, conf
+
+
+class GroupedModel(LoraSharedModel):
+    """Several task checkpoints of one encoder shape -- merged LoRA models, fine-tunes of one base, any mix -- served in
+    ONE pass (sr_b200.h: sr_model_load_grouped): tensors equal in every task are held once, every task's copy of the rows
+    runs with that task's weights, and every task's results are bitwise those of the directory loaded alone as Model."""
+    _loader = "sr_model_load_grouped"
 
 
 class Cache:

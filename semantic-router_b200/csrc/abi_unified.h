@@ -7,14 +7,38 @@
 
 namespace {
 Slot g_lora_intent, g_lora_pii, g_lora_security;
-// The three LoRA tasks as ONE shared-base model when their checkpoints are unmerged adapters over one base (sr_b200.h:
-// sr_model_load_lora_shared): a batch then runs once through the encoder instead of three times.  SR_B200_LORA_SHARED=0
-// keeps the three slots.
+// The three LoRA tasks as ONE grouped model when their checkpoints share one encoder shape (sr_b200.h:
+// sr_model_load_lora_shared for unmerged adapters over one base, sr_model_load_grouped for merged or fine-tuned
+// checkpoints): a batch then runs once through the encoder instead of three times, with the three-slot results.
+// SR_B200_LORA_SHARED=0 keeps the three slots; so does anything the grouped loaders refuse.
 Slot g_lora_shared;
 std::map<int, std::string> g_lora_labels[3];
 Slot g_unified;  // shared encoder + 3 heads (legacy unified classifier)
 int g_unified_heads[3] = {-1, -1, -1};
 std::vector<std::string> g_unified_labels[3];
+// A grouped model tokenises a text once for all its tasks and runs one pooler mode (lora_config.json, slot_init): it
+// answers like separate slots only where those would tokenise and pool alike -- the same tokenizer.json bytes, and
+// lora_config.json in every directory or in none.
+bool same_serving_files(const char* const* dirs, int n) {
+  auto slurp = [](const std::string& path, std::string& out) {
+    FILE* f = fopen(path.c_str(), "rb");
+    if (!f) return false;
+    char buf[65536];
+    size_t k;
+    out.clear();
+    while ((k = fread(buf, 1, sizeof buf, f)) > 0) out.append(buf, k);
+    fclose(f);
+    return true;
+  };
+  std::string first, other;
+  const bool lora0 = file_exists(std::string(dirs[0]) + "/lora_config.json");
+  if (!slurp(std::string(dirs[0]) + "/tokenizer.json", first)) return false;
+  for (int i = 1; i < n; ++i)
+    if (file_exists(std::string(dirs[i]) + "/lora_config.json") != lora0 ||
+        !slurp(std::string(dirs[i]) + "/tokenizer.json", other) || other != first)
+      return false;
+  return true;
+}
 bool unified_slot_init(Slot& s, const char* dir, int token_level) {
   if (!slot_init(s, dir, token_level, true)) return false;
   if (SRB_ABI_HEAD_FLAVOR != 0)
@@ -35,12 +59,16 @@ bool init_lora_unified_classifier(const char* intent, const char* pii, const cha
   if (g_lora_shared.ready()) return true;
   static const bool shared_on = [] { const char* e = getenv("SR_B200_LORA_SHARED"); return !(e && e[0] == '0'); }();
   const bool fresh = !g_lora_intent.ready() && !g_lora_pii.ready() && !g_lora_security.ready();
-  if (shared_on && fresh && sr_checkpoint_has_adapters(intent) == 1 && sr_checkpoint_has_adapters(pii) == 1 &&
-      sr_checkpoint_has_adapters(security) == 1) {
+  if (shared_on && fresh) {
     const char* dirs[3] = {intent, pii, security};
     const int token_level[3] = {0, 1, 0};
-    const bool ok = slot_init(g_lora_shared, intent, -2, true,
-                              [&](int device, sr_model** out) { return sr_model_load_lora_shared(dirs, token_level, 3, device, out); });
+    const bool adapters = sr_checkpoint_has_adapters(intent) == 1 && sr_checkpoint_has_adapters(pii) == 1 &&
+                          sr_checkpoint_has_adapters(security) == 1;
+    const bool same_files = same_serving_files(dirs, 3);
+    const bool ok = slot_init(g_lora_shared, intent, -2, true, [&](int device, sr_model** out) {
+      if (adapters && sr_model_load_lora_shared(dirs, token_level, 3, device, out) == 0) return 0;
+      return same_files ? sr_model_load_grouped(dirs, token_level, 3, device, out) : -1;
+    });
     if (ok) {
       if (SRB_ABI_HEAD_FLAVOR != 0)
         for (auto& rep : g_lora_shared.reps) sr_model_set_head_flavor(rep->model, SRB_ABI_HEAD_FLAVOR);
@@ -50,7 +78,7 @@ bool init_lora_unified_classifier(const char* intent, const char* pii, const cha
       }
       return true;
     }
-    // different bases (or anything else the shared loader refuses): the tasks load as three independent slots
+    // different encoder shapes, architectures (or anything else the grouped loaders refuse): three independent slots
   }
   const bool a = unified_slot_init(g_lora_intent, intent, 0);
   const bool b = unified_slot_init(g_lora_pii, pii, 1);
@@ -69,7 +97,7 @@ static std::string lora_label(int task, int cls) {
 }
 
 // intent classes / confidences, per-token PII predictions, security classes / confidences of `n` texts from ONE encoder
-// pass per piece over the shared-base model (three copies of the rows, each with its task's adapters)
+// pass per piece over the grouped model (three copies of the rows, each with its task's weights)
 static bool lora_shared_packed(const char* const* texts, int n, std::vector<int32_t>& icls, std::vector<float>& iconf,
                                std::vector<std::vector<TokenPred>>& toks_out, std::vector<int32_t>& scls, std::vector<float>& sconf) {
   Slot& s = g_lora_shared;
@@ -109,7 +137,7 @@ LoRABatchResult classify_batch_with_lora(const char** texts, int num_texts) {
   int iC = 0, sC = 0;
   bool iok, pok, sok;
   if (shared) {
-    // one packed varlen pass per piece, the three tasks as three copies of the rows over ONE base (abi_unified.h top)
+    // one packed varlen pass per piece, the three tasks as three copies of the rows in ONE grouped model (abi_unified.h top)
     iok = pok = sok = lora_shared_packed(texts, num_texts, icls, iconf, toks, scls, sconf);
   } else {
     // three packed varlen passes (intent, PII tokens, security) over the whole batch -- the reference's

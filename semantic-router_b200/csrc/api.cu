@@ -375,43 +375,59 @@ int sr_classify_multi_ids(sr_model* h, const int* heads, int n_heads, const int3
   return 0;
 }
 
-// ---- shared-base multi-task pass over unmerged LoRA checkpoints (engine.h: LoraShared) --------------------------------
-int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_level, int n_tasks, int device, sr_model** out) {
-  if (!task_dirs || n_tasks <= 0 || n_tasks > 8 || !out) return fail("bad arguments");
+// ---- several task checkpoints of one encoder in one pass (engine.h: Grouped) -----------------------------------------
+namespace {
+using GroupedLoader = Model* (*)(const std::vector<std::string>&, const std::vector<int>&, int, std::string*);
+int load_grouped(const char* what, GroupedLoader load, const char* const* task_dirs, const int* token_level, int n_tasks,
+                 int device, sr_model** out) {
+  if (!task_dirs || !out) return fail(std::string(what) + ": bad arguments");
+  if (n_tasks <= 0 || n_tasks > kMaxRowGroups)
+    return fail(std::string(what) + ": n_tasks must be 1 to " + std::to_string(kMaxRowGroups));
   std::vector<std::string> dirs;
   std::vector<int> tl;
   for (int t = 0; t < n_tasks; ++t) {
-    if (!task_dirs[t]) return fail("bad arguments");
+    if (!task_dirs[t]) return fail(std::string(what) + ": bad arguments");
     dirs.push_back(task_dirs[t]);
     tl.push_back(token_level ? token_level[t] : -1);
   }
   std::string err;
-  Model* m = model_load_lora_shared(dirs, tl, device, &err);
-  if (!m) return fail("sr_model_load_lora_shared: " + err);
+  Model* m = load(dirs, tl, device, &err);
+  if (!m) return fail(std::string(what) + ": " + err);
   sr_model* h = new sr_model();
   h->m = m;
   h->private_stream = m->stream;
   *out = h;
   return 0;
 }
+}  // namespace
+
+int sr_model_load_grouped(const char* const* task_dirs, const int* token_level, int n_tasks, int device, sr_model** out) {
+  return load_grouped("sr_model_load_grouped", model_load_grouped, task_dirs, token_level, n_tasks, device, out);
+}
+
+int sr_model_load_lora_shared(const char* const* task_dirs, const int* token_level, int n_tasks, int device, sr_model** out) {
+  return load_grouped("sr_model_load_lora_shared", model_load_lora_shared, task_dirs, token_level, n_tasks, device, out);
+}
 
 int sr_checkpoint_has_adapters(const char* model_dir) { return model_dir ? checkpoint_has_adapters(model_dir) : -1; }
 
-int sr_lora_shared_tasks(const sr_model* h) { return h ? h->m->lora.tasks : -1; }
+int sr_lora_shared_tasks(const sr_model* h) { return h ? h->m->group.tasks : -1; }
+
+long long sr_model_device_bytes(const sr_model* h) { return h ? static_cast<long long>(h->m->weight_bytes) : -1; }
 
 int sr_classify_lora_shared_ids(sr_model* h, const int32_t* ids, const int32_t* cu, int batch, int pooler_mode,
                                 float** probs_out, int32_t** cls_out, float** conf_out) {
   if (!h) return fail("null model");
   Model& m = *h->m;
-  const int nt = m.lora.tasks;
-  if (nt <= 0) return fail("not a shared-LoRA model");
+  const int nt = m.group.tasks;
+  if (nt <= 0) return fail("not a grouped model");
   if (batch <= 0 || !ids || !cu || cu[0] != 0) return fail("bad arguments");
   std::lock_guard<std::mutex> lk(m.mu);
   DeviceGuard dg(m.device);
-  if (m.precise.on) return fail("the precise path serves merged weights only");
+  if (m.precise.on) return fail("the precise path serves ordinary models only");
   const int T1 = cu[batch];
   if (T1 <= 0 || static_cast<long long>(T1) * nt > (1ll << 30)) return fail("bad arguments");
-  // the batch once per task, task-major: rows [t * T1p, t * T1p + T1) run with task t's adapters.  Every copy is padded to
+  // the batch once per task, task-major: rows [t * T1p, t * T1p + T1) run with task t's weights.  Every copy is padded to
   // whole 256-row GEMM blocks (a block multiplies ONE task's matrices); the pad rows form one extra sequence per copy that
   // runs through the encoder and is read by nobody.
   const int T1p = (T1 + 255) / 256 * 256;
@@ -425,23 +441,23 @@ int sr_classify_lora_shared_ids(sr_model* h, const int32_t* ids, const int32_t* 
   rcu[static_cast<size_t>(Bp) * nt] = nt * T1p;
   size_t cseq = 0, ctok = 0;
   for (int t = 0; t < nt; ++t) {
-    const Head& hd = m.heads[m.lora.head_of_task[t]];
+    const Head& hd = m.heads[m.group.head_of_task[t]];
     if (hd.token_level) ctok = std::max<size_t>(ctok, hd.num_classes);
     else cseq = std::max<size_t>(cseq, hd.num_classes);
   }
   int T, max_len;
   if (stage_inputs(m, rids.data(), rcu.data(), Bp * nt, cseq, ctok, &T, &max_len)) return -1;
   Workspace& w = m.ws;
-  m.lora.rows_per_task = T1p;
+  m.group.rows_per_task = T1p;
   const uint64_t key = (1ull << 63) ^ (static_cast<uint64_t>(batch) << 48) ^ (static_cast<uint64_t>(T1) << 28) ^
                        (static_cast<uint64_t>(max_len) << 12);
   const int rc = run_graphed(h, key, T <= kGraphMaxTokens && Bp * nt <= 64, [&]() {
     return encoder_forward(m, w.ids, w.cu, Bp * nt, T, max_len, 0) ? fail("encoder_forward failed") : 0;
   });
-  m.lora.rows_per_task = 0;
+  m.group.rows_per_task = 0;
   if (rc) return -1;
   for (int t = 0; t < nt; ++t) {
-    const int head = m.lora.head_of_task[t];
+    const int head = m.group.head_of_task[t];
     const Head& hd = m.heads[head];
     const size_t rows = hd.token_level ? T1 : batch;
     if (hd.token_level ? head_tokens(m, head, batch, T1, t * T1p) : head_sequence(m, head, w.cu + static_cast<size_t>(t) * Bp, batch, pooler_mode))
@@ -462,7 +478,7 @@ int sr_model_set_precise(sr_model* h, int on) {
   if (!h) return fail("null model");
   std::lock_guard<std::mutex> lk(h->m->mu);
   DeviceGuard dg(h->m->device);
-  if (on && h->m->lora.tasks > 0) return fail("sr_model_set_precise: shared-LoRA models have no precise form (load the tasks as separate slots)");
+  if (on && h->m->group.tasks > 0) return fail("sr_model_set_precise: grouped models have no precise form (load the tasks as separate slots)");
   if (on) {
     std::string err;
     if (precise_prepare(*h->m, &err)) return fail("sr_model_set_precise: " + err);

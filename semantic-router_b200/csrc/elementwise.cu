@@ -65,18 +65,22 @@ __device__ __forceinline__ void row_store16(__half* row, const float4 (&v)[NV]) 
 
 constexpr int kRowThreads = 256;  // 8 rows per CTA
 
+// group of a row in a grouped pass (RowGroups): 0 when the launch is not grouped
+__device__ __forceinline__ int row_group(int row, int group_rows) { return group_rows > 0 ? row / group_rows : 0; }
+
 template <int NV>
 __global__ void __launch_bounds__(kRowThreads)
-embed_ln_mb_kernel(const int* __restrict__ ids, int T, int vocab, const float* __restrict__ table,
-                   const float* __restrict__ w, float eps, float* __restrict__ x, __half* __restrict__ h,
-                   __half* __restrict__ lo) {
+embed_ln_mb_kernel(const int* __restrict__ ids, int T, int vocab, const __grid_constant__ RowGroups table,
+                   const __grid_constant__ RowGroups w, int group_rows, float eps, float* __restrict__ x,
+                   __half* __restrict__ h, __half* __restrict__ lo) {
   const int row = blockIdx.x * (kRowThreads / 32) + (threadIdx.x >> 5);
   if (row >= T) return;
+  const int g = row_group(row, group_rows);
   int id = __ldg(ids + row);
   id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
   float4 v[NV];
-  row_load<NV>(table + static_cast<size_t>(id) * (NV * 128), v);
-  row_layernorm<NV>(v, w, nullptr, eps);
+  row_load<NV>(table.p[g] + static_cast<size_t>(id) * (NV * 128), v);
+  row_layernorm<NV>(v, w.p[g], nullptr, eps);
   if (x) row_store32<NV>(x + static_cast<size_t>(row) * (NV * 128), v);
   row_store16<NV>(h + static_cast<size_t>(row) * (NV * 128), v);
   if (lo) {   // residual stream as an fp16 pair (gemm.h: EPI_RESID_HL): lo = fp16(x - fp16(x))
@@ -113,39 +117,42 @@ __global__ void hl_to_f32_kernel(const __half* __restrict__ hi, const __half* __
 template <int NV>
 __global__ void __launch_bounds__(kRowThreads)
 embed_ln_bert_kernel(const int* __restrict__ ids, const int* __restrict__ pos, int T, int vocab, int max_pos,
-                     const float* __restrict__ word, const float* __restrict__ pos_emb,
-                     const float* __restrict__ type0, const float* __restrict__ w, const float* __restrict__ b,
-                     float eps, float* __restrict__ x, __half* __restrict__ h) {
+                     const __grid_constant__ RowGroups word, const __grid_constant__ RowGroups pos_emb,
+                     const __grid_constant__ RowGroups type0, const __grid_constant__ RowGroups w,
+                     const __grid_constant__ RowGroups b, int group_rows, float eps, float* __restrict__ x,
+                     __half* __restrict__ h) {
   const int row = blockIdx.x * (kRowThreads / 32) + (threadIdx.x >> 5);
   if (row >= T) return;
+  const int g = row_group(row, group_rows);
   int id = __ldg(ids + row);
   id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
   int p = __ldg(pos + row);
   p = p >= max_pos ? max_pos - 1 : p;
   float4 v[NV], a[NV];
-  row_load<NV>(word + static_cast<size_t>(id) * (NV * 128), v);
-  row_load<NV>(type0, a);   // reference order: word + token_type, then + position
+  row_load<NV>(word.p[g] + static_cast<size_t>(id) * (NV * 128), v);
+  row_load<NV>(type0.p[g], a);   // reference order: word + token_type, then + position
 #pragma unroll
   for (int i = 0; i < NV; ++i) { v[i].x += a[i].x; v[i].y += a[i].y; v[i].z += a[i].z; v[i].w += a[i].w; }
-  row_load<NV>(pos_emb + static_cast<size_t>(p) * (NV * 128), a);
+  row_load<NV>(pos_emb.p[g] + static_cast<size_t>(p) * (NV * 128), a);
 #pragma unroll
   for (int i = 0; i < NV; ++i) { v[i].x += a[i].x; v[i].y += a[i].y; v[i].z += a[i].z; v[i].w += a[i].w; }
-  row_layernorm<NV>(v, w, b, eps);
+  row_layernorm<NV>(v, w.p[g], b.p[g], eps);
   row_store32<NV>(x + static_cast<size_t>(row) * (NV * 128), v);
   row_store16<NV>(h + static_cast<size_t>(row) * (NV * 128), v);
 }
 
 template <int NV>
 __global__ void __launch_bounds__(kRowThreads)
-layernorm_kernel(const float* x, int T, const float* __restrict__ w, const float* __restrict__ b, float eps,
-                 float* y32, __half* __restrict__ y16) {
+layernorm_kernel(const float* x, int T, const __grid_constant__ RowGroups w, const __grid_constant__ RowGroups b,
+                 int group_rows, float eps, float* y32, __half* __restrict__ y16) {
   const int row = blockIdx.x * (kRowThreads / 32) + (threadIdx.x >> 5);
   if (row >= T) return;
+  const int g = row_group(row, group_rows);
   float4 v[NV];
   const float4* r4 = reinterpret_cast<const float4*>(x + static_cast<size_t>(row) * (NV * 128));
 #pragma unroll
   for (int i = 0; i < NV; ++i) v[i] = r4[i * 32 + lane_id()];
-  row_layernorm<NV>(v, w, b, eps);
+  row_layernorm<NV>(v, w.p[g], b.p[g], eps);
   if (y32) row_store32<NV>(y32 + static_cast<size_t>(row) * (NV * 128), v);
   if (y16) row_store16<NV>(y16 + static_cast<size_t>(row) * (NV * 128), v);
 }
@@ -461,9 +468,15 @@ int compute_positions(cudaStream_t stream, const int* cu_seqlens, int batch, int
 
 int embed_ln_modernbert(cudaStream_t stream, const int* ids, int T, int H, int vocab, const float* table,
                         const float* ln_w, float eps, float* x, __half* h, __half* lo) {
+  return embed_ln_modernbert(stream, ids, T, H, vocab, RowGroups::one(table), RowGroups::one(ln_w), 0, eps, x, h, lo);
+}
+
+int embed_ln_modernbert(cudaStream_t stream, const int* ids, int T, int H, int vocab, const RowGroups& table,
+                        const RowGroups& ln_w, int group_rows, float eps, float* x, __half* h, __half* lo) {
   if (T <= 0) return 0;
+  if (group_rows < 0 || (group_rows > 0 && (T + group_rows - 1) / group_rows > kMaxRowGroups)) return -1;
   SRB_DISPATCH_H(H, (embed_ln_mb_kernel<NV><<<row_blocks(T), kRowThreads, 0, stream>>>(ids, T, vocab, table, ln_w,
-                                                                                        eps, x, h, lo)));
+                                                                                        group_rows, eps, x, h, lo)));
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   return 0;
@@ -482,9 +495,17 @@ int hl_to_f32(cudaStream_t stream, const __half* hi, const __half* lo, const flo
 int embed_ln_bert(cudaStream_t stream, const int* ids, const int* pos, int T, int H, int vocab, int max_pos,
                   const float* word, const float* pos_emb, const float* type0, const float* ln_w,
                   const float* ln_b, float eps, float* x, __half* h) {
+  return embed_ln_bert(stream, ids, pos, T, H, vocab, max_pos, RowGroups::one(word), RowGroups::one(pos_emb),
+                       RowGroups::one(type0), RowGroups::one(ln_w), RowGroups::one(ln_b), 0, eps, x, h);
+}
+
+int embed_ln_bert(cudaStream_t stream, const int* ids, const int* pos, int T, int H, int vocab, int max_pos,
+                  const RowGroups& word, const RowGroups& pos_emb, const RowGroups& type0, const RowGroups& ln_w,
+                  const RowGroups& ln_b, int group_rows, float eps, float* x, __half* h) {
   if (T <= 0) return 0;
+  if (group_rows < 0 || (group_rows > 0 && (T + group_rows - 1) / group_rows > kMaxRowGroups)) return -1;
   SRB_DISPATCH_H(H, (embed_ln_bert_kernel<NV><<<row_blocks(T), kRowThreads, 0, stream>>>(
-                        ids, pos, T, vocab, max_pos, word, pos_emb, type0, ln_w, ln_b, eps, x, h)));
+                        ids, pos, T, vocab, max_pos, word, pos_emb, type0, ln_w, ln_b, group_rows, eps, x, h)));
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   return 0;
@@ -492,8 +513,15 @@ int embed_ln_bert(cudaStream_t stream, const int* ids, const int* pos, int T, in
 
 int layernorm_rows(cudaStream_t stream, const float* x, int T, int H, const float* w, const float* b, float eps,
                    float* y32, __half* y16) {
+  return layernorm_rows(stream, x, T, H, RowGroups::one(w), RowGroups::one(b), 0, eps, y32, y16);
+}
+
+int layernorm_rows(cudaStream_t stream, const float* x, int T, int H, const RowGroups& w, const RowGroups& b,
+                   int group_rows, float eps, float* y32, __half* y16) {
   if (T <= 0) return 0;
-  SRB_DISPATCH_H(H, (layernorm_kernel<NV><<<row_blocks(T), kRowThreads, 0, stream>>>(x, T, w, b, eps, y32, y16)));
+  if (group_rows < 0 || (group_rows > 0 && (T + group_rows - 1) / group_rows > kMaxRowGroups)) return -1;
+  SRB_DISPATCH_H(H, (layernorm_kernel<NV><<<row_blocks(T), kRowThreads, 0, stream>>>(x, T, w, b, group_rows, eps, y32,
+                                                                                      y16)));
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   return 0;

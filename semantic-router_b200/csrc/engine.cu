@@ -247,6 +247,7 @@ struct Loader {
       return nullptr;
     }
     m->allocs.push_back(p);
+    m->weight_bytes += bytes;
     return p;
   }
   bool host_f32(const std::string& name, std::vector<float>& out, const std::vector<int64_t>& shape,
@@ -269,9 +270,7 @@ struct Loader {
     return true;
   }
   double lora_alpha = 32.0;   // LoRAConfig::default (lora_adapter.rs:29-38); <dir>/lora_config.json {"alpha", "rank"} overrides
-  bool keep_adapters = false; // shared-LoRA models: the base weights load unmerged
   bool merge_lora(const std::string& name, const StTensor& base, std::vector<float>& w) {
-    if (keep_adapters) return true;
     std::string e;
     if (!lora_fold(*st, name, base, lora_alpha, w, &e)) { fail(e); return false; }
     return true;
@@ -344,6 +343,66 @@ bool tensor_prefix(const SafeTensors& st, Arch arch, std::string& P) {
 
 std::string layer_prefix(const EncoderConfig& c, const std::string& P, int li) {
   return P + (c.arch == ARCH_MODERNBERT ? "layers." : "encoder.layer.") + std::to_string(li) + ".";
+}
+
+// config.json and the checkpoint's tensor names -> the encoder's shape and its tensor-name prefix P.  false: *err says why
+// the checkpoint cannot be served.  Host only.
+bool read_encoder_config(const Json& cfgj, const SafeTensors& st, EncoderConfig& c, std::string& P, std::string* err) {
+  std::string e;
+  const std::string mt = cfgj.str_or("model_type", "");
+  c.arch = (mt == "modernbert" || tensor_prefix(st, ARCH_MODERNBERT, P)) ? ARCH_MODERNBERT : ARCH_BERT;
+  if (!tensor_prefix(st, c.arch, P))
+    e = c.arch == ARCH_MODERNBERT ? "no tok_embeddings tensor under any known prefix" : "no BERT word_embeddings tensor found";
+  c.vocab = static_cast<int>(cfgj.num_or("vocab_size", 0));
+  c.H = static_cast<int>(cfgj.num_or("hidden_size", 0));
+  c.L = static_cast<int>(cfgj.num_or("num_hidden_layers", 0));
+  c.heads = static_cast<int>(cfgj.num_or("num_attention_heads", 0));
+  c.I = static_cast<int>(cfgj.num_or("intermediate_size", 0));
+  c.max_pos = static_cast<int>(cfgj.num_or("max_position_embeddings", 512));
+  c.pad_id = static_cast<int>(cfgj.num_or("pad_token_id", 0));
+  if (c.arch == ARCH_MODERNBERT) {
+    c.ln_eps = static_cast<float>(cfgj.num_or("layer_norm_eps", cfgj.num_or("norm_eps", 1e-5)));
+    c.global_every = static_cast<int>(cfgj.num_or("global_attn_every_n_layers", 3));
+    c.theta_global = cfgj.num_or("global_rope_theta", 160000.0);
+    c.theta_local = cfgj.num_or("local_rope_theta", 10000.0);
+    c.local_attention = static_cast<int>(cfgj.num_or("local_attention", 128));
+    if (const Json* cp = cfgj.get("classifier_pooling")) c.cls_pooling = (cp->is_str() && cp->str == "mean") ? 1 : 0;
+  } else {
+    c.ln_eps = static_cast<float>(cfgj.num_or("layer_norm_eps", 1e-12));
+    c.type_vocab = static_cast<int>(cfgj.num_or("type_vocab_size", 2));
+  }
+  parse_id2label(cfgj, c.id2label);
+  if (e.empty() && (c.H <= 0 || c.L <= 0 || c.heads <= 0 || c.vocab <= 0 || c.I <= 0)) e = "config.json incomplete";
+  const int head_dim = (c.heads > 0) ? c.H / c.heads : 0;
+  if (e.empty() && (c.H % (c.heads > 0 ? c.heads : 1) != 0 || !(head_dim == 64 || (head_dim == 32 && c.arch == ARCH_BERT))))
+    e = "head_dim " + std::to_string(head_dim) + " unsupported (64; 32 for BERT/MiniLM encoders)";
+  c.attn_w = c.heads * 64;
+  if (e.empty() && !(c.H == 384 || c.H == 768 || c.H == 1024)) e = "hidden_size unsupported";
+  // gemm_f16 refuses EPI_GEGLU unless N = 2 I is a multiple of 128 (its host check, not the tile walk: the kernel stores
+  // 64-column (a | b) groups one by one).  Whether that check can be relaxed is unmeasured; until then such a model is
+  // refused here instead of failing in every forward.
+  if (e.empty() && c.arch == ARCH_MODERNBERT && c.I % 64 != 0) e = "intermediate_size must be a multiple of 64";
+  if (!e.empty()) { *err = e; return false; }
+  return true;
+}
+
+// model_load's device requirements: an sm_90 device at index `device`, made current
+bool use_device(int device, std::string* err) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    *err = "no CUDA device available (this library has no CPU path)";
+    return false;
+  }
+  if (device < 0 || device >= ndev) { *err = "invalid device index " + std::to_string(device); return false; }
+  cudaDeviceProp prop;
+  cudaGetDeviceProperties(&prop, device);
+  if (prop.major != 9 || prop.minor != 0) {
+    *err = std::string("device ") + prop.name + " is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) +
+           "; this library is built for sm_90a only";
+    return false;
+  }
+  if (cudaSetDevice(device) != cudaSuccess) { *err = "cudaSetDevice failed"; return false; }
+  return true;
 }
 
 // One encoder projection: how the checkpoint stores it and how the kernels read it.
@@ -454,7 +513,7 @@ bool device_projection(Loader& ld, const Projection& pr, std::vector<float>& w, 
 // W'' = W diag(gamma), every row re-centred to sum zero, rounded to fp16.  Two refinement passes push the sum of the
 // ROUNDED row (what the tensor core multiplies) from ~1e-4 down to the last bit of its largest elements, so the
 // residual mean * sum(W''[n,:]) is far below the fp16 rounding of the output.
-__half* fold_weights(Loader& ld, const std::vector<float>& w, const std::vector<float>& gamma, int n, int k) {
+std::vector<float> fold_weights(const std::vector<float>& w, const std::vector<float>& gamma, int n, int k) {
   std::vector<float> wf(w.size());
   std::vector<double> row(k);
   for (int r = 0; r < n; ++r) {
@@ -470,33 +529,50 @@ __half* fold_weights(Loader& ld, const std::vector<float>& w, const std::vector<
     }
     for (int c = 0; c < k; ++c) wf[static_cast<size_t>(r) * k + c] = static_cast<float>(row[c]);
   }
-  return ld.up_f16(wf);
+  return wf;
 }
 
-// fp16 upload of `rows` device rows of K-wide weights, folded with `gamma` when it names a LayerNorm weight
-__half* upload_weight(Loader& ld, const std::vector<float>& w, const std::string& gamma, int rows, int K) {
-  if (gamma.empty()) return ld.up_f16(w);
+// device_projection, then folded with the projection's LayerNorm gamma when it names one: the fp32 host form of what the
+// device multiplies
+bool device_weight(Loader& ld, const Projection& pr, std::vector<float>& w, std::vector<float>* bias) {
+  if (!device_projection(ld, pr, w, bias)) return false;
+  if (pr.gamma.empty()) return true;
   std::vector<float> g;
-  return ld.host_f32(gamma, g, {K}) ? fold_weights(ld, w, g, rows, K) : nullptr;
+  if (!ld.host_f32(pr.gamma, g, {pr.dK})) return false;
+  w = fold_weights(w, g, pr.dN, pr.dK);
+  return true;
 }
 
-// Device form of projection p of a layer: uploads `w` (T stacked device weights for a shared-LoRA model) into the plain or
-// the folded slot
-void store_projection(Loader& ld, const Projection& pr, int p, const std::vector<float>& w, int copies, LayerWeights& lw) {
+// fp16 upload of projection p of a layer (the device weights of one task, or of several stacked along N) into its plain
+// or its folded slot, and of its bias
+void store_projection(Loader& ld, const Projection& pr, int p, const std::vector<float>& w, const std::vector<float>& b,
+                      LayerWeights& lw) {
   __half** plain[] = {&lw.wqkv, &lw.wo, &lw.wi, &lw.wo2};
-  __half** slot = pr.gamma.empty() ? plain[p] : (p == 0 ? &lw.wqkv_f : &lw.wi_f);
-  *slot = upload_weight(ld, w, pr.gamma, copies * pr.dN, pr.dK);
+  float** biases[] = {&lw.bqkv, &lw.bo, &lw.bi, &lw.bo2};
+  *(pr.gamma.empty() ? plain[p] : (p == 0 ? &lw.wqkv_f : &lw.wi_f)) = ld.up_f16(w);
+  if (pr.bias) *biases[p] = ld.up_f32(b);
 }
 
 // The ordinary model: the four projections of one layer (and BERT's biases) from the loader's checkpoint
 void load_projections(Loader& ld, const std::array<Projection, 4>& pr, LayerWeights& lw) {
-  float** biases[] = {&lw.bqkv, &lw.bo, &lw.bi, &lw.bo2};
   for (int p = 0; p < 4 && ld.ok; ++p) {
     std::vector<float> w, b;
-    if (!device_projection(ld, pr[p], w, pr[p].bias ? &b : nullptr)) return;
-    store_projection(ld, pr[p], p, w, 1, lw);
-    if (pr[p].bias) *biases[p] = ld.up_f32(b);
+    if (!device_weight(ld, pr[p], w, pr[p].bias ? &b : nullptr)) return;
+    store_projection(ld, pr[p], p, w, b, lw);
   }
+}
+
+// ModernBERT's rotary tables for both thetas, max_position_embeddings rows
+void load_rope(Loader& ld, Model& m) {
+  const EncoderConfig& c = m.cfg;
+  m.rope_len = c.max_pos;
+  std::vector<float> cs, sn;
+  rope_tables(64, c.theta_global, c.max_pos, cs, sn);
+  m.rope_cos_g = ld.up_f32(cs);
+  m.rope_sin_g = ld.up_f32(sn);
+  rope_tables(64, c.theta_local, c.max_pos, cs, sn);
+  m.rope_cos_l = ld.up_f32(cs);
+  m.rope_sin_l = ld.up_f32(sn);
 }
 
 bool load_head(Loader& ld, const Json& cfgj, Arch arch, int H, const std::string& bert_prefix,
@@ -540,22 +616,9 @@ bool load_head(Loader& ld, const Json& cfgj, Arch arch, int H, const std::string
 // ------------------------------------------------------------------------------------------------
 // model load
 // ------------------------------------------------------------------------------------------------
-Model* model_load(const std::string& dir, int device, std::string* err, int flags) {
+Model* model_load(const std::string& dir, int device, std::string* err) {
   std::string e;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    *err = "no CUDA device available (this library has no CPU path)";
-    return nullptr;
-  }
-  if (device < 0 || device >= ndev) { *err = "invalid device index " + std::to_string(device); return nullptr; }
-  cudaDeviceProp prop;
-  cudaGetDeviceProperties(&prop, device);
-  if (prop.major != 9 || prop.minor != 0) {
-    *err = std::string("device ") + prop.name + " is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) +
-           "; this library is built for sm_90a only";
-    return nullptr;
-  }
-  if (cudaSetDevice(device) != cudaSuccess) { *err = "cudaSetDevice failed"; return nullptr; }
+  if (!use_device(device, err)) return nullptr;
 
   Json cfgj;
   if (!parse_json_file(dir + "/config.json", cfgj)) { *err = "cannot read " + dir + "/config.json"; return nullptr; }
@@ -567,45 +630,12 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
   m->dir = dir;
   Loader ld{m, &st};
   ld.lora_alpha = lora_alpha_of(dir);
-  ld.keep_adapters = (flags & kLoadKeepAdapters) != 0;
   EncoderConfig& c = m->cfg;
-  const std::string mt = cfgj.str_or("model_type", "");
   std::string P;  // tensor-name prefix
-  c.arch = (mt == "modernbert" || tensor_prefix(st, ARCH_MODERNBERT, P)) ? ARCH_MODERNBERT : ARCH_BERT;
-  if (!tensor_prefix(st, c.arch, P))
-    ld.fail(c.arch == ARCH_MODERNBERT ? "no tok_embeddings tensor under any known prefix" : "no BERT word_embeddings tensor found");
-  c.vocab = static_cast<int>(cfgj.num_or("vocab_size", 0));
-  c.H = static_cast<int>(cfgj.num_or("hidden_size", 0));
-  c.L = static_cast<int>(cfgj.num_or("num_hidden_layers", 0));
-  c.heads = static_cast<int>(cfgj.num_or("num_attention_heads", 0));
-  c.I = static_cast<int>(cfgj.num_or("intermediate_size", 0));
-  c.max_pos = static_cast<int>(cfgj.num_or("max_position_embeddings", 512));
-  c.pad_id = static_cast<int>(cfgj.num_or("pad_token_id", 0));
-  if (c.arch == ARCH_MODERNBERT) {
-    c.ln_eps = static_cast<float>(cfgj.num_or("layer_norm_eps", cfgj.num_or("norm_eps", 1e-5)));
-    c.global_every = static_cast<int>(cfgj.num_or("global_attn_every_n_layers", 3));
-    c.theta_global = cfgj.num_or("global_rope_theta", 160000.0);
-    c.theta_local = cfgj.num_or("local_rope_theta", 10000.0);
-    c.local_attention = static_cast<int>(cfgj.num_or("local_attention", 128));
-    if (const Json* cp = cfgj.get("classifier_pooling")) c.cls_pooling = (cp->is_str() && cp->str == "mean") ? 1 : 0;
-  } else {
-    c.ln_eps = static_cast<float>(cfgj.num_or("layer_norm_eps", 1e-12));
-    c.type_vocab = static_cast<int>(cfgj.num_or("type_vocab_size", 2));
-  }
-  parse_id2label(cfgj, c.id2label);
-  if (ld.ok && (c.H <= 0 || c.L <= 0 || c.heads <= 0 || c.vocab <= 0 || c.I <= 0)) ld.fail("config.json incomplete");
-  const int head_dim = (c.heads > 0) ? c.H / c.heads : 0;
-  if (ld.ok && (c.H % (c.heads > 0 ? c.heads : 1) != 0 || !(head_dim == 64 || (head_dim == 32 && c.arch == ARCH_BERT))))
-    ld.fail("head_dim " + std::to_string(head_dim) + " unsupported (64; 32 for BERT/MiniLM encoders)");
-  c.attn_w = c.heads * 64;
-  if (ld.ok && !(c.H == 384 || c.H == 768 || c.H == 1024)) ld.fail("hidden_size unsupported");
+  if (!read_encoder_config(cfgj, st, c, P, &e)) ld.fail(e);
 
-  const int H = c.H, I = c.I;
+  const int H = c.H;
   if (ld.ok && c.arch == ARCH_MODERNBERT) {
-    // gemm_f16 refuses EPI_GEGLU unless N = 2 I is a multiple of 128 (its host check, not the tile walk: the kernel stores
-    // 64-column (a | b) groups one by one).  Whether that check can be relaxed is unmeasured; until then such a model is
-    // refused here instead of failing in every forward.
-    if (I % 64 != 0) ld.fail("intermediate_size must be a multiple of 64");
     m->emb_word = ld.f32(P + "embeddings.tok_embeddings.weight", {c.vocab, H});
     m->emb_ln_w = ld.f32(P + "embeddings.norm.weight", {H});
     m->layers.resize(c.L);
@@ -617,16 +647,7 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
       load_projections(ld, layer_projections(c, P, li, lw.attn_norm_w != nullptr), lw);
     }
     m->final_norm_w = ld.f32(P + "final_norm.weight", {H});
-    if (ld.ok) {
-      m->rope_len = c.max_pos;
-      std::vector<float> cs, sn;
-      rope_tables(64, c.theta_global, c.max_pos, cs, sn);
-      m->rope_cos_g = ld.up_f32(cs);
-      m->rope_sin_g = ld.up_f32(sn);
-      rope_tables(64, c.theta_local, c.max_pos, cs, sn);
-      m->rope_cos_l = ld.up_f32(cs);
-      m->rope_sin_l = ld.up_f32(sn);
-    }
+    if (ld.ok) load_rope(ld, *m);
   } else if (ld.ok) {
     const std::string E = P + "embeddings.";
     m->emb_word = ld.f32(E + "word_embeddings.weight", {c.vocab, H});
@@ -649,7 +670,7 @@ Model* model_load(const std::string& dir, int device, std::string* err, int flag
       lw.out_norm_b = ld.f32(Lp + "output.LayerNorm.bias", {H});
     }
   }
-  if (ld.ok && !(flags & kLoadNoHead) && st.find("classifier.weight")) {
+  if (ld.ok && st.find("classifier.weight")) {
     Head hd;
     if (load_head(ld, cfgj, c.arch, H, P, -1, hd)) m->heads.push_back(hd);
   }
@@ -684,24 +705,205 @@ int model_add_head(Model* m, const std::string& dir, int force_token_level, std:
 
 
 // ------------------------------------------------------------------------------------------------
-// shared-base multi-task model from unmerged LoRA checkpoints (engine.h: LoraShared)
+// grouped model: several task checkpoints of one encoder in one pass (engine.h: Grouped)
 // ------------------------------------------------------------------------------------------------
 namespace {
 bool is_head_tensor(const std::string& n) {
   return n.compare(0, 11, "classifier.") == 0 || n.compare(0, 5, "head.") == 0 || n.find("pooler.") != std::string::npos;
 }
+
+std::string num_text(double v) {
+  char b[32];
+  snprintf(b, sizeof b, "%.9g", v);
+  return b;
+}
+// the EncoderConfig fields every task of a grouped model must share, by their config.json names
+std::vector<std::pair<const char*, std::string>> shape_fields(const EncoderConfig& c) {
+  return {{"architecture", c.arch == ARCH_MODERNBERT ? "modernbert" : "bert"},
+          {"hidden_size", num_text(c.H)},
+          {"num_hidden_layers", num_text(c.L)},
+          {"num_attention_heads", num_text(c.heads)},
+          {"intermediate_size", num_text(c.I)},
+          {"vocab_size", num_text(c.vocab)},
+          {"max_position_embeddings", num_text(c.max_pos)},
+          {"global_attn_every_n_layers", num_text(c.global_every)},
+          {"local_attention", num_text(c.local_attention)},
+          {"global_rope_theta", num_text(c.theta_global)},
+          {"local_rope_theta", num_text(c.theta_local)},
+          {"layer_norm_eps", num_text(c.ln_eps)},
+          {"classifier_pooling", c.cls_pooling ? "mean" : "cls"}};
+}
+
+bool has_adapter(const SafeTensors& st, const std::string& name) {
+  const std::string suffix = ".weight";
+  if (name.size() <= suffix.size() || name.compare(name.size() - suffix.size(), suffix.size(), suffix) != 0) return false;
+  const std::string stem = name.substr(0, name.size() - suffix.size());
+  return st.find(stem + ".lora_A.weight") || st.find(stem + ".lora_B.weight");
+}
+
+// One tensor of every task: names[t] in task t's checkpoint (the prefixes may differ).  A task whose tensor is bitwise
+// that of an earlier task (neither with adapters) shares that task's device copy; `rows` > 0 keeps the first rows only.
+// Missing and not required: null for that task.
+std::vector<float*> load_each(std::vector<Loader>& lt, const std::vector<std::string>& names,
+                              const std::vector<int64_t>& shape, bool required = true, int64_t rows = 0) {
+  const size_t T = lt.size();
+  std::vector<float*> out(T, nullptr);
+  std::vector<float> v;
+  for (size_t t = 0; t < T && lt[t].ok; ++t) {
+    const SafeTensors& st = *lt[t].st;
+    const StTensor* a = st.find(names[t]);
+    if (!a && !required) continue;
+    bool shared = false;
+    for (size_t u = 0; u < t && a && !shared; ++u) {
+      const StTensor* b = lt[u].st->find(names[u]);
+      if (b && out[u] && a->dtype == b->dtype && a->shape == b->shape && a->bytes == b->bytes &&
+          memcmp(a->data, b->data, a->bytes) == 0 && !has_adapter(st, names[t]) && !has_adapter(*lt[u].st, names[u])) {
+        out[t] = out[u];
+        shared = true;
+      }
+    }
+    if (shared || !lt[t].host_f32(names[t], v, shape)) continue;
+    if (rows > 0 && !shape.empty()) v.resize(static_cast<size_t>(rows) * (v.size() / shape[0]));
+    out[t] = lt[t].up_f32(v);
+  }
+  return out;
+}
 }  // namespace
+
+Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
+                          std::string* err) {
+  const int T = static_cast<int>(dirs.size());
+  if (T < 1 || T > kMaxRowGroups) { *err = "a grouped model takes 1 to " + std::to_string(kMaxRowGroups) + " task checkpoints"; return nullptr; }
+  if (token_level.size() != dirs.size()) { *err = "one token_level per task checkpoint"; return nullptr; }
+  // every refusal of the directories first, on the host
+  std::vector<Json> cfgj(T);
+  std::vector<std::unique_ptr<SafeTensors>> sts;
+  std::vector<EncoderConfig> cfg(T);
+  std::vector<std::string> P(T);
+  for (int t = 0; t < T; ++t) {
+    const std::string& d = dirs[t];
+    if (!parse_json_file(d + "/config.json", cfgj[t])) { *err = "cannot read " + d + "/config.json"; return nullptr; }
+    sts.emplace_back(new SafeTensors());
+    std::string e;
+    if (!sts.back()->open(d + "/model.safetensors", &e)) { *err = e; return nullptr; }
+    if (!read_encoder_config(cfgj[t], *sts[t], cfg[t], P[t], &e)) { *err = d + ": " + e; return nullptr; }
+    if (cfg[t].attn_w != cfg[t].H) { *err = d + ": grouped serving is not available for padded-head (MiniLM) encoders"; return nullptr; }
+    const auto f0 = shape_fields(cfg[0]), ft = shape_fields(cfg[t]);
+    for (size_t i = 0; i < f0.size(); ++i)
+      if (f0[i].second != ft[i].second) {
+        *err = std::string("the checkpoints do not share one encoder shape: ") + f0[i].first + " is " + ft[i].second + " in " + d +
+               " and " + f0[i].second + " in " + dirs[0];
+        return nullptr;
+      }
+    if (!sts[t]->find("classifier.weight")) { *err = "no classifier.weight in " + d; return nullptr; }
+  }
+  if (!use_device(device, err)) return nullptr;
+
+  Model* m = new Model();
+  m->device = device;
+  m->dir = dirs[0];
+  m->cfg = cfg[0];
+  const EncoderConfig& c = m->cfg;
+  const int H = c.H;
+  std::vector<Loader> lt;
+  for (int t = 0; t < T; ++t) {
+    lt.push_back(Loader{m, sts[t].get()});
+    lt.back().lora_alpha = lora_alpha_of(dirs[t]);   // adapters are merged as model_load merges them
+  }
+  auto ok = [&]() {
+    for (const Loader& l : lt)
+      if (!l.ok) { *err = l.err; return false; }
+    return true;
+  };
+  auto names = [&](const std::string& rest, int li = -1) {   // `rest` under every task's prefix (and layer li)
+    std::vector<std::string> n(T);
+    for (int t = 0; t < T; ++t) n[t] = (li < 0 ? P[t] : layer_prefix(c, P[t], li)) + rest;
+    return n;
+  };
+  Grouped& g = m->group;
+  g.task.resize(T);
+  for (TaskTensors& tt : g.task) tt.layers.resize(c.L);
+  auto each = [&](std::vector<float*> v, float* TaskTensors::*f) { for (int t = 0; t < T; ++t) g.task[t].*f = v[t]; };
+  auto each_layer = [&](std::vector<float*> v, int li, float* TaskNorms::*f) { for (int t = 0; t < T; ++t) g.task[t].layers[li].*f = v[t]; };
+  if (c.arch == ARCH_MODERNBERT) {
+    each(load_each(lt, names("embeddings.tok_embeddings.weight"), {c.vocab, H}), &TaskTensors::emb_word);
+    each(load_each(lt, names("embeddings.norm.weight"), {H}), &TaskTensors::emb_ln_w);
+    for (int li = 0; li < c.L && ok(); ++li) {
+      each_layer(load_each(lt, names("attn_norm.weight", li), {H}, false), li, &TaskNorms::attn_w);
+      each_layer(load_each(lt, names("mlp_norm.weight", li), {H}), li, &TaskNorms::mid_w);
+      for (int t = 1; t < T && ok(); ++t)
+        if ((g.task[t].layers[li].attn_w != nullptr) != (g.task[0].layers[li].attn_w != nullptr)) {
+          *err = "layer " + std::to_string(li) + " has an attn_norm in " + dirs[g.task[0].layers[li].attn_w ? 0 : t] +
+                 " but not in " + dirs[g.task[0].layers[li].attn_w ? t : 0];
+          model_free(m);
+          return nullptr;
+        }
+    }
+    each(load_each(lt, names("final_norm.weight"), {H}), &TaskTensors::final_norm_w);
+    if (ok()) load_rope(lt[0], *m);
+  } else {
+    each(load_each(lt, names("embeddings.word_embeddings.weight"), {c.vocab, H}), &TaskTensors::emb_word);
+    each(load_each(lt, names("embeddings.position_embeddings.weight"), {c.max_pos, H}), &TaskTensors::emb_pos);
+    // token_type_ids are always zero (traditional/bert.rs:227): row 0 only
+    each(load_each(lt, names("embeddings.token_type_embeddings.weight"), {c.type_vocab, H}, true, 1), &TaskTensors::emb_type0);
+    each(load_each(lt, names("embeddings.LayerNorm.weight"), {H}), &TaskTensors::emb_ln_w);
+    each(load_each(lt, names("embeddings.LayerNorm.bias"), {H}), &TaskTensors::emb_ln_b);
+    for (int li = 0; li < c.L && ok(); ++li) {
+      each_layer(load_each(lt, names("attention.output.LayerNorm.weight", li), {H}), li, &TaskNorms::mid_w);
+      each_layer(load_each(lt, names("attention.output.LayerNorm.bias", li), {H}), li, &TaskNorms::mid_b);
+      each_layer(load_each(lt, names("output.LayerNorm.weight", li), {H}), li, &TaskNorms::out_w);
+      each_layer(load_each(lt, names("output.LayerNorm.bias", li), {H}), li, &TaskNorms::out_b);
+    }
+  }
+  // projections: every task's device weights (its own gamma folded in) and biases, stacked along N
+  m->layers.resize(c.L);
+  for (int li = 0; li < c.L && ok(); ++li) {
+    std::vector<std::array<Projection, 4>> pr;
+    for (int t = 0; t < T; ++t) pr.push_back(layer_projections(c, P[t], li, g.task[t].layers[li].attn_w != nullptr));
+    for (int p = 0; p < 4 && ok(); ++p) {
+      std::vector<float> stack, bstack, w, b;
+      for (int t = 0; t < T && ok(); ++t) {
+        if (!device_weight(lt[t], pr[t][p], w, pr[t][p].bias ? &b : nullptr)) break;
+        stack.insert(stack.end(), w.begin(), w.end());
+        bstack.insert(bstack.end(), b.begin(), b.end());
+      }
+      if (ok()) store_projection(lt[0], pr[0][p], p, stack, bstack, m->layers[li]);
+    }
+  }
+  for (int t = 0; t < T && ok(); ++t) {
+    Head hd;
+    if (!load_head(lt[t], cfgj[t], c.arch, H, P[t], token_level[t], hd)) {
+      if (lt[t].ok) lt[t].fail("classifier.weight of " + dirs[t] + " does not fit hidden_size");
+      break;
+    }
+    hd.final_norm_w = g.task[t].final_norm_w;
+    m->heads.push_back(hd);
+    g.head_of_task.push_back(t);
+  }
+  if (ok() && cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess) lt[0].fail("stream create failed");
+  if (!ok()) { model_free(m); return nullptr; }
+  // outside a grouped pass the model is task 0: its tensors, and the first matrix / bias of every stack
+  const TaskTensors& t0 = g.task[0];
+  m->emb_word = t0.emb_word; m->emb_pos = t0.emb_pos; m->emb_type0 = t0.emb_type0;
+  m->emb_ln_w = t0.emb_ln_w; m->emb_ln_b = t0.emb_ln_b; m->final_norm_w = t0.final_norm_w;
+  for (int li = 0; li < c.L; ++li) {
+    LayerWeights& lw = m->layers[li];
+    const TaskNorms& n = t0.layers[li];
+    lw.attn_norm_w = n.attn_w; lw.mid_norm_w = n.mid_w; lw.mid_norm_b = n.mid_b; lw.out_norm_w = n.out_w; lw.out_norm_b = n.out_b;
+  }
+  g.tasks = T;
+  cudaDeviceSynchronize();
+  return m;
+}
 
 Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
                               std::string* err) {
   const int T = static_cast<int>(dirs.size());
   if (T < 1 || token_level.size() != dirs.size()) { *err = "bad arguments"; return nullptr; }
   std::vector<std::unique_ptr<SafeTensors>> sts;
-  std::vector<double> alpha;
   for (const std::string& d : dirs) {
     sts.emplace_back(new SafeTensors());
     if (!sts.back()->open(d + "/model.safetensors", err)) return nullptr;
-    alpha.push_back(lora_alpha_of(d));
   }
   // one base: every non-adapter, non-head tensor of task 0 must sit, bit for bit, in the other checkpoints
   int max_rank = 0;
@@ -722,38 +924,9 @@ Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::v
         max_rank = std::max(max_rank, static_cast<int>(kv.second.shape[0]));
   if (max_rank <= 0) { *err = "no lora_A / lora_B tensors in these checkpoints (merged models load as separate slots)"; return nullptr; }
   if (max_rank > 256) { *err = "LoRA rank above 256"; return nullptr; }
-  Model* m = model_load(dirs[0], device, err, kLoadKeepAdapters | kLoadNoHead);
-  if (!m) return nullptr;
-  const EncoderConfig& c = m->cfg;
-  if (c.attn_w != c.H) { *err = "shared-LoRA serving is not available for padded-head (MiniLM) encoders"; model_free(m); return nullptr; }
-  Loader ld{m, sts[0].get()};
-  std::string P;
-  tensor_prefix(*sts[0], c.arch, P);
-  m->lora.glayers = m->layers;   // norms / biases are the base's (adapters touch projection weights only)
-  for (int li = 0; li < c.L && ld.ok; ++li) {
-    const auto pr = layer_projections(c, P, li, m->layers[li].attn_norm_w != nullptr);
-    for (int p = 0; p < 4 && ld.ok; ++p) {
-      // every task's merged weights, stacked along N.  Loader{.., sts[t]} merges task t's adapters exactly as a separately
-      // loaded model would (lora_fold, double precision, before the fp16 rounding).
-      std::vector<float> stack, w;
-      for (int t = 0; t < T && ld.ok; ++t) {
-        Loader lt{m, sts[t].get()};
-        lt.lora_alpha = alpha[t];
-        if (!device_projection(lt, pr[p], w, nullptr)) ld.fail(lt.err);
-        stack.insert(stack.end(), w.begin(), w.end());
-      }
-      if (ld.ok) store_projection(ld, pr[p], p, stack, T, m->lora.glayers[li]);
-    }
-  }
-  if (!ld.ok) { *err = ld.err; model_free(m); return nullptr; }
-  for (int t = 0; t < T; ++t) {
-    const int h = model_add_head(m, dirs[t], token_level[t], err);
-    if (h < 0) { model_free(m); return nullptr; }
-    m->lora.head_of_task.push_back(h);
-  }
-  m->lora.tasks = T;
-  cudaDeviceSynchronize();
-  return m;
+  // every task's adapters merged into its own copy of the projections (lora_fold, double precision, before the fp16
+  // rounding), the base's other tensors once
+  return model_load_grouped(dirs, token_level, device, err);
 }
 
 // 1: <dir>/model.safetensors carries lora_A / lora_B tensors; 0: it does not; -1: unreadable
@@ -909,14 +1082,26 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
   GemmDesc g;
   g.M = T;
   g.a_rows = w.cap_tokens;
-  // shared-LoRA pass (engine.h: LoraShared): every projection GEMM picks the task's matrix per row block (gemm.h: w_groups)
-  const bool grouped = m.lora.tasks > 0 && m.lora.rows_per_task > 0;
-  if (grouped && (T != m.lora.tasks * m.lora.rows_per_task || m.lora.rows_per_task % 256 != 0 ||
-                  static_cast<int>(m.lora.glayers.size()) != c.L))
-    return -1;
+  // grouped pass (engine.h: Grouped): every projection GEMM picks the task's matrix and bias per row block (gemm.h:
+  // w_groups), every row kernel the task's embeddings and norms (kernels.h: RowGroups)
+  const Grouped& gp = m.group;
+  const bool grouped = gp.tasks > 0 && gp.rows_per_task > 0;
+  if (grouped && (T != gp.tasks * gp.rows_per_task || gp.rows_per_task % 256 != 0)) return -1;
+  const int group_rows = grouped ? gp.rows_per_task : 0;
   auto run_proj = [&](GemmDesc& gd) {
-    if (grouped) { gd.w_groups = m.lora.tasks; gd.w_group_rows = m.lora.rows_per_task; }
+    if (grouped) { gd.w_groups = gp.tasks; gd.w_group_rows = gp.rows_per_task; gd.bias_per_group = true; }
     return gemm_f16(s, gd);
+  };
+  // a task tensor per row group; outside a grouped pass the model's own (task 0's)
+  auto per_task = [&](float* TaskTensors::*f, const float* own) {
+    RowGroups r = RowGroups::one(own);
+    for (int t = 0; grouped && t < gp.tasks; ++t) r.p[t] = gp.task[t].*f;
+    return r;
+  };
+  auto per_task_norm = [&](int li, float* TaskNorms::*f, const float* own) {
+    RowGroups r = RowGroups::one(own);
+    for (int t = 0; grouped && t < gp.tasks; ++t) r.p[t] = gp.task[t].layers[li].*f;
+    return r;
   };
   if (c.arch == ARCH_MODERNBERT) {
     // Residual stream as an fp16 pair (gemm.h: EPI_RESID_HL): w.h / w.lo hold x - pivot, the residual GEMMs update the
@@ -926,7 +1111,9 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
     // Layer 0's attn_norm (when the checkpoint has one) is the exception: it runs on the fp32 embedding output.
     const bool ln0 = m.layers[0].attn_norm_w != nullptr;
     { ProfScope ps(m, PC_EMBED);
-      if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, m.emb_word, m.emb_ln_w, c.ln_eps, ln0 ? w.x : nullptr, w.h, w.lo)) return -1; }
+      if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, per_task(&TaskTensors::emb_word, m.emb_word),
+                              per_task(&TaskTensors::emb_ln_w, m.emb_ln_w), group_rows, c.ln_eps, ln0 ? w.x : nullptr, w.h, w.lo))
+        return -1; }
     // one statistics record [H/128][T][2] partials + [T] pivots, padded so that the second record keeps the float2
     // alignment of the partials; the residual GEMMs ping-pong between the two
     const size_t rec = (static_cast<size_t>(T) * (2 * static_cast<size_t>(H / 128) + 1) + 3) & ~static_cast<size_t>(3);
@@ -946,7 +1133,7 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       ++n_rec;
     };
     for (int li = 0; li < L; ++li) {
-      const LayerWeights& lw = grouped ? m.lora.glayers[li] : m.layers[li];
+      const LayerWeights& lw = m.layers[li];
       const bool local = (li % c.global_every) != 0;
       const bool folded = lw.wqkv_f != nullptr;   // model_load: li > 0 with attn_norm
       g = GemmDesc();
@@ -958,7 +1145,9 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
         // this layer's attention has not written it yet)
         ProfScope ps(m, PC_NORM);
         if (li == 0) {
-          if (layernorm_rows(s, w.x, T, H, lw.attn_norm_w, nullptr, c.ln_eps, nullptr, w.ctx)) return -1;
+          if (layernorm_rows(s, w.x, T, H, per_task_norm(0, &TaskNorms::attn_w, lw.attn_norm_w), RowGroups::one(nullptr),
+                             group_rows, c.ln_eps, nullptr, w.ctx))
+            return -1;
         } else {
           if (hl_to_f32(s, w.h, w.lo, cur_stats + piv_off, T, H, w.x)) return -1;
           if (cast_rows_f16(s, w.x, static_cast<size_t>(T) * H, w.ctx)) return -1;
@@ -991,11 +1180,13 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
     }
   } else {
     ProfScope ps_embed(m, PC_EMBED);
-    if (embed_ln_bert(s, d_ids, w.pos, T, H, c.vocab, c.max_pos, m.emb_word, m.emb_pos, m.emb_type0, m.emb_ln_w,
-                      m.emb_ln_b, c.ln_eps, w.x, w.h))
+    if (embed_ln_bert(s, d_ids, w.pos, T, H, c.vocab, c.max_pos, per_task(&TaskTensors::emb_word, m.emb_word),
+                      per_task(&TaskTensors::emb_pos, m.emb_pos), per_task(&TaskTensors::emb_type0, m.emb_type0),
+                      per_task(&TaskTensors::emb_ln_w, m.emb_ln_w), per_task(&TaskTensors::emb_ln_b, m.emb_ln_b), group_rows,
+                      c.ln_eps, w.x, w.h))
       return -1;
     for (int li = 0; li < L; ++li) {
-      const LayerWeights& lw = grouped ? m.lora.glayers[li] : m.layers[li];
+      const LayerWeights& lw = m.layers[li];
       g = GemmDesc();
       const int Hq = c.attn_w;   // == H unless the heads were padded (MiniLM)
       g.M = T; g.a_rows = w.cap_tokens; g.N = 3 * Hq; g.K = H; g.A = w.h; g.W = lw.wqkv; g.out = w.qkv; g.ldo = 3 * Hq;
@@ -1006,7 +1197,10 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = Hq; g.A = w.ctx; g.W = lw.wo; g.out = w.x; g.ldo = H;
       g.epi = EPI_RESID; g.resid = w.x; g.ldr = H; g.bias = lw.bo;
       { ProfScope ps(m, PC_GEMM_WO); if (run_proj(g)) return -1; }
-      { ProfScope ps(m, PC_NORM); if (layernorm_rows(s, w.x, T, H, lw.mid_norm_w, lw.mid_norm_b, c.ln_eps, w.x, w.h)) return -1; }
+      { ProfScope ps(m, PC_NORM);
+        if (layernorm_rows(s, w.x, T, H, per_task_norm(li, &TaskNorms::mid_w, lw.mid_norm_w),
+                           per_task_norm(li, &TaskNorms::mid_b, lw.mid_norm_b), group_rows, c.ln_eps, w.x, w.h))
+          return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = I; g.K = H; g.A = w.h; g.W = lw.wi; g.out = w.mid; g.ldo = I;
       g.epi = EPI_GELU; g.bias = lw.bi;
@@ -1015,7 +1209,10 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       g.M = T; g.a_rows = w.cap_tokens; g.N = H; g.K = I; g.A = w.mid; g.W = lw.wo2; g.out = w.x; g.ldo = H;
       g.epi = EPI_RESID; g.resid = w.x; g.ldr = H; g.bias = lw.bo2;
       { ProfScope ps(m, PC_GEMM_WO2); if (run_proj(g)) return -1; }
-      { ProfScope ps(m, PC_NORM); if (layernorm_rows(s, w.x, T, H, lw.out_norm_w, lw.out_norm_b, c.ln_eps, w.x, w.h)) return -1; }
+      { ProfScope ps(m, PC_NORM);
+        if (layernorm_rows(s, w.x, T, H, per_task_norm(li, &TaskNorms::out_w, lw.out_norm_w),
+                           per_task_norm(li, &TaskNorms::out_b, lw.out_norm_b), group_rows, c.ln_eps, w.x, w.h))
+          return -1; }
     }
   }
   return 0;
@@ -1027,12 +1224,13 @@ int head_sequence(Model& m, int head, const int* d_cu, int B, int pooler_mode) {
   const EncoderConfig& c = m.cfg;
   Workspace& w = m.ws;
   if (static_cast<size_t>(B) * hd.num_classes > w.out_elems) return -1;
+  const float* final_norm = hd.final_norm_w ? hd.final_norm_w : m.final_norm_w;
   SeqHeadWeights sw;
   sw.cls_w = hd.cls_w; sw.cls_b = hd.cls_b; sw.num_classes = hd.num_classes;
   if (c.arch == ARCH_MODERNBERT) {
     // always MEAN pooling over final_norm(hidden) (traditional/modernbert.rs:818,1146-1169)
     const bool hf = m.head_flavor == 1;
-    if (pool_rows(m.stream, w.x, d_cu, B, c.H, (hf && c.cls_pooling == 0) ? POOL_CLS : POOL_MEAN, m.final_norm_w, nullptr,
+    if (pool_rows(m.stream, w.x, d_cu, B, c.H, (hf && c.cls_pooling == 0) ? POOL_CLS : POOL_MEAN, final_norm, nullptr,
                   c.ln_eps, w.pooled, w.pool_part, w.pool_arrived))
       return -1;
     sw.dense_mode = hd.has_dense ? 1 : 0;
@@ -1058,10 +1256,11 @@ int head_tokens(Model& m, int head, int B, int T, int row0) {
   if (static_cast<size_t>(T) * hd.num_classes > w.out_elems || row0 < 0 || row0 + T > w.cap_tokens) return -1;
   const size_t off = static_cast<size_t>(row0) * c.H;   // the head reads rows [row0, row0 + T) of the hidden states
   const float* x = w.x + off;
+  const float* final_norm = hd.final_norm_w ? hd.final_norm_w : m.final_norm_w;
   if (c.arch == ARCH_MODERNBERT) {
     if (hd.has_dense) {
       // final_norm -> fp16, head.dense on the wgmma GEMM, then gelu/LN/classifier per token
-      if (layernorm_rows(m.stream, x, T, c.H, m.final_norm_w, nullptr, c.ln_eps, nullptr, w.h + off)) return -1;
+      if (layernorm_rows(m.stream, x, T, c.H, final_norm, nullptr, c.ln_eps, nullptr, w.h + off)) return -1;
       GemmDesc g;
       g.M = T; g.a_rows = w.cap_tokens - row0; g.N = c.H; g.K = c.H; g.A = w.h + off; g.W = hd.dense_w16; g.out = w.ctx + off; g.ldo = c.H;
       g.epi = EPI_F16;
@@ -1070,7 +1269,7 @@ int head_tokens(Model& m, int head, int B, int T, int row0) {
       return token_head(m.stream, nullptr, w.ctx + off, T, c.H, hd.norm_w, nullptr, 0.f, hd.cls_w, hd.cls_b, hd.num_classes,
                         hf ? 1 : 0, w.logits, w.probs, w.cls, w.conf, hf ? 1 : 0, hf ? c.ln_eps : 1e-12f);
     }
-    return token_head(m.stream, x, nullptr, T, c.H, nullptr, m.final_norm_w, c.ln_eps, hd.cls_w, hd.cls_b,
+    return token_head(m.stream, x, nullptr, T, c.H, nullptr, final_norm, c.ln_eps, hd.cls_w, hd.cls_b,
                       hd.num_classes, 0, w.logits, w.probs, w.cls, w.conf);
   }
   return token_head(m.stream, x, nullptr, T, c.H, nullptr, nullptr, 0.f, hd.cls_w, hd.cls_b, hd.num_classes, 1,

@@ -66,6 +66,7 @@ struct Head {
   float* norm_w = nullptr;
   float* cls_w = nullptr;
   float* cls_b = nullptr;
+  float* final_norm_w = nullptr;   // ModernBERT: this head's task's final_norm (grouped models); null: the model's
   std::map<int, std::string> id2label;
 };
 
@@ -134,14 +135,24 @@ struct PreciseState {
   size_t split_cap = 0, qkv_cap = 0, ctx_cap = 0, mid_cap = 0, act_cap = 0;
 };
 
-// Shared-base multi-task serving from UNMERGED LoRA checkpoints (SURVEY section 8 f3; lora_adapter.rs:136-144): T task
-// checkpoints over one base.  Every task's adapters are folded into its own copy of the projection weights at load
-// (W_t = W + (alpha_t / r_t) B_t A_t) and the T copies are stacked along N.  A batch runs ONCE as T copies of its rows
-// (task-major, each copy padded to whole 256-row blocks), and every row block of a projection GEMM picks its task's
-// matrix in the TMA producer (gemm.h: w_groups) -- the numerics of T separately loaded models in one pass.
-struct LoraShared {
-  int tasks = 0;
-  std::vector<LayerWeights> glayers;   // per layer: the base layer's norms / biases + the stacked projection weights
+// Several task checkpoints of one encoder served in ONE pass (model_load_grouped): merged or fully fine-tuned
+// checkpoints, or unmerged LoRA adapters over one base (model_load_lora_shared).  The T tasks' projection matrices are
+// stacked along N in Model::layers, each task's own LayerNorm gamma folded into its slice and BERT's biases stacked the
+// same way.  A batch runs ONCE as T copies of its rows (task-major, each copy padded to whole 256-row blocks): every row
+// block of a projection GEMM picks its task's matrix and bias (gemm.h: w_groups), every row kernel its task's embeddings
+// and norms (kernels.h: RowGroups), every task's head its task's final_norm -- the numerics of T separately loaded
+// models in one pass.  Outside such a pass the model is task 0.
+struct TaskNorms {      // one layer's norms of one task (null where the architecture has none)
+  float *attn_w = nullptr, *mid_w = nullptr, *mid_b = nullptr, *out_w = nullptr, *out_b = nullptr;
+};
+struct TaskTensors {    // one task's tensors outside the projections; a tensor equal in every task is ONE allocation
+  float *emb_word = nullptr, *emb_pos = nullptr, *emb_type0 = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
+  float* final_norm_w = nullptr;
+  std::vector<TaskNorms> layers;
+};
+struct Grouped {
+  int tasks = 0;        // 0: an ordinary model
+  std::vector<TaskTensors> task;
   std::vector<int> head_of_task;
   int rows_per_task = 0;   // set (under mu) for one forward: rows [t * rows_per_task, (t + 1) * rows_per_task) belong to task t
 };
@@ -149,7 +160,7 @@ struct LoraShared {
 struct Model {
   int device = 0;
   PreciseState precise;
-  LoraShared lora;
+  Grouped group;
   Profiler prof;
   EncoderConfig cfg;
   std::string dir;
@@ -173,14 +184,17 @@ struct Model {
   cudaStream_t stream = nullptr;
   std::mutex mu;
   std::vector<void*> allocs;  // everything to cudaFree
+  size_t weight_bytes = 0;    // bytes of those allocations (the loaded tensors)
 };
 
-// flags: kLoadKeepAdapters = leave `lora_A / lora_B` tensors unmerged (the base weights load as they are),
-// kLoadNoHead = do not load <dir>'s classifier
-enum { kLoadKeepAdapters = 1, kLoadNoHead = 2 };
-Model* model_load(const std::string& dir, int device, std::string* err, int flags = 0);
-// One base + n task checkpoints (each a full unmerged-LoRA checkpoint over the SAME base weights, with its own head);
-// token_level[t]: 1 / 0 / -1 (from config.json).  Fails when the base tensors differ between the directories.
+Model* model_load(const std::string& dir, int device, std::string* err);
+// 1..8 task checkpoints of one encoder shape (every EncoderConfig field equal, no padded heads), each with its own head,
+// as one grouped model (engine.h: Grouped).  Adapters a checkpoint carries are merged as model_load merges them.
+// token_level[t]: 1 / 0 / -1 (from config.json).  Every refusal of the directories comes before a device is touched.
+Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
+                          std::string* err);
+// model_load_grouped for unmerged LoRA checkpoints over ONE base: refuses directories whose base tensors differ or that
+// carry no adapters.
 Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
                               std::string* err);
 int checkpoint_has_adapters(const std::string& dir);
@@ -207,7 +221,7 @@ void precise_free(Model& m);
 // Sequence classification with head `head`: writes ws.logits/probs [B,C], ws.cls, ws.conf.
 int head_sequence(Model& m, int head, const int* d_cu, int B, int pooler_mode);
 // Token classification with head `head`: writes ws.logits/probs [T,C], ws.cls [T], ws.conf [T].
-// row0: first row of the hidden states this head reads (shared-LoRA passes hold one copy of the batch per task)
+// row0: first row of the hidden states this head reads (grouped passes hold one copy of the batch per task)
 int head_tokens(Model& m, int head, int B, int T, int row0 = 0);
 // Embedding: mean/CLS pool (+final norm for ModernBERT) -> narrow(dim) -> L2 normalise into ws.emb [B,dim].
 int head_embedding(Model& m, const int* d_cu, int B, int dim, float norm_eps);

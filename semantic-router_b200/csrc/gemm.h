@@ -29,7 +29,7 @@ struct GemmDesc {
   void* out = nullptr;
   int ldo = 0;
   GemmEpilogue epi = EPI_F16;
-  const float* bias = nullptr;   // fp32 [N] or null
+  const float* bias = nullptr;   // fp32 [N] or null (bias_per_group: [w_groups * N])
   const float* resid = nullptr;  // fp32 [M, ldr] (EPI_RESID)
   int ldr = 0;
   const int* pos = nullptr;      // int32 [M] (EPI_ROPE)
@@ -71,8 +71,11 @@ struct GemmDesc {
   // ---- grouped weights: W = w_groups matrices [N, K] stacked along N; rows [g * w_group_rows, (g + 1) * w_group_rows) of A are
   // multiplied with matrix g (w_group_rows a multiple of 128, the row-block height: a row block never straddles two
   // groups; gemm_f16 refuses anything else).  One launch serves
-  // several tasks' merged weights (engine.h: LoraShared).
+  // several tasks' weights (engine.h: Grouped).
   int w_groups = 0, w_group_rows = 0;
+  // with w_groups > 1: `bias` holds one [N] vector per matrix, stacked like them, and the rows of group g add bias + g * N
+  // (otherwise every group adds the one [N] bias)
+  bool bias_per_group = false;
 };
 
 int gemm_f16(cudaStream_t stream, const GemmDesc& g);

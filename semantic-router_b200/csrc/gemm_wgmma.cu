@@ -88,6 +88,7 @@ struct KArgs {
   int grouped;               // EPI_TOPK: grouped tile schedule (see the kernel)
   int interleave;            // tiles w, w + W, ... per worker instead of a contiguous range
   int grp_rows;              // > 0: W is a stack of [N, K] matrices, rows [g * grp_rows, (g + 1) * grp_rows) of A multiply matrix g
+  int bias_stride;           // grp_rows > 0: group g's bias starts at bias + g * bias_stride (0: one bias for every group)
 };
 constexpr int kTopK = 8;
 
@@ -396,6 +397,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     for (int t = t_begin; t < t_end; t += t_step) {
       const int m_blk = tile_m(t);
       const int row0 = row_base(m_blk) + quad * 32;
+      // grouped weights with a bias per matrix (stacked like the matrices): the row block adds its matrix's
+      const float* bias = (p.bias && p.grp_rows > 0) ? p.bias + static_cast<size_t>((m_blk * BM) / p.grp_rows) * p.bias_stride : p.bias;
       if constexpr (EPI == EPI_TOPK) {
         if (m_blk != tk_mblk) {
           if (tk_mblk >= 0) tk_flush(tk_mblk);
@@ -514,8 +517,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lw[k]));
                 float x0 = (fh.x + fl.x) + (__uint_as_float(r[8 * u + 2 * k]) - pv);
                 float x1 = (fh.y + fl.y) + (__uint_as_float(r[8 * u + 2 * k + 1]) - pv);
-                if (p.bias) {
-                  const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + ocol0 + hf * 32 + 8 * u) + k);
+                if (bias) {
+                  const float2 b = __ldg(reinterpret_cast<const float2*>(bias + ocol0 + hf * 32 + 8 * u) + k);
                   x0 += b.x; x1 += b.y;
                 }
                 st1 += x0 + x1;
@@ -579,8 +582,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             x.y += __uint_as_float(r[4 * i + 1]);
             x.z += __uint_as_float(r[4 * i + 2]);
             x.w += __uint_as_float(r[4 * i + 3]);
-            if (p.bias) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + ocol0) + i);
+            if (bias) {
+              const float4 b = __ldg(reinterpret_cast<const float4*>(bias + ocol0) + i);
               x.x += b.x; x.y += b.y; x.z += b.z; x.w += b.w;
             }
             *q = x;
@@ -594,8 +597,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
               float v0 = __uint_as_float(r[2 * i]), v1 = __uint_as_float(r[2 * i + 1]);
-              if (p.bias) {
-                const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + ocol0 + hf * 32) + i);
+              if (bias) {
+                const float2 b = __ldg(reinterpret_cast<const float2*>(bias + ocol0 + hf * 32) + i);
                 v0 += b.x; v1 += b.y;
               }
               if constexpr (EPI == EPI_GELU) { v0 = gelu_erf_fast_f(v0); v1 = gelu_erf_fast_f(v1); }
@@ -1153,6 +1156,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
                    g.N / BN > 1) ? 1 : 0;
   ka.fold_stats = nullptr; ka.fold_eps = 0.f; ka.fold_inv_h = 0.f; ka.fold_parts = 0;
   ka.grp_rows = w_groups > 1 ? g.w_group_rows : 0;
+  ka.bias_stride = (w_groups > 1 && g.bias_per_group) ? g.N : 0;
   CUtensorMap tx = tc;   // auxiliary map (EPI_RESID_HL: the low halves of the pair); unused otherwise
   if (is_hl && make_tmap_2d(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.lo16, g.N, g.M, g.N, 64, 32)) return -1;
   if (g.fold_stats) {

@@ -21,21 +21,38 @@ int attention_wgmma_fwd(cudaStream_t stream, const __half* qkv, __half* out, con
                         int max_len, int num_heads, int head_dim, int window, const int* kv_lens = nullptr);
 
 // ---- elementwise.cu
+// Per-row parameters of a grouped pass (engine.h: Grouped): rows [g * rows, (g + 1) * rows) read p[g]; rows == 0: every
+// row reads p[0].  A tensor every group shares is the same pointer in every slot.  Passed by value to the kernels.
+constexpr int kMaxRowGroups = 8;
+struct RowGroups {
+  const float* p[kMaxRowGroups] = {};
+  static RowGroups one(const float* q) { RowGroups r; r.p[0] = q; return r; }
+};
+
 // pos[t] = t - cu_seqlens[seq(t)]
 int compute_positions(cudaStream_t stream, const int* cu_seqlens, int batch, int* pos);
 // ModernBERT embeddings: x = LN_nobias(E[ids]); writes fp32 residual stream and its fp16 copy.
 // lo (optional): fp16(x - fp16(x)), the low half of the fp16-pair form of the residual stream; x may be null then
 int embed_ln_modernbert(cudaStream_t stream, const int* ids, int T, int H, int vocab, const float* table,
                         const float* ln_w, float eps, float* x, __half* h, __half* lo = nullptr);
+// the same with the table and LayerNorm weight of row r's group (group_rows > 0: g = r / group_rows)
+int embed_ln_modernbert(cudaStream_t stream, const int* ids, int T, int H, int vocab, const RowGroups& table,
+                        const RowGroups& ln_w, int group_rows, float eps, float* x, __half* h, __half* lo);
 // x[r, :] = pivot[r] + hi[r, :] + lo[r, :]  (pivot null: 0)
 int hl_to_f32(cudaStream_t stream, const __half* hi, const __half* lo, const float* pivot, int T, int H, float* x);
 // BERT embeddings: x = LN(word[id] + pos[p] + type[0]).
 int embed_ln_bert(cudaStream_t stream, const int* ids, const int* pos, int T, int H, int vocab, int max_pos,
                   const float* word, const float* pos_emb, const float* type0, const float* ln_w,
                   const float* ln_b, float eps, float* x, __half* h);
+int embed_ln_bert(cudaStream_t stream, const int* ids, const int* pos, int T, int H, int vocab, int max_pos,
+                  const RowGroups& word, const RowGroups& pos_emb, const RowGroups& type0, const RowGroups& ln_w,
+                  const RowGroups& ln_b, int group_rows, float eps, float* x, __half* h);
 // Row LayerNorm of fp32 x[T,H]; optional outputs: y32 (may alias x) and y16.
 int layernorm_rows(cudaStream_t stream, const float* x, int T, int H, const float* w, const float* b, float eps,
                    float* y32, __half* y16);
+// the same with the weight and bias (null slots: no bias) of row r's group
+int layernorm_rows(cudaStream_t stream, const float* x, int T, int H, const RowGroups& w, const RowGroups& b,
+                   int group_rows, float eps, float* y32, __half* y16);
 // fp32 -> fp16 copy of n elements, any n (x 16-byte and y 8-byte aligned)
 int cast_rows_f16(cudaStream_t stream, const float* x, size_t n, __half* y);
 

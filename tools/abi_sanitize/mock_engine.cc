@@ -196,6 +196,13 @@ int sr_model_load_lora_shared(const char* const* dirs, const int* token_level, i
   *out = m;
   return 0;
 }
+// grouped model of merged checkpoints: SR_MOCK_GROUPED=1 makes the loader accept the directories (the same mock model as
+// the shared-LoRA one); otherwise it refuses them as the engine refuses checkpoints of different encoder shapes
+int sr_model_load_grouped(const char* const* dirs, const int* token_level, int n, int device, sr_model** out) {
+  const char* e = getenv("SR_MOCK_GROUPED");
+  if (!(e && e[0] == '1')) return -1;
+  return sr_model_load_lora_shared(dirs, token_level, n, device, out);
+}
 int sr_lora_shared_tasks(const sr_model* m) {
   std::lock_guard<std::mutex> lk(g_shared_mu);
   for (const auto& kv : g_shared)
