@@ -61,7 +61,6 @@ typedef struct sr_gemm_desc {
   const uint8_t* topk_valid;
   int topk_n;
   float* row_stats;
-  void* reserved;   /* must be null: keeps the offsets of the fields below fixed for existing callers */
   void* lo16;
   float* pivot_out;
   const float* pivot_in;

@@ -106,7 +106,7 @@ class GemmDesc(C.Structure):
         ("epi", C.c_int), ("bias", C.c_void_p), ("resid", C.c_void_p), ("ldr", C.c_int), ("pos", C.c_void_p),
         ("rope_cos", C.c_void_p), ("rope_sin", C.c_void_p), ("rope_cols", C.c_int), ("topk_idx", C.c_void_p),
         ("topk_score", C.c_void_p), ("topk_valid", C.c_void_p), ("topk_n", C.c_int), ("row_stats", C.c_void_p),
-        ("reserved", C.c_void_p), ("lo16", C.c_void_p), ("pivot_out", C.c_void_p), ("pivot_in", C.c_void_p),
+        ("lo16", C.c_void_p), ("pivot_out", C.c_void_p), ("pivot_in", C.c_void_p),
         ("pivot_in_stats", C.c_void_p), ("fold_stats", C.c_void_p), ("fold_eps", C.c_float), ("fold_h", C.c_int),
         ("w_groups", C.c_int), ("w_group_rows", C.c_int)]
 

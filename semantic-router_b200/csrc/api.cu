@@ -578,7 +578,7 @@ int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* workers) {
   return *workers > 0 ? 0 : -1;
 }
 int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
-  if (!d || d->reserved) return -1;
+  if (!d) return -1;
   GemmDesc g;
   g.M = d->m; g.N = d->n; g.K = d->k; g.A = d->a; g.a_rows = d->a_rows; g.W = d->w; g.out = d->out; g.ldo = d->ldo;
   g.epi = static_cast<GemmEpilogue>(d->epi);

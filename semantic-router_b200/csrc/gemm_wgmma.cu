@@ -4,9 +4,13 @@
 //
 // Replaces the dense f32 `gemm`+rayon matmuls behind candle's Linear on the reference's hot loop
 // (candle-binding/src/model_architectures/traditional/candle_models/modernbert.rs
-//  :123 Wqkv, :196 Wo, :236-238 Wi/GeGLU/Wo) with two persistent kernels:
-//   * gemm_kernel, 128 x 128 tiles: EPI_F16 (bias), EPI_RESID (fp32 residual add, :300-303), EPI_GELU (erf-GELU, BERT
-//     intermediate), EPI_TOPK (the cache scan) and EPI_RESID_HL (the fp16-pair residual stream)
+//  :123 Wqkv, :196 Wo, :236-238 Wi/GeGLU/Wo) with two persistent kernels.  In this file, in order:
+//   * what both kernels share: the wgmma wrappers, the operand-ring position (Ring), the tile schedule (tile_range),
+//     the TMA producer (produce_operands), the prologue (kernel_prologue) and the closing barrier (cta_sync).
+//   * gemm_kernel's epilogues, one Epilogue<EPI> per output form with only its own state: EPI_F16 / EPI_GELU (bias,
+//     erf-GELU for BERT's intermediate), EPI_RESID (fp32 residual add, :300-303), EPI_RESID_HL (the fp16-pair residual
+//     stream) and EPI_TOPK (the cache scan's running top-8).
+//   * gemm_kernel, 128 x 128 tiles, for those epilogues
 //     - warp 8      : TMA producer  (cp.async.bulk.tensor 2D, 128B swizzle, mbarrier complete_tx)
 //     - warps 4..7  : one MMA warpgroup -- wgmma.mma_async m64n128k16 twice per k-step (rows 0-63, 64-127), fp32
 //                     accumulators in registers; at the end of a tile they go to a swizzled fp32 tile in shared memory
@@ -14,17 +18,15 @@
 //     - the accumulator tile in shared memory is the hand-off: the epilogue of tile i overlaps the mainloop of tile i+1,
 //       whose accumulators live in the MMA warpgroup's registers until the epilogue has released the shared tile.
 //   * gemm_wide_kernel, 128 x 192 tiles: the LayerNorm-fold projections, EPI_ROPE (rotate-half, modernbert.rs:61-85)
-//     and EPI_GEGLU (gelu_erf(a)*b, :238), with two MMA warpgroups and the epilogue from their registers (see there).
-//     It is the only kernel that runs in thread-block clusters (gemm_cluster_size): the cn CTAs of a cluster compute
-//     neighbouring column tiles of one row block; each loads a 1/cn slice of the shared A box and multicasts it (TMA
-//     .multicast::cluster), and frees a stage by arriving on the empty barrier of every CTA that wrote into it.  Tiles,
-//     the wgmma sequence, the accumulation order and the epilogues are the same as without clusters: results are
-//     bitwise identical.
+//     and EPI_GEGLU (gelu_erf(a)*b, :238), with two MMA warpgroups and the epilogue from their registers.  It is the
+//     only kernel that runs in thread-block clusters (see there); results are bitwise those without clusters.
+//   * the host side: tensor maps, the one list of kernel instances (with_kernel) and the launch.
 #include "gemm.h"
 
 #include <atomic>
 #include <cstdlib>
 #include <mutex>
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -44,21 +46,21 @@ constexpr int kStageBufBytes = 4096;   // one epilogue staging box: 32 rows x 12
 constexpr int kBarrierBytes = 512;
 constexpr int kSmemLimit = 232448;     // 227 KB opt-in limit per CTA (sm_90)
 constexpr int kAccBytes = BM * BN * 4; // fp32 accumulator tile handed from the MMA warpgroup to the epilogue
-// staging boxes per epilogue warp.  The fp32-residual epilogue keeps one residual load in flight next to the box being
-// computed; the fp16-pair residual epilogue has one (hi, lo) box pair, loaded at the start of the chunk that uses it.
-// Shared memory is what limits this on sm_90: the 64 KB accumulator tile plus these boxes leave 4 mainloop stages.  A
-// second pair (to load a chunk ahead) costs the fourth stage, and the residual GEMMs are bound by their operand feed,
-// not by the epilogue's load latency: at T = 131072 on an H100 80GB HBM3 (700 W), two pairs and 3 stages ran Wo in
-// 0.518 ms and Wo2 in 0.651-0.662 ms, one pair and 4 stages 0.443-0.444 and 0.528-0.536 ms (tools/gemm_prof.py).
+// staging boxes per epilogue warp: the fp32-residual epilogue's two-box ring, or the fp16-pair residual epilogue's one
+// (hi, lo) box pair, loaded at the start of the chunk that uses it.  Shared memory is what limits this on sm_90: the
+// 64 KB accumulator tile plus these boxes leave 4 mainloop stages.  A second pair (to load a chunk ahead) costs the
+// fourth stage, and the residual GEMMs are bound by their operand feed, not by the epilogue's load latency: at
+// T = 131072 on an H100 80GB HBM3 (700 W), two pairs and 3 stages ran Wo in 0.518 ms and Wo2 in 0.651-0.662 ms, one
+// pair and 4 stages 0.443-0.444 and 0.528-0.536 ms (tools/gemm_prof.py).
 constexpr int kStageBufs = 2;
 
-template <int EPI>
+// gemm_kernel's shared memory: the operand ring, the accumulator tile, the staging boxes and the barriers
 struct GemmCfg {
-  static constexpr int kBufs = kStageBufs;
+  static constexpr int kBN = BN;   // W box height
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kEpiBytes = kEpiWarps * kBufs * kStageBufBytes;
+  static constexpr int kEpiBytes = kEpiWarps * kStageBufs * kStageBufBytes;
   static constexpr int kFit = (kSmemLimit - kAccBytes - kEpiBytes - 1024 /*align slack*/ - kBarrierBytes) / kStageBytes;
   static constexpr int kStages = kFit < 6 ? kFit : 6;   // as deep as shared memory allows, 6 at most
   static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + kEpiBytes + 1024 + kBarrierBytes;
@@ -168,14 +170,425 @@ __device__ __forceinline__ uint32_t acc_off(int row, int col) {
   return static_cast<uint32_t>(row * (BN * 4) + (((u & ~7) | ((u & 7) ^ (row & 7))) << 4) + (col & 3) * 4);
 }
 
+// ---- shared by both kernels ---------------------------------------------------------------------------------------
+// Position in a ring of kStages buffers: the stage and the parity of its current round (the mbarrier phase bit)
+template <int kStages>
+struct Ring {
+  int s = 0;
+  uint32_t ph = 0;
+  __device__ __forceinline__ void advance() {
+    if (++s == kStages) { s = 0; ph ^= 1; }
+  }
+};
+
+// The tiles of one worker: t = begin, begin + step, ... < end, numbered t = m_blk * n_tiles + n_tile (n fastest).  The
+// workers of gemm_wide_kernel are clusters and its tiles cluster tiles.
+struct TileRange { int begin, end, step; };
+__device__ __forceinline__ TileRange tile_range(int m_blocks, int n_tiles, int worker, int workers, bool interleave,
+                                                bool grouped) {
+  const int num_tiles = m_blocks * n_tiles;
+  if (grouped) {
+    // EPI_TOPK, grouped schedule (p.grouped): worker w owns query block w % m_blocks for its whole life (its running
+    // top-8 lists live in registers) and walks the stored-row tiles g, g + G, g + 2G, ... with g = w / m_blocks,
+    // G = workers / m_blocks.  The m_blocks workers of a group therefore ask for the SAME stored-row tile at about the
+    // same time: one HBM read, the rest L2 hits -- the store streams once per batch instead of once per query block.
+    const int groups = workers / m_blocks;
+    const int m_own = worker % m_blocks, g_own = worker / m_blocks;
+    const int begin = m_own * n_tiles + g_own;
+    return {begin, g_own < groups ? (m_own + 1) * n_tiles : begin, groups};   // workers beyond the last full group idle
+  }
+  // Interleaved schedule (p.interleave; the residual GEMMs): worker w takes tiles w, w + W, w + 2W, ...  With
+  // n fastest in the tile numbering the N / BN tiles of one row block run AT THE SAME TIME on neighbouring workers, so
+  // each A k-block is pulled from HBM once and hit in L2 by the others, where the contiguous ranges could lose the row
+  // block from L2 to the residual stream passing through between two tiles of one worker.
+  if (interleave) return {worker, num_tiles, workers};
+  // contiguous tile range per worker: one worker walks all N tiles of its M blocks back to back, so the A row-block
+  // stays hot in L2 and per-row epilogue state (pivots, top-8 lists, rstd, positions) is reused across tiles
+  const int base = num_tiles / workers, rem = num_tiles % workers;
+  const int begin = worker * base + (worker < rem ? worker : rem);
+  return {begin, begin + base + (worker < rem ? 1 : 0), 1};
+}
+
+// TMA producer (one lane): every k-block of every tile of the worker into the operand ring, W in boxes of Cfg::kBN rows.
+// CTA rn of a cluster of CN (1: none) loads its slice of the shared A box (tensor-map box height BM / CN rows, a multiple
+// of the 8-row swizzle atom, so the slices assemble into exactly the tile layout one full-box load would give) and
+// multicasts it to the whole cluster.
+template <class Cfg, int CN>
+__device__ __forceinline__ void produce_operands(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, uint8_t* smem_a,
+                                                 uint8_t* smem_b, uint64_t* full_bar, uint64_t* empty_bar,
+                                                 const TileRange& tr, int n_tiles, int rn, int k_blocks, const KArgs& p) {
+  Ring<Cfg::kStages> ring;
+  constexpr int a_rows = BM / CN;
+  const uint16_t a_mask = static_cast<uint16_t>((1u << CN) - 1);
+  for (int t = tr.begin; t < tr.end; t += tr.step) {
+    const int m_blk = t / n_tiles, n_blk = (t % n_tiles) * CN + rn;
+    // grouped weights (one matrix per task, stacked along N): the row block picks its matrix; blocks never straddle
+    // two groups (grp_rows is a multiple of the block height, checked on the host)
+    const int w_row0 = p.grp_rows > 0 ? ((m_blk * BM) / p.grp_rows) * p.N : 0;
+    for (int kb = 0; kb < k_blocks; ++kb) {
+      mbar_wait(&empty_bar[ring.s], ring.ph ^ 1);
+      const int kc = kb * BK;
+      // the stage fills with the A slices of every CTA of the cluster and this CTA's own W box: the whole stage
+      mbar_expect_tx(&full_bar[ring.s], Cfg::kStageBytes);
+      uint8_t* da = smem_a + ring.s * Cfg::kABytes + rn * a_rows * (BK * 2);
+      const int ya = m_blk * BM + rn * a_rows;
+      if constexpr (CN > 1) tma_load_2d_multicast(da, tmap_a, &full_bar[ring.s], kc, ya, a_mask);
+      else tma_load_2d(da, tmap_a, &full_bar[ring.s], kc, ya);
+      tma_load_2d(smem_b + ring.s * Cfg::kBBytes, tmap_b, &full_bar[ring.s], kc, w_row0 + n_blk * Cfg::kBN);
+      ring.advance();
+    }
+  }
+}
+
+// Barrier of the CTA, or of its cluster for CN > 1: no CTA may multicast into another or arrive on its barriers before
+// those exist (kernel start), nor leave while another of its cluster may still arrive on its own (kernel end).
+template <int CN>
+__device__ __forceinline__ void cta_sync() {
+  if constexpr (CN > 1) cluster_sync();
+  else __syncthreads();
+}
+
+// Kernel start: thread 0 prefetches the tensor maps and sets up the operand ring's barriers (full: the producer's
+// arrival and the stage's bytes; empty: `empty_arrivals`) and, in `init_more`, the kernel's own; then cta_sync.
+template <int CN, int kStages, class InitMore>
+__device__ __forceinline__ void kernel_prologue(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b,
+                                                const CUtensorMap* tmap_out, uint64_t* full_bar, uint64_t* empty_bar,
+                                                uint32_t empty_arrivals, InitMore init_more) {
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(tmap_a);
+    tma_prefetch_desc(tmap_b);
+    tma_prefetch_desc(tmap_out);
+#pragma unroll
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], empty_arrivals);
+    }
+    init_more();
+    mbar_fence_init();
+  }
+  cta_sync<CN>();
+  // PDL: everything above overlapped the previous kernel's tail; nothing below may start before its writes are visible
+  griddep_launch_dependents();
+  griddep_wait();
+}
+
+// ---- gemm_kernel's epilogues ---------------------------------------------------------------------------------------
+// An epilogue warp of gemm_kernel: warp `quad` owns rows 32 quad .. 32 quad + 31 of the tile, one per lane, and
+// kStageBufs boxes of 32 rows x 128 bytes (one chunk of output columns) with a residual-load barrier each.  Per tile
+// it runs row_block before the accumulator tile is ready (per-row loads overlap the mainloop), then tile.
+struct EpiWarp {
+  const KArgs& p;
+  const CUtensorMap *tmap_out, *tmap_aux;   // tmap_aux: the lo boxes of EPI_RESID_HL
+  int lane, quad;
+  const uint8_t* acc_row;   // this thread's row of the accumulator tile
+  uint8_t* bufs;
+  uint64_t* rbar;
+  TileRange tr;             // this CTA's tiles, n_blocks to a row block
+  int n_blocks;
+  // this thread's row, accumulator columns [col, col + 32) (col a multiple of 32)
+  __device__ __forceinline__ void acc_ld32(int col, uint32_t* r) const {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const uint4 v = *reinterpret_cast<const uint4*>(acc_row + ((((col >> 2) + (i ^ (lane & 7)))) << 4));
+      r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
+    }
+  }
+  // TMA-store the box(es) this warp has written, as one store group (aux_buf: the lo box of EPI_RESID_HL's pair)
+  __device__ __forceinline__ void store(const uint8_t* buf, int col, int row0, const uint8_t* aux_buf = nullptr) const {
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      tma_store_2d(tmap_out, buf, col, row0);  // rows >= M / cols >= N are clipped by the TMA unit
+      if (aux_buf) tma_store_2d(tmap_aux, aux_buf, col, row0);
+      bulk_commit();
+    }
+  }
+  __device__ __forceinline__ void row_block(int) {}
+  __device__ __forceinline__ void finish() {}
+};
+
+// EPI_F16 / EPI_GELU: fp16 out = acc + bias, erf-GELU'd for EPI_GELU, in 64-column chunks through the two boxes in
+// turn.  A box is rewritten once its previous store has been read out: all but the newest store group, bulk_wait_read<1>.
+template <int EPI>
+struct Epilogue : EpiWarp {
+  static_assert(EPI == EPI_F16 || EPI == EPI_GELU, "no gemm_kernel epilogue of this kind");
+  int cb = 0;   // box of the next chunk
+  __device__ __forceinline__ void tile(int, int m_blk, int n_blk, const float* bias) {
+    const int row0 = m_blk * BM + quad * 32;
+#pragma unroll 1
+    for (int c = 0; c < BN / 64; ++c) {
+      const int ocol0 = n_blk * BN + c * 64;
+      if (ocol0 >= p.N) break;   // the last column tile of an N % 128 == 64 output is half empty
+      uint8_t* my_row = bufs + cb * kStageBufBytes;  // + box_off(lane, chunk16)
+      if (lane == 0) bulk_wait_read<1>();
+      __syncwarp();
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        uint32_t r[32];
+        acc_ld32(c * 64 + hf * 32, r);
+        uint32_t h[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          float v0 = __uint_as_float(r[2 * i]), v1 = __uint_as_float(r[2 * i + 1]);
+          if (bias) {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(bias + ocol0 + hf * 32) + i);
+            v0 += b.x; v1 += b.y;
+          }
+          if constexpr (EPI == EPI_GELU) { v0 = gelu_erf_fast_f(v0); v1 = gelu_erf_fast_f(v1); }
+          h[i] = pack_half2(v0, v1);
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          sts16(my_row + box_off(lane, hf * 4 + i), h[4 * i], h[4 * i + 1], h[4 * i + 2], h[4 * i + 3]);
+      }
+      store(my_row, ocol0, row0);
+      cb ^= 1;
+    }
+  }
+};
+
+// EPI_RESID: fp32 out = acc + bias, plus out itself in place (has_resid), in 32-column chunks.  With a residual the two
+// boxes are a ring over this CTA's (tile, chunk) sequence: while a chunk is computed in one, the next chunk's residual
+// loads into the other.  The previous chunk stored from that box, the newest store group, so the load waits for every
+// store to be read out: bulk_wait_read<0>.  Without a residual the boxes alternate as in EPI_F16.
+template <>
+struct Epilogue<EPI_RESID> : EpiWarp {
+  static constexpr int kChunks = BN / 32;
+  const bool use_resid;
+  int cb = 0;         // box of the next chunk
+  uint32_t rph = 0;   // phase bit per box (residual loads)
+  __device__ __forceinline__ Epilogue(const EpiWarp& w) : EpiWarp(w), use_resid(w.p.has_resid) {
+    if (use_resid && lane == 0 && tr.begin < tr.end) load(0, tr.begin, 0);   // the first chunk
+  }
+  // lane 0: the residual of chunk c of tile t into box b
+  __device__ __forceinline__ void load(int b, int t, int c) {
+    mbar_expect_tx(&rbar[b], kStageBufBytes);
+    tma_load_2d(bufs + b * kStageBufBytes, tmap_out, &rbar[b], (t % n_blocks) * BN + c * 32, (t / n_blocks) * BM + quad * 32);
+  }
+  __device__ __forceinline__ void tile(int t, int m_blk, int n_blk, const float* bias) {
+    const int row0 = m_blk * BM + quad * 32;
+#pragma unroll 1
+    for (int c = 0; c < kChunks; ++c) {
+      const int ocol0 = n_blk * BN + c * 32;
+      if (ocol0 >= p.N) break;   // the last column tile of an N % 128 == 64 output is half empty
+      uint8_t* my_row = bufs + cb * kStageBufBytes;  // + box_off(lane, chunk16)
+      if (use_resid) {
+        if (lane == 0) {
+          bulk_wait_read<0>();
+          if (c + 1 < kChunks && ocol0 + 32 < p.N) load(cb ^ 1, t, c + 1);
+          else if (t + tr.step < tr.end) load(cb ^ 1, t + tr.step, 0);
+        }
+        mbar_wait(&rbar[cb], (rph >> cb) & 1u);
+        rph ^= 1u << cb;
+      } else {
+        if (lane == 0) bulk_wait_read<1>();  // this box's previous store has been read out
+        __syncwarp();
+      }
+      uint32_t r[32];
+      acc_ld32(c * 32, r);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        float4* q = reinterpret_cast<float4*>(my_row + box_off(lane, i));
+        float4 x = use_resid ? *q : make_float4(0.f, 0.f, 0.f, 0.f);
+        x.x += __uint_as_float(r[4 * i]);
+        x.y += __uint_as_float(r[4 * i + 1]);
+        x.z += __uint_as_float(r[4 * i + 2]);
+        x.w += __uint_as_float(r[4 * i + 3]);
+        if (bias) {
+          const float4 b = __ldg(reinterpret_cast<const float4*>(bias + ocol0) + i);
+          x.x += b.x; x.y += b.y; x.z += b.z; x.w += b.w;
+        }
+        *q = x;
+      }
+      store(my_row, ocol0, row0);
+      cb ^= 1;
+    }
+  }
+};
+
+// EPI_RESID_HL: the fp16-pair residual stream, hi (tmap_out) + lo (tmap_aux) = x - pivot.  Per 64-column chunk the
+// warp's one (hi, lo) box pair is loaded once its previous store has been read out (bulk_wait_read<0>), updated in
+// place and stored.  Row statistics go out per 128-column slice (N % 128 == 0: no chunk is past N), in chunk order.
+template <>
+struct Epilogue<EPI_RESID_HL> : EpiWarp {
+  float pv = 0.f;       // the pivot SHIFT of this GEMM for this thread's row
+  float pv_prev = 0.f;  // the pivot the stored pair is relative to
+  int pv_mblk = -1;
+  uint32_t rph = 0;     // phase bit of the pair's barrier
+  __device__ __forceinline__ void row_block(int m_blk) {
+    // pivot shift of this row: the stored pair is x - pivot_in; the new pivot is pivot_in + (mean of x - pivot_in),
+    // read from the previous residual GEMM's statistics (0 for the first one: the embedding's pair is x itself)
+    if (m_blk == pv_mblk) return;
+    pv = 0.f;
+    pv_prev = 0.f;
+    if (p.pivot_in_stats) {
+      const int row0 = m_blk * BM + quad * 32;
+      const int row = row0 + lane < p.M ? row0 + lane : p.M - 1;
+      float s1 = 0.f;
+      const int parts = p.N >> 7;
+      for (int k = 0; k < parts; ++k)
+        s1 += __ldg(reinterpret_cast<const float2*>(p.pivot_in_stats) + static_cast<size_t>(k) * p.M + row).x;
+      pv = s1 / static_cast<float>(p.N);
+      pv_prev = __ldg(p.pivot_in + row);
+    }
+    pv_mblk = m_blk;
+  }
+
+  __device__ __forceinline__ void tile(int, int m_blk, int n_blk, const float* bias) {
+    const int row0 = m_blk * BM + quad * 32;
+    uint8_t* hb = bufs;
+    uint8_t* lb = hb + kStageBufBytes;
+    float st1 = 0.f, st2 = 0.f;   // this row's (sum, sum of squares) over the current 128-column slice
+#pragma unroll 1
+    for (int c = 0; c < BN / 64; ++c) {
+      const int ocol0 = n_blk * BN + c * 64;
+      if (lane == 0) {
+        bulk_wait_read<0>();
+        mbar_expect_tx(&rbar[0], 2 * kStageBufBytes);
+        tma_load_2d(hb, tmap_out, &rbar[0], ocol0, row0);
+        tma_load_2d(lb, tmap_aux, &rbar[0], ocol0, row0);
+      }
+      mbar_wait(&rbar[0], rph);
+      rph ^= 1u;
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        uint32_t r[32];
+        acc_ld32(c * 64 + hf * 32, r);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {   // 16-byte units: 8 columns each
+          const uint32_t off = box_off(lane, hf * 4 + u);
+          uint4 hv = *reinterpret_cast<const uint4*>(hb + off);
+          uint4 lv = *reinterpret_cast<const uint4*>(lb + off);
+          uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hw[k]));
+            const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lw[k]));
+            float x0 = (fh.x + fl.x) + (__uint_as_float(r[8 * u + 2 * k]) - pv);
+            float x1 = (fh.y + fl.y) + (__uint_as_float(r[8 * u + 2 * k + 1]) - pv);
+            if (bias) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(bias + ocol0 + hf * 32 + 8 * u) + k);
+              x0 += b.x; x1 += b.y;
+            }
+            st1 += x0 + x1;
+            st2 += x0 * x0 + x1 * x1;
+            const __half2 nh = __floats2half2_rn(x0, x1);
+            const float2 fb = __half22float2(nh);
+            hw[k] = *reinterpret_cast<const uint32_t*>(&nh);
+            lw[k] = pack_half2(x0 - fb.x, x1 - fb.y);
+          }
+          sts16(hb + off, hw[0], hw[1], hw[2], hw[3]);
+          sts16(lb + off, lw[0], lw[1], lw[2], lw[3]);
+        }
+      }
+      if (c & 1) {   // a 128-column slice is complete: its partial goes out, once
+        if (row0 + lane < p.M) {
+          const size_t part = static_cast<size_t>((ocol0 - 64) >> 7);
+          *reinterpret_cast<float2*>(p.row_stats + 2 * (part * p.M + row0 + lane)) = make_float2(st1, st2);
+          if (part == 0) p.pivot_out[row0 + lane] = pv_prev + pv;
+        }
+        st1 = 0.f;
+        st2 = 0.f;
+      }
+      store(hb, ocol0, row0, lb);
+    }
+  }
+};
+
+// EPI_TOPK: this thread's running top-8 (descending) over the columns this CTA walks for its current row, written out
+// as this CTA's list for the row when the row block changes and after the last tile.
+template <>
+struct Epilogue<EPI_TOPK> : EpiWarp {
+  float tk_v[kTopK];   // set at the first row block
+  int tk_i[kTopK];
+  int tk_mblk = -1;
+  __device__ __forceinline__ Epilogue(const EpiWarp& w) : EpiWarp(w) {}
+  __device__ __forceinline__ void flush() {   // this CTA's list for the row it has just left
+    const int row = tk_mblk * BM + quad * 32 + lane;
+    if (row < p.M) {
+      const size_t at = (static_cast<size_t>(row) * gridDim.x + blockIdx.x) * kTopK;
+#pragma unroll
+      for (int i = 0; i < kTopK; ++i) { p.topk_idx[at + i] = tk_i[i]; p.topk_score[at + i] = tk_v[i]; }
+    }
+  }
+  __device__ __forceinline__ void row_block(int m_blk) {
+    if (m_blk == tk_mblk) return;
+    if (tk_mblk >= 0) flush();
+#pragma unroll
+    for (int i = 0; i < kTopK; ++i) { tk_v[i] = -INFINITY; tk_i[i] = -1; }
+    tk_mblk = m_blk;
+  }
+  __device__ __forceinline__ void finish() {
+    if (tk_mblk >= 0) flush();
+  }
+  // This warp scans the tile's columns 32 at a time.  The common path per chunk is the maximum of 32 scores and
+  // one compare against the list's tail; validity (invalidated rows, padding rows >= topk_n) is only looked up
+  // for a score that would enter the list -- after the first tiles that is rare.
+  __device__ __forceinline__ void topk_chunk(uint32_t* r, int ocol0) {
+    float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 32; i += 8) {
+      m0 = fmax3(m0, __uint_as_float(r[i]), __uint_as_float(r[i + 1]));
+      m1 = fmax3(m1, __uint_as_float(r[i + 2]), __uint_as_float(r[i + 3]));
+      m2 = fmax3(m2, __uint_as_float(r[i + 4]), __uint_as_float(r[i + 5]));
+      m3 = fmax3(m3, __uint_as_float(r[i + 6]), __uint_as_float(r[i + 7]));
+    }
+    // Take the chunk's maximum while it beats the list's tail (usually zero or one round): a round is ~150
+    // instructions, against ~1300 for trying all 32 scores in turn.
+    float cm = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
+    while (cm > tk_v[kTopK - 1]) {   // strict: an equal score at a higher column never displaces
+      int ci = 31;
+#pragma unroll
+      for (int i = 30; i >= 0; --i)
+        if (__uint_as_float(r[i]) == cm) ci = i;          // lowest column holding the maximum
+      ci = __uint_as_float(r[31]) == cm && ci == 31 ? 31 : ci;
+      float cv = cm;
+      int cidx = ocol0 + ci;
+      const bool ok = cidx < p.topk_n && (!p.topk_valid || __ldg(p.topk_valid + (cidx < p.topk_n ? cidx : 0)));
+      if (ok) {
+        // insertion into the descending list: strict > finds the slot (after any equal score, which has the lower
+        // column), and from there every entry shifts down one, ties included, so the tail is the one dropped
+        bool shift = false;
+#pragma unroll
+        for (int j = 0; j < kTopK; ++j) {
+          if (shift || cv > tk_v[j]) {
+            shift = true;
+            const float tv = tk_v[j]; const int ti = tk_i[j];
+            tk_v[j] = cv; tk_i[j] = cidx;
+            cv = tv; cidx = ti;
+          }
+        }
+      }
+      float n0 = -INFINITY, n1 = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {   // drop it and find the next maximum
+        if (i == ci) r[i] = 0xff800000u;
+        if (i + 1 == ci) r[i + 1] = 0xff800000u;
+        n0 = fmaxf(n0, __uint_as_float(r[i]));
+        n1 = fmaxf(n1, __uint_as_float(r[i + 1]));
+      }
+      cm = fmaxf(n0, n1);
+    }
+  }
+
+  __device__ __forceinline__ void tile(int, int, int n_blk, const float*) {
+#pragma unroll 1
+    for (int c = 0; c < BN / 32; ++c) {
+      uint32_t r[32];
+      acc_ld32(c * 32, r);
+      topk_chunk(r, n_blk * BN + c * 32);
+    }
+  }
+};
+
+// ================= gemm_kernel: 128 x 128 tiles, epilogue warps fed through the shared accumulator tile =================
 template <int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_aux, const KArgs p) {
   static_assert(EPI != EPI_ROPE && EPI != EPI_GEGLU, "the LayerNorm-fold projections run on gemm_wide_kernel");
-  using Cfg = GemmCfg<EPI>;
+  using Cfg = GemmCfg;
   static_assert(Cfg::kSmemBytes <= kSmemLimit, "over the 227 KB shared-memory opt-in limit");
-  constexpr bool kHL = EPI == EPI_RESID_HL;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -196,97 +609,30 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int m_blocks = (p.M + BM - 1) / BM;
   const int n_blocks = (p.N + BN - 1) / BN;
   const int k_blocks = (p.K + BK - 1) / BK;
-  const int num_tiles = m_blocks * n_blocks;
-  auto tile_m = [&](int t) { return t / n_blocks; };
-  auto tile_n = [&](int t) { return t % n_blocks; };
-  auto row_base = [&](int m_blk) { return m_blk * BM; };
-  // contiguous tile range per worker (n fastest): one worker walks all N tiles of its M blocks back to back, so the
-  // A row-block stays hot in L2 and per-row epilogue state (pivots, top-8 lists) is reused across tiles
-  const int num_workers = gridDim.x;
-  const int base = num_tiles / num_workers, rem = num_tiles % num_workers;
-  const int bid = blockIdx.x;
-  int t_begin = bid * base + (bid < rem ? bid : rem);
-  int t_end = t_begin + base + (bid < rem ? 1 : 0);
-  // EPI_TOPK, grouped schedule (p.grouped): worker w owns query block w % m_blocks for its whole life (its running
-  // top-8 lists live in registers) and walks the stored-row tiles g, g + G, g + 2G, ... with g = w / m_blocks,
-  // G = workers / m_blocks.  The m_blocks workers of a group therefore ask for the SAME stored-row tile at about the
-  // same time: one HBM read, the rest L2 hits -- the store streams once per batch instead of once per query block.
-  // Tiles are numbered t = m_blk * n_blocks + n_blk as everywhere else; `t_step` is the distance between two tiles of
-  // this worker (1 for the contiguous ranges).
-  int t_step = 1;
-  // Interleaved schedule (p.interleave; the residual GEMMs): worker w takes tiles w, w + W, w + 2W, ...  With
-  // n fastest in the tile numbering the N / BN tiles of one row block run AT THE SAME TIME on neighbouring workers, so
-  // each A k-block is pulled from HBM once and hit in L2 by the others, where the contiguous ranges could lose the row
-  // block from L2 to the residual stream passing through between two tiles of one worker.
-  if (p.interleave) {
-    t_begin = bid;
-    t_end = num_tiles;
-    t_step = num_workers;
-  }
-  if constexpr (EPI == EPI_TOPK) {
-    if (p.grouped) {
-      const int groups = num_workers / m_blocks;
-      const int m_own = bid % m_blocks, g_own = bid / m_blocks;
-      t_begin = m_own * n_blocks + g_own;
-      t_end = (m_own + 1) * n_blocks;
-      t_step = groups;
-      if (g_own >= groups) t_end = t_begin;   // workers beyond the last full group stay idle
-    }
-  }
+  const TileRange tr = tile_range(m_blocks, n_blocks, blockIdx.x, gridDim.x, p.interleave, EPI == EPI_TOPK && p.grouped);
 
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_out);
-#pragma unroll
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 4);   // one arrival per MMA warp
-    }
+  kernel_prologue<1, Cfg::kStages>(&tmap_a, &tmap_b, &tmap_out, full_bar, empty_bar, 4 /*one arrival per MMA warp*/, [&] {
     mbar_init(tfull_bar, 128);            // every thread of the MMA warpgroup, after its fragment stores
     mbar_init(tempty_bar, kEpiWarps);
     for (int i = 0; i < kEpiWarps * kStageBufs; ++i) mbar_init(&resid_bar[i], 1);
-    mbar_fence_init();
-  }
-  __syncthreads();
-  // PDL: everything above overlapped the previous kernel's tail; nothing below may start before its writes are visible
-  griddep_launch_dependents();
-  griddep_wait();
+  });
 
   if (warp == kProducerWarp) {
     // ================= TMA producer =================
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int t = t_begin; t < t_end; t += t_step) {
-        const int m_blk = tile_m(t), n_blk = tile_n(t);
-        // grouped weights (one matrix per task, stacked along N): the row block picks its matrix; blocks never straddle
-        // two groups (grp_rows is a multiple of the block height, checked on the host)
-        const int w_row0 = p.grp_rows > 0 ? ((m_blk * BM) / p.grp_rows) * p.N : 0;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          const int kc = kb * BK;
-          mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
-          tma_load_2d(smem_a + s * Cfg::kABytes, &tmap_a, &full_bar[s], kc, m_blk * BM);
-          tma_load_2d(smem_b + s * Cfg::kBBytes, &tmap_b, &full_bar[s], kc, w_row0 + n_blk * BN);
-          if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
+    if (lane == 0) produce_operands<Cfg, 1>(&tmap_a, &tmap_b, smem_a, smem_b, full_bar, empty_bar, tr, n_blocks, 0, k_blocks, p);
   } else if (warp >= kMmaWarp0) {
     // ================= MMA warpgroup =================
     const int wq = warp - kMmaWarp0;   // warp of the warpgroup: fragment rows 16 wq .. 16 wq + 15 of each 64-row half
     float acc[2][64];
-    int s = 0;
-    uint32_t ph = 0;
+    Ring<Cfg::kStages> ring;
     uint32_t eph = 0;   // tempty phase
-    for (int t = t_begin; t < t_end; t += t_step) {
+    for (int t = tr.begin; t < tr.end; t += tr.step) {
       int prev = -1;
       for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&full_bar[s], ph);
+        mbar_wait(&full_bar[ring.s], ring.ph);
         wgmma_fence();
-        const uint32_t a0 = smem_u32(smem_a + s * Cfg::kABytes);
-        const uint32_t b0 = smem_u32(smem_b + s * Cfg::kBBytes);
+        const uint32_t a0 = smem_u32(smem_a + ring.s * Cfg::kABytes);
+        const uint32_t b0 = smem_u32(smem_b + ring.s * Cfg::kBBytes);
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
           // advance 16 fp16 = 32 B along K inside the swizzle atom; rows 64..127 of A start 64 x 128 B further
@@ -300,8 +646,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         wgmma_wait<1>();
         __syncwarp();
         if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-        prev = s;
-        if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
+        prev = ring.s;
+        ring.advance();
       }
       wgmma_wait<0>();
       __syncwarp();
@@ -323,311 +669,26 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
   } else {
     // ================= epilogue warps: shared fp32 tile -> registers -> swizzled smem box -> TMA store =================
-    const int quad = warp;  // 32-row quarter of the tile this warp owns (one row per lane)
-    uint8_t* my_bufs = smem_epi + warp * (kStageBufs * kStageBufBytes);
-    float pv = 0.f;       // EPI_RESID_HL: the pivot SHIFT of this GEMM for this thread's row
-    float pv_prev = 0.f;  // EPI_RESID_HL: the pivot the stored pair is relative to
-    int pv_mblk = -1;
-    uint64_t* my_rbar = resid_bar + warp * kStageBufs;
+    Epilogue<EPI> epi{EpiWarp{p, &tmap_out, &tmap_aux, lane, warp, smem_acc + (warp * 32 + lane) * (BN * 4),
+                              smem_epi + warp * (kStageBufs * kStageBufBytes), resid_bar + warp * kStageBufs, tr, n_blocks}};
     uint32_t aph = 0;
-    int cb = 0;                 // staging buffer to use next
-    uint32_t rph = 0;           // phase bit per staging buffer (residual loads)
-    const uint8_t* acc_row = smem_acc + (quad * 32 + lane) * (BN * 4);
-    // this thread's row, accumulator columns [col, col + 32) (col a multiple of 32)
-    auto acc_ld32 = [&](int col, uint32_t* r) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const uint4 v = *reinterpret_cast<const uint4*>(acc_row + ((((col >> 2) + (i ^ (lane & 7)))) << 4));
-        r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
-      }
-    };
-    // chunk geometry: a chunk is one 32-row x 128-byte output box of this warp
-    constexpr int kChunkCols = (EPI == EPI_RESID || EPI == EPI_TOPK) ? 32 : 64;   // accumulator = output columns
-    constexpr int kChunks = BN / kChunkCols;
-    constexpr int kPairs = kStageBufs / 2;   // EPI_RESID_HL: (hi, lo) box pairs of this warp (one)
-    const bool use_resid = (EPI == EPI_RESID) && p.has_resid;
-
-    // EPI_RESID: residual boxes are TMA-loaded one chunk ahead (flat over (tile, chunk) of this CTA)
-    auto out_col = [&](int t, int c) { return tile_n(t) * BN + c * kChunkCols; };
-    auto chunk_valid = [&](int t, int c) { return t < t_end && out_col(t, c) < p.N; };
-    auto issue_resid = [&](int t, int c, int buf) {  // lane 0 only
-      if constexpr (kHL) {   // buf = pair index: hi box, then lo box, one barrier for both
-        uint8_t* pb = my_bufs + buf * 2 * kStageBufBytes;
-        mbar_expect_tx(&my_rbar[buf], 2 * kStageBufBytes);
-        tma_load_2d(pb, &tmap_out, &my_rbar[buf], out_col(t, c), row_base(tile_m(t)) + quad * 32);
-        tma_load_2d(pb + kStageBufBytes, &tmap_aux, &my_rbar[buf], out_col(t, c), row_base(tile_m(t)) + quad * 32);
-      } else {
-        mbar_expect_tx(&my_rbar[buf], kStageBufBytes);
-        tma_load_2d(my_bufs + buf * kStageBufBytes, &tmap_out, &my_rbar[buf], out_col(t, c),
-                    row_base(tile_m(t)) + quad * 32);
-      }
-    };
-    // residual prefetch cursor: runs kAhead chunks in front of the chunk being processed (flat over this CTA's
-    // (tile, chunk) sequence); EPI_RESID_HL: 0, the single pair is loaded at the start of its own chunk
-    constexpr int kRing = kHL ? kPairs : kStageBufs;   // residual-load ring: boxes, or box pairs
-    constexpr int kAhead = kHL ? kPairs - 1 : (kStageBufs - 2 > 0 ? kStageBufs - 2 : 1);
-    int pf_t = t_begin, pf_c = 0, pf_buf = 0;
-    auto pf_issue = [&]() {  // lane 0 only
-      if (!chunk_valid(pf_t, pf_c)) return;
-      issue_resid(pf_t, pf_c, pf_buf);
-      if (++pf_buf == kRing) pf_buf = 0;
-      if (++pf_c >= kChunks || !chunk_valid(pf_t, pf_c)) { pf_t += t_step; pf_c = 0; }
-    };
-    if ((use_resid || kHL) && lane == 0) {
-#pragma unroll
-      for (int i = 0; i < kAhead; ++i) pf_issue();
-    }
-
-    // EPI_TOPK: this thread's running top-8 (descending) over the columns this CTA walks for its current row
-    float tk_v[EPI == EPI_TOPK ? kTopK : 1];
-    int tk_i[EPI == EPI_TOPK ? kTopK : 1];
-    int tk_mblk = -1;
-    auto tk_reset = [&]() {
-#pragma unroll
-      for (int i = 0; i < (EPI == EPI_TOPK ? kTopK : 1); ++i) { tk_v[i] = -INFINITY; tk_i[i] = -1; }
-    };
-    auto tk_flush = [&](int m_blk_done) {   // this CTA's list for the row it has just left
-      const int row = row_base(m_blk_done) + quad * 32 + lane;
-      if (row < p.M) {
-        const size_t at = (static_cast<size_t>(row) * gridDim.x + bid) * kTopK;
-#pragma unroll
-        for (int i = 0; i < (EPI == EPI_TOPK ? kTopK : 1); ++i) { p.topk_idx[at + i] = tk_i[i]; p.topk_score[at + i] = tk_v[i]; }
-      }
-    };
-    for (int t = t_begin; t < t_end; t += t_step) {
-      const int m_blk = tile_m(t);
-      const int row0 = row_base(m_blk) + quad * 32;
+    for (int t = tr.begin; t < tr.end; t += tr.step) {
+      const int m_blk = t / n_blocks, n_blk = t % n_blocks;
       // grouped weights with a bias per matrix (stacked like the matrices): the row block adds its matrix's
       const float* bias = (p.bias && p.grp_rows > 0) ? p.bias + static_cast<size_t>((m_blk * BM) / p.grp_rows) * p.bias_stride : p.bias;
-      if constexpr (EPI == EPI_TOPK) {
-        if (m_blk != tk_mblk) {
-          if (tk_mblk >= 0) tk_flush(tk_mblk);
-          tk_reset();
-          tk_mblk = m_blk;
-        }
-      }
-      float st1 = 0.f, st2 = 0.f;   // EPI_RESID_HL: this row's (sum, sum of squares) over the current 128-column slice
-      if constexpr (kHL) {
-        // pivot shift of this row: the stored pair is x - pivot_in; the new pivot is pivot_in + (mean of x - pivot_in),
-        // read from the previous residual GEMM's statistics (0 for the first one: the embedding's pair is x itself)
-        if (m_blk != pv_mblk) {
-          pv = 0.f;
-          pv_prev = 0.f;
-          if (p.pivot_in_stats) {
-            const int row = row0 + lane < p.M ? row0 + lane : p.M - 1;
-            float s1 = 0.f;
-            const int parts = p.N >> 7;
-            for (int k = 0; k < parts; ++k)
-              s1 += __ldg(reinterpret_cast<const float2*>(p.pivot_in_stats) + static_cast<size_t>(k) * p.M + row).x;
-            pv = s1 / static_cast<float>(p.N);
-            pv_prev = __ldg(p.pivot_in + row);
-          }
-          pv_mblk = m_blk;
-        }
-      }
+      epi.row_block(m_blk);
       mbar_wait(tfull_bar, aph);
       aph ^= 1;
-
-      if constexpr (EPI == EPI_TOPK) {
-        // This warp scans the tile's columns 32 at a time.  The common path per chunk is the maximum of 32 scores and
-        // one compare against the list's tail; validity (invalidated rows, padding rows >= topk_n) is only looked up
-        // for a score that would enter the list -- after the first tiles that is rare.
-        auto topk_chunk = [&](uint32_t* r, int ocol0) {
-          float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            m0 = fmax3(m0, __uint_as_float(r[i]), __uint_as_float(r[i + 1]));
-            m1 = fmax3(m1, __uint_as_float(r[i + 2]), __uint_as_float(r[i + 3]));
-            m2 = fmax3(m2, __uint_as_float(r[i + 4]), __uint_as_float(r[i + 5]));
-            m3 = fmax3(m3, __uint_as_float(r[i + 6]), __uint_as_float(r[i + 7]));
-          }
-          // Take the chunk's maximum while it beats the list's tail (usually zero or one round): a round is ~150
-          // instructions, against ~1300 for trying all 32 scores in turn.
-          float cm = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-          while (cm > tk_v[kTopK - 1]) {   // strict: an equal score at a higher column never displaces
-            int ci = 31;
-#pragma unroll
-            for (int i = 30; i >= 0; --i)
-              if (__uint_as_float(r[i]) == cm) ci = i;          // lowest column holding the maximum
-            ci = __uint_as_float(r[31]) == cm && ci == 31 ? 31 : ci;
-            float cv = cm;
-            int cidx = ocol0 + ci;
-            const bool ok = cidx < p.topk_n && (!p.topk_valid || __ldg(p.topk_valid + (cidx < p.topk_n ? cidx : 0)));
-            if (ok) {
-              // insertion into the descending list: strict > finds the slot (after any equal score, which has the lower
-              // column), and from there every entry shifts down one, ties included, so the tail is the one dropped
-              bool shift = false;
-#pragma unroll
-              for (int j = 0; j < kTopK; ++j) {
-                if (shift || cv > tk_v[j]) {
-                  shift = true;
-                  const float tv = tk_v[j]; const int ti = tk_i[j];
-                  tk_v[j] = cv; tk_i[j] = cidx;
-                  cv = tv; cidx = ti;
-                }
-              }
-            }
-            float n0 = -INFINITY, n1 = -INFINITY;
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {   // drop it and find the next maximum
-              if (i == ci) r[i] = 0xff800000u;
-              if (i + 1 == ci) r[i + 1] = 0xff800000u;
-              n0 = fmaxf(n0, __uint_as_float(r[i]));
-              n1 = fmaxf(n1, __uint_as_float(r[i + 1]));
-            }
-            cm = fmaxf(n0, n1);
-          }
-        };
-#pragma unroll 1
-        for (int c = 0; c < kChunks; ++c) {
-          uint32_t r[32];
-          acc_ld32(c * 32, r);
-          topk_chunk(r, out_col(t, c));
-        }
-      }
-      if constexpr (kHL) {
-        // 64-column chunks: the (hi, lo) boxes of the chunk arrive by TMA, are updated in place in shared memory and
-        // leave by TMA; statistics go out per 128-column slice
-#pragma unroll 1
-        for (int c = 0; c < kChunks; ++c) {
-          const int ocol0 = out_col(t, c);
-          if (ocol0 >= p.N) break;
-          uint8_t* hb = my_bufs + cb * 2 * kStageBufBytes;
-          uint8_t* lb = hb + kStageBufBytes;
-          if (lane == 0) {
-            // the pair the prefetch cursor points at was last stored kPairs - kAhead chunks ago: read out by now
-            bulk_wait_read<kPairs - kAhead - 1>();
-            pf_issue();
-          }
-          mbar_wait(&my_rbar[cb], (rph >> cb) & 1u);
-          rph ^= 1u << cb;
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            uint32_t r[32];
-            acc_ld32(c * 64 + hf * 32, r);
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {   // 16-byte units: 8 columns each
-              const uint32_t off = box_off(lane, hf * 4 + u);
-              uint4 hv = *reinterpret_cast<const uint4*>(hb + off);
-              uint4 lv = *reinterpret_cast<const uint4*>(lb + off);
-              uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hw[k]));
-                const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lw[k]));
-                float x0 = (fh.x + fl.x) + (__uint_as_float(r[8 * u + 2 * k]) - pv);
-                float x1 = (fh.y + fl.y) + (__uint_as_float(r[8 * u + 2 * k + 1]) - pv);
-                if (bias) {
-                  const float2 b = __ldg(reinterpret_cast<const float2*>(bias + ocol0 + hf * 32 + 8 * u) + k);
-                  x0 += b.x; x1 += b.y;
-                }
-                st1 += x0 + x1;
-                st2 += x0 * x0 + x1 * x1;
-                const __half2 nh = __floats2half2_rn(x0, x1);
-                const float2 fb = __half22float2(nh);
-                hw[k] = *reinterpret_cast<const uint32_t*>(&nh);
-                lw[k] = pack_half2(x0 - fb.x, x1 - fb.y);
-              }
-              sts16(hb + off, hw[0], hw[1], hw[2], hw[3]);
-              sts16(lb + off, lw[0], lw[1], lw[2], lw[3]);
-            }
-          }
-          if (c & 1) {   // a 128-column slice is complete: its partial goes out, once
-            if (row0 + lane < p.M) {
-              const size_t part = static_cast<size_t>((ocol0 - 64) >> 7);
-              *reinterpret_cast<float2*>(p.row_stats + 2 * (part * p.M + row0 + lane)) = make_float2(st1, st2);
-              if (part == 0) p.pivot_out[row0 + lane] = pv_prev + pv;
-            }
-            st1 = 0.f;
-            st2 = 0.f;
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(&tmap_out, hb, ocol0, row0);
-            tma_store_2d(&tmap_aux, lb, ocol0, row0);
-            bulk_commit();
-          }
-          if (++cb == kPairs) cb = 0;
-        }
-      }
-#pragma unroll 1
-      for (int c = 0; c < ((EPI == EPI_TOPK || kHL) ? 0 : kChunks); ++c) {
-        const int ocol0 = out_col(t, c);
-        if (ocol0 >= p.N) break;   // the last column tile of an N % 128 == 64 output is half empty
-        uint8_t* buf = my_bufs + cb * kStageBufBytes;
-        uint8_t* my_row = buf;  // + box_off(lane, chunk16)
-        if (use_resid) {
-          // the box the prefetch cursor points at was last used kStageBufs - kAhead chunks ago: its store must have
-          // been read out (all but the newest kStageBufs - kAhead - 1 store groups complete)
-          if (lane == 0) {
-            bulk_wait_read<(kStageBufs - kAhead - 1 > 0 ? kStageBufs - kAhead - 1 : 0)>();
-            pf_issue();
-          }
-          mbar_wait(&my_rbar[cb], (rph >> cb) & 1u);
-          rph ^= 1u << cb;
-        } else {
-          if (lane == 0) bulk_wait_read<kStageBufs - 1>();  // this buffer's previous store has been read out
-          __syncwarp();
-        }
-
-        if constexpr (EPI == EPI_RESID) {
-          uint32_t r[32];
-          acc_ld32(c * 32, r);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float4* q = reinterpret_cast<float4*>(my_row + box_off(lane, i));
-            float4 x = use_resid ? *q : make_float4(0.f, 0.f, 0.f, 0.f);
-            x.x += __uint_as_float(r[4 * i]);
-            x.y += __uint_as_float(r[4 * i + 1]);
-            x.z += __uint_as_float(r[4 * i + 2]);
-            x.w += __uint_as_float(r[4 * i + 3]);
-            if (bias) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(bias + ocol0) + i);
-              x.x += b.x; x.y += b.y; x.z += b.z; x.w += b.w;
-            }
-            *q = x;
-          }
-        } else if constexpr (EPI == EPI_F16 || EPI == EPI_GELU) {
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            uint32_t r[32];
-            acc_ld32(c * 64 + hf * 32, r);
-            uint32_t h[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              float v0 = __uint_as_float(r[2 * i]), v1 = __uint_as_float(r[2 * i + 1]);
-              if (bias) {
-                const float2 b = __ldg(reinterpret_cast<const float2*>(bias + ocol0 + hf * 32) + i);
-                v0 += b.x; v1 += b.y;
-              }
-              if constexpr (EPI == EPI_GELU) { v0 = gelu_erf_fast_f(v0); v1 = gelu_erf_fast_f(v1); }
-              h[i] = pack_half2(v0, v1);
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              sts16(my_row + box_off(lane, hf * 4 + i), h[4 * i], h[4 * i + 1], h[4 * i + 2], h[4 * i + 3]);
-          }
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmap_out, buf, ocol0, row0);  // rows >= M / cols >= N are clipped by the TMA unit
-          bulk_commit();
-        }
-        if (++cb == kStageBufs) cb = 0;
-      }
+      epi.tile(t, m_blk, n_blk, bias);
       // release the accumulator tile back to the MMA warpgroup
       __syncwarp();
       if (lane == 0) mbar_arrive(tempty_bar);
     }
-    if constexpr (EPI == EPI_TOPK) {
-      if (tk_mblk >= 0) tk_flush(tk_mblk);
-    }
+    epi.finish();
     if (lane == 0) bulk_wait_read<0>();  // smem must outlive the last stores' reads
     __syncwarp();
   }
-  __syncthreads();
+  cta_sync<1>();
 }
 
 // ================= the LayerNorm-fold projections (EPI_ROPE, EPI_GEGLU) on 128 x 192 tiles =================
@@ -642,9 +703,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 // thread.  The 96 accumulators and the epilogue fit in that without spilling (-Xptxas -v: 166-168).
 // 192 = three 64-wide heads, and in the fragment columns c and c + 32 sit in the same thread, which is the pairing of
 // both rotate-half RoPE and the 32-row (a | b) interleave of the GeGLU weights.
-// Schedule: persistent, one contiguous range of tiles per worker (n fastest), so that a worker walks all N tiles of its
-// row blocks back to back, the A row block stays hot in L2 and the per-row state (rstd, positions) is reused.
-// Thread-block clusters of CN CTAs along N (1: none): the schedule hands out CLUSTER tiles -- cn neighbouring tiles of
+// Thread-block clusters of CN CTAs along N (1: none): the schedule (contiguous ranges) hands out CLUSTER tiles -- cn neighbouring tiles of
 // one row block -- and CTA rn of the cluster computes tile (m_c, cn n_c + rn) of cluster tile (m_c, n_c).  The cn CTAs
 // share the A row block: each loads a 1/cn slice of the A box and multicasts it to all of them, so an A k-block is read
 // out of L2 once per cluster instead of once per CTA.  All CTAs of a cluster walk the same cluster tiles and k-blocks in
@@ -658,6 +717,7 @@ constexpr int kWideThreads = 32 * 9;
 
 template <int EPI>
 struct WideCfg {
+  static constexpr int kBN = BNW;   // W box height
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BNW * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
@@ -675,8 +735,7 @@ struct WideCfg {
 template <int EPI, int CN>
 __global__ void __launch_bounds__(kWideThreads, 1)
 gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap /*unused*/,
-                 const KArgs p) {
+                 const __grid_constant__ CUtensorMap tmap_out, const KArgs p) {
   static_assert(EPI == EPI_ROPE || EPI == EPI_GEGLU, "the wide kernel serves the LayerNorm-fold projections");
   using Cfg = WideCfg<EPI>;
   static_assert(Cfg::kSmemBytes <= kSmemLimit, "over the 227 KB shared-memory opt-in limit");
@@ -694,62 +753,17 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int m_blocks = (p.M + BM - 1) / BM;
   const int n_blocks = (p.N + BNW - 1) / BNW;
   const int k_blocks = (p.K + BK - 1) / BK;
-  // cluster tiles and contiguous ranges (see above)
   constexpr int cn = CN;
   const int rn = blockIdx.x % cn;
-  const int n_cblocks = (n_blocks + cn - 1) / cn;
-  const int num_tiles = m_blocks * n_cblocks;
-  const int num_workers = gridDim.x / cn;
-  const int base = num_tiles / num_workers, rem = num_tiles % num_workers;
-  const int bid = blockIdx.x / cn;
-  const int t_begin = bid * base + (bid < rem ? bid : rem);
-  const int t_end = t_begin + base + (bid < rem ? 1 : 0);
+  const int n_cblocks = (n_blocks + cn - 1) / cn;   // cluster tiles per row block (see above)
+  const TileRange tr = tile_range(m_blocks, n_cblocks, blockIdx.x / cn, gridDim.x / cn, false, false);
 
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_out);
-#pragma unroll
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8 * cn);   // one arrival per MMA warp of every CTA of the cluster
-    }
-    mbar_fence_init();
-  }
-  // no CTA of the cluster multicasts into another or arrives on its barriers before those barriers exist
-  if constexpr (CN > 1) cluster_sync();
-  else __syncthreads();
-  griddep_launch_dependents();
-  griddep_wait();
+  // one arrival per MMA warp of every CTA of the cluster frees a stage
+  kernel_prologue<CN, Cfg::kStages>(&tmap_a, &tmap_b, &tmap_out, full_bar, empty_bar, 8 * cn, [] {});
 
   if (warp == 8) {
     // ================= TMA producer =================
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      // this CTA's slice of the shared A box (tensor-map box height BM / cn rows, a multiple of the 8-row swizzle atom,
-      // so the slices assemble into exactly the tile layout one full-box load would give), multicast to the whole cluster
-      const int a_rows = BM / cn;
-      const uint16_t a_mask = static_cast<uint16_t>((1u << cn) - 1);
-      for (int t = t_begin; t < t_end; ++t) {
-        const int m_blk = t / n_cblocks, n_blk = (t % n_cblocks) * cn + rn;
-        // grouped weights (one matrix per task, stacked along N): the row block picks its matrix; blocks never straddle
-        // two groups (grp_rows is a multiple of the block height, checked on the host)
-        const int w_row0 = p.grp_rows > 0 ? ((m_blk * BM) / p.grp_rows) * p.N : 0;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          const int kc = kb * BK;
-          // the stage fills with the A slices of every CTA of the cluster and this CTA's own W box: the whole stage
-          mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
-          uint8_t* da = smem_a + s * Cfg::kABytes + rn * a_rows * (BK * 2);
-          const int ya = m_blk * BM + rn * a_rows;
-          if (cn > 1) tma_load_2d_multicast(da, &tmap_a, &full_bar[s], kc, ya, a_mask);
-          else tma_load_2d(da, &tmap_a, &full_bar[s], kc, ya);
-          tma_load_2d(smem_b + s * Cfg::kBBytes, &tmap_b, &full_bar[s], kc, w_row0 + n_blk * BNW);
-          if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
+    if (lane == 0) produce_operands<Cfg, CN>(&tmap_a, &tmap_b, smem_a, smem_b, full_bar, empty_bar, tr, n_cblocks, rn, k_blocks, p);
   } else {
     // ================= MMA warpgroups, epilogue from the accumulator fragment =================
     const int wg = warp >> 2;         // 64-row half of the tile
@@ -763,8 +777,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     float rstd[2] = {1.f, 1.f};   // per row of the thread: the fold's rstd and (EPI_ROPE) the position
     int pos[2] = {0, 0};
     int row_mblk = -1;
-    int s = 0;
-    uint32_t ph = 0;
+    Ring<Cfg::kStages> ring;
     // a stage of this CTA is written by the producers of every CTA of its cluster (A slices): freeing it is one
     // arrival on the empty barrier of each of them, lane i for CTA i, so that the arrivals go out side by side on the
     // MMA warp's critical path
@@ -775,7 +788,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         mbar_arrive_cluster(&empty_bar[st], lane);
       }
     };
-    for (int t = t_begin; t < t_end; ++t) {
+    for (int t = tr.begin; t < tr.end; t += tr.step) {
       const int m_blk = t / n_cblocks, n_blk = (t % n_cblocks) * cn + rn;
       const int row0 = m_blk * BM + 64 * wg + 16 * wq;   // first row of this warp's boxes
       if (m_blk != row_mblk) {   // per-row state, reloaded only when the row block changes
@@ -801,10 +814,10 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
       int prev = -1;
       for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&full_bar[s], ph);
+        mbar_wait(&full_bar[ring.s], ring.ph);
         wgmma_fence();
-        const uint32_t a0 = smem_u32(smem_a + s * Cfg::kABytes) + wg * 64 * 128;
-        const uint32_t b0 = smem_u32(smem_b + s * Cfg::kBBytes);
+        const uint32_t a0 = smem_u32(smem_a + ring.s * Cfg::kABytes) + wg * 64 * 128;
+        const uint32_t b0 = smem_u32(smem_b + ring.s * Cfg::kBBytes);
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k)
           wgmma_m64n192k16(acc, gmma_desc_sw128(a0 + 32 * k), gmma_desc_sw128(b0 + 32 * k), (kb > 0 || k > 0) ? 1u : 0u);
@@ -812,8 +825,8 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         wgmma_wait<1>();
         __syncwarp();
         if (prev >= 0) release(prev);
-        prev = s;
-        if (++s == Cfg::kStages) { s = 0; ph ^= 1; }
+        prev = ring.s;
+        ring.advance();
       }
       wgmma_wait<0>();
       __syncwarp();
@@ -897,9 +910,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (lane == 0) bulk_wait_read<0>();   // smem must outlive the last stores' reads
     __syncwarp();
   }
-  // no CTA leaves while another of its cluster may still arrive on its barriers
-  if constexpr (CN > 1) cluster_sync();
-  else __syncthreads();
+  cta_sync<CN>();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -923,91 +934,95 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// The kernel gemm_f16 launches for an epilogue, with its shared memory, block size and tile width: gemm_wide_kernel for
-// the LayerNorm-fold projections, in clusters of CN CTAs; gemm_kernel, which has no clusters, for every other epilogue.
-template <int EPI>
+// The kernel instance of an epilogue and cluster size: gemm_wide_kernel for the LayerNorm-fold projections, in clusters
+// of CN CTAs; gemm_kernel, which has no clusters, for every other epilogue.
+template <int EPI, int CN>
 struct Kernel {
   static constexpr bool kWide = EPI == EPI_ROPE || EPI == EPI_GEGLU;
-  template <int CN>
-  static constexpr auto fn() {
-    if constexpr (kWide) {
-      return gemm_wide_kernel<EPI, CN>;
-    } else {
-      static_assert(CN == 1, "gemm_kernel runs without clusters");
-      return gemm_kernel<EPI>;
-    }
-  }
-  static constexpr int kSmem = kWide ? WideCfg<EPI>::kSmemBytes : GemmCfg<EPI>::kSmemBytes;
+  static_assert(kWide || CN == 1, "gemm_kernel runs without clusters");
+  static constexpr int kCN = CN;
+  using Cfg = std::conditional_t<kWide, WideCfg<EPI>, GemmCfg>;
   static constexpr int kThreads = kWide ? kWideThreads : kGemmThreads;
-  static constexpr int kBN = kWide ? BNW : BN;
+  static constexpr auto fn() {
+    if constexpr (kWide) return gemm_wide_kernel<EPI, CN>;
+    else return gemm_kernel<EPI>;
+  }
 };
 
-// Clusters of CN CTAs of the kernel that are co-resident on the device.  A GPC holds a whole number of
-// clusters, so this is the occupancy query's answer, not num_sms / CN.  Asked once per kernel and cluster size
-// (all devices of one box are the same part).
-template <int EPI, int CN>
+// f(Kernel<EPI, CN>{}) for the kernel instance of (epi, cn): the one list of the instances gemm_f16 launches
+template <class F>
+int with_kernel(int epi, int cn, F&& f) {
+  switch (epi) {
+    case EPI_F16: return f(Kernel<EPI_F16, 1>{});
+    case EPI_ROPE: return cn == 2 ? f(Kernel<EPI_ROPE, 2>{}) : f(Kernel<EPI_ROPE, 1>{});
+    case EPI_RESID: return f(Kernel<EPI_RESID, 1>{});
+    case EPI_RESID_HL: return f(Kernel<EPI_RESID_HL, 1>{});
+    case EPI_GEGLU: return cn == 2 ? f(Kernel<EPI_GEGLU, 2>{}) : f(Kernel<EPI_GEGLU, 1>{});
+    case EPI_GELU: return f(Kernel<EPI_GELU, 1>{});
+    case EPI_TOPK: return f(Kernel<EPI_TOPK, 1>{});
+  }
+  return -1;
+}
+
+// Launch configuration of kernel instance Kn but its grid, the cluster shape in attr[0].  The shared-memory opt-in is a
+// per-device attribute, cheap enough to set before every use (multi-GPU processes switch devices).
+template <class Kn>
+int kernel_config(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attr) {
+  SRB_CUDA_CHECK(cudaFuncSetAttribute(Kn::fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::Cfg::kSmemBytes));
+  cfg = {};
+  cfg.blockDim = dim3(Kn::kThreads);
+  cfg.dynamicSmemBytes = Kn::Cfg::kSmemBytes;
+  cfg.attrs = attr;
+  if (Kn::kCN > 1) {
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = Kn::kCN;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.numAttrs = 1;
+  }
+  return 0;
+}
+
+// Clusters of the kernel instance that are co-resident on the device.  A GPC holds a whole number of clusters, so
+// this is the occupancy query's answer, not num_sms / CN.  Asked once per instance (all devices of one box are the
+// same part).
+template <class Kn>
 int max_clusters(int num_sms) {
-  using Kn = Kernel<EPI>;
-  const auto fn = Kn::template fn<CN>();
-  constexpr int csize = CN;
   static std::atomic<int> cached{0};
   int n = cached.load(std::memory_order_relaxed);
   if (n > 0) return n;
-  SRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::kSmem));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(csize * num_sms);
-  cfg.blockDim = dim3(Kn::kThreads);
-  cfg.dynamicSmemBytes = Kn::kSmem;
-  cudaLaunchAttribute attr;
-  attr.id = cudaLaunchAttributeClusterDimension;
-  attr.val.clusterDim.x = csize;
-  attr.val.clusterDim.y = 1;
-  attr.val.clusterDim.z = 1;
-  cfg.attrs = &attr;
-  cfg.numAttrs = 1;
-  SRB_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&n, fn, &cfg));
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  if (kernel_config<Kn>(cfg, attr)) return -1;
+  cfg.gridDim = dim3(Kn::kCN * num_sms);
+  SRB_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&n, Kn::fn(), &cfg));
   if (n <= 0) {
-    fprintf(stderr, "[srb200] gemm_f16: no %d-CTA cluster of this kernel fits the device\n", csize);
+    fprintf(stderr, "[srb200] gemm_f16: no %d-CTA cluster of this kernel fits the device\n", Kn::kCN);
     return -1;
   }
   cached.store(n, std::memory_order_relaxed);
   return n;
 }
 
-template <int EPI, int CN = 1>
+template <class Kn>
 int launch(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
-           const CUtensorMap& tx, const KArgs& ka, int num_sms, int grid_override = 0) {
-  using Kn = Kernel<EPI>;
-  const auto fn = Kn::template fn<CN>();
-  // per-device attribute; cheap enough to set on every launch (multi-GPU processes switch devices)
-  SRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, Kn::kSmem));
-  constexpr int csize = CN;
-  const int tiles = ((ka.M + BM - 1) / BM) * ((ka.N + Kn::kBN * csize - 1) / (Kn::kBN * csize));   // cluster tiles
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(Kn::kThreads);
-  cfg.dynamicSmemBytes = Kn::kSmem;
-  cfg.stream = stream;
+           const CUtensorMap& tx, const KArgs& ka, int num_sms, int grid_override) {
+  cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
-  int nattr = 0;
+  if (kernel_config<Kn>(cfg, attr)) return -1;
+  cfg.stream = stream;
   if (pdl_enabled()) {
-    attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[nattr++].val.programmaticStreamSerializationAllowed = 1;
+    attr[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[cfg.numAttrs++].val.programmaticStreamSerializationAllowed = 1;
   }
+  constexpr int tile_n = Kn::Cfg::kBN * Kn::kCN;   // cluster tiles
+  const int tiles = ((ka.M + BM - 1) / BM) * ((ka.N + tile_n - 1) / tile_n);
   // persistent grid: one worker per co-resident cluster (one per SM without clusters)
-  int workers = num_sms;
-  if constexpr (csize > 1) {
-    attr[nattr].id = cudaLaunchAttributeClusterDimension;
-    attr[nattr].val.clusterDim.x = csize;
-    attr[nattr].val.clusterDim.y = 1;
-    attr[nattr++].val.clusterDim.z = 1;
-    workers = max_clusters<EPI, CN>(num_sms);
-    if (workers <= 0) return -1;
-  }
-  const int grid = grid_override > 0 ? grid_override : csize * (tiles < workers ? tiles : workers);
-  cfg.gridDim = dim3(grid);
-  cfg.attrs = attr;
-  cfg.numAttrs = nattr;
-  SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, fn, ta, tb, tc, tx, ka));
+  const int workers = Kn::kCN > 1 ? max_clusters<Kn>(num_sms) : num_sms;
+  if (workers <= 0) return -1;
+  cfg.gridDim = dim3(grid_override > 0 ? grid_override : Kn::kCN * (tiles < workers ? tiles : workers));
+  if constexpr (Kn::kWide) SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, Kn::fn(), ta, tb, tc, ka));
+  else SRB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, Kn::fn(), ta, tb, tc, tx, ka));
   note_launch();
   return 0;
 }
@@ -1080,10 +1095,7 @@ int gemm_cluster_workers(int epi, int N, int K) {
   const int cn = gemm_cluster_size(epi, N, K);
   const int num_sms = device_sms();
   if (num_sms <= 0 || cn == 1) return num_sms;
-  // gemm_cluster_size forms pairs for these two epilogues only
-  if (epi == EPI_ROPE) return max_clusters<EPI_ROPE, 2>(num_sms);
-  if (epi == EPI_GEGLU) return max_clusters<EPI_GEGLU, 2>(num_sms);
-  return -1;
+  return with_kernel(epi, cn, [&](auto kn) { return max_clusters<decltype(kn)>(num_sms); });
 }
 
 int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
@@ -1157,7 +1169,7 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
   ka.fold_stats = nullptr; ka.fold_eps = 0.f; ka.fold_inv_h = 0.f; ka.fold_parts = 0;
   ka.grp_rows = w_groups > 1 ? g.w_group_rows : 0;
   ka.bias_stride = (w_groups > 1 && g.bias_per_group) ? g.N : 0;
-  CUtensorMap tx = tc;   // auxiliary map (EPI_RESID_HL: the low halves of the pair); unused otherwise
+  CUtensorMap tx = tc;   // gemm_kernel's auxiliary map (EPI_RESID_HL: the low halves of the pair); unused otherwise
   if (is_hl && make_tmap_2d(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, g.lo16, g.N, g.M, g.N, 64, 32)) return -1;
   if (g.fold_stats) {
     if ((g.epi != EPI_ROPE && g.epi != EPI_GEGLU) || g.fold_h <= 0 || g.fold_h % 128 != 0) {
@@ -1168,39 +1180,26 @@ int gemm_f16(cudaStream_t stream, const GemmDesc& g) {
     ka.fold_inv_h = 1.0f / static_cast<float>(g.fold_h);
     ka.fold_parts = g.fold_h / 128;
   }
-  switch (g.epi) {
-    case EPI_F16: return launch<EPI_F16>(stream, ta, tb, tc, tx, ka, num_sms);
-    case EPI_ROPE:
-      return cn == 2 ? launch<EPI_ROPE, 2>(stream, ta, tb, tc, tx, ka, num_sms)
-                     : launch<EPI_ROPE>(stream, ta, tb, tc, tx, ka, num_sms);
-    case EPI_RESID: return launch<EPI_RESID>(stream, ta, tb, tc, tx, ka, num_sms);
-    case EPI_RESID_HL: return launch<EPI_RESID_HL>(stream, ta, tb, tc, tx, ka, num_sms);
-    case EPI_GEGLU:
-      return cn == 2 ? launch<EPI_GEGLU, 2>(stream, ta, tb, tc, tx, ka, num_sms)
-                     : launch<EPI_GEGLU>(stream, ta, tb, tc, tx, ka, num_sms);
-    case EPI_GELU: return launch<EPI_GELU>(stream, ta, tb, tc, tx, ka, num_sms);
-    case EPI_TOPK: {
-      if (!g.topk_idx || !g.topk_score || !g.topk_lists || g.N % 256 != 0) {
-        fprintf(stderr, "[srb200] gemm_f16: EPI_TOPK needs list buffers and N %% 256 == 0\n");
-        return -1;
-      }
-      // the query batch is the short dimension here, the stored rows stream as N; one list per worker and query row
-      const int m_blocks = (g.M + BM - 1) / BM, n_blocks = g.N / BN;
-      const long long tiles = static_cast<long long>(m_blocks) * n_blocks;
-      // grouped schedule (kernel comment at t_step): whole groups of m_blocks workers, each group at least one tile.
-      // SRB_TOPK_GROUPED=0 restores the contiguous ranges (A/B measurements).
-      static const bool grouped_on = [] { const char* e = getenv("SRB_TOPK_GROUPED"); return !(e && e[0] == '0'); }();
-      const int groups = m_blocks > 0 ? num_sms / m_blocks : 0;
-      if (grouped_on && m_blocks > 1 && groups >= 1 && n_blocks >= groups) {
-        ka.grouped = 1;
-        *g.topk_lists = groups * m_blocks;
-        return launch<EPI_TOPK>(stream, ta, tb, tc, tx, ka, num_sms, groups * m_blocks);
-      }
-      *g.topk_lists = static_cast<int>(tiles < num_sms ? tiles : num_sms);
-      return launch<EPI_TOPK>(stream, ta, tb, tc, tx, ka, num_sms);
+  int grid = 0;   // 0: the persistent grid of launch
+  if (g.epi == EPI_TOPK) {
+    if (!g.topk_idx || !g.topk_score || !g.topk_lists || g.N % 256 != 0) {
+      fprintf(stderr, "[srb200] gemm_f16: EPI_TOPK needs list buffers and N %% 256 == 0\n");
+      return -1;
     }
+    // the query batch is the short dimension here, the stored rows stream as N; one list per worker and query row
+    const int m_blocks = (g.M + BM - 1) / BM, n_blocks = g.N / BN;
+    const long long tiles = static_cast<long long>(m_blocks) * n_blocks;
+    // grouped schedule (tile_range): whole groups of m_blocks workers, each group at least one tile.
+    // SRB_TOPK_GROUPED=0 restores the contiguous ranges (A/B measurements).
+    static const bool grouped_on = [] { const char* e = getenv("SRB_TOPK_GROUPED"); return !(e && e[0] == '0'); }();
+    const int groups = m_blocks > 0 ? num_sms / m_blocks : 0;
+    if (grouped_on && m_blocks > 1 && groups >= 1 && n_blocks >= groups) {
+      ka.grouped = 1;
+      grid = groups * m_blocks;
+    }
+    *g.topk_lists = ka.grouped ? grid : static_cast<int>(tiles < num_sms ? tiles : num_sms);
   }
-  return -1;
+  return with_kernel(g.epi, cn, [&](auto kn) { return launch<decltype(kn)>(stream, ta, tb, tc, tx, ka, num_sms, grid); });
 }
 
 }  // namespace srb
