@@ -1,12 +1,18 @@
 """Per-token hidden rows of the whole encoder against float64 (TEST INFRASTRUCTURE ONLY; see encoder_oracle.py header).
 
-Four things, used by tests/test_hidden_oracle.py (CPU) and tests/test_encoder_hidden_conformance_gpu.py (GPU):
+Five things, used by tests/test_hidden_oracle.py (CPU), tests/test_encoder_hidden_conformance_gpu.py and
+tests/test_encoder_long_context_gpu.py (GPU):
 
   * `trained_like_modernbert_weights`: a second synthetic family next to synth.make_modernbert_weights with the statistics
     of trained ModernBERT / mmBERT checkpoints that the LayerNorm fold and the fp16 pair exist for: LayerNorm gains
     log-uniform over [0.05, 8], a few outlier residual channels 34 - 58x the median entry, row means far from zero.
   * `modernbert_hidden64` / `bert_hidden64`: the residual stream after every layer from encoder_oracle's forward, run on
     float64 copies of the fp32 checkpoint values.
+  * `modernbert_hidden64_long`: the same forward for sequences up to 32 768 tokens and batches of 131 072 rows.  It takes
+    [B, S] ids, runs attention a chunk of queries at a time over only the keys they see (`chunked_attention`: all keys on a
+    global layer, the band |i - j| <= local_attention / 2 on a local one), so no [S, S] tensor exists, and keeps float64
+    rows only at the depths asked for, with the running sum_j s_j that row_bound needs (`Hidden64`).  Its memory is
+    bounded by B and the query chunk (its docstring).
   * `row_bound`: the per-row error bound, stated once, for the production path (fp16 operands) and the precise path
     (fp32 accumulation on the tensor cores).
   * `modernbert_restated` / `bert_restated`: the float64 forward with operands rounded to fp16 exactly where
@@ -38,6 +44,21 @@ to cover it with the margin of 2 a bound should keep; nothing else in it is fitt
 restatement and not by the derivation alone: tests/test_hidden_oracle.py shows that on every family and geometry the restated engine
 stays inside it with a margin >= 2 and by how much each wrong engine of MUTATIONS leaves it (> 10x, but for one
 dropped statistics block at the geometries where a block is a third or a sixth of the row: 5.7x - 9x).
+
+LONG CONTEXT.  The count above does not depend on the number of keys n: a softmax row is a weighted mean of v, and
+rounding each normal weight of P to fp16 moves it by at most 2^-11 of the weighted mean of |v|, whatever n.  Two terms do
+grow with n.  Weights below 2^-14 are fp16 subnormals, rounded with an absolute 2^-25 against a denominator >= 1: n 2^-25
+in the worst case (2^-10 at 32 768 keys), but the roundings take either sign and add as sqrt(n) 2^-25, 2^-17.5 at 32 768.
+The fp32 denominator summed over n / 64 key blocks adds (n / 64) 2^-24 at worst, 2^-15 at 32 768.  Both stay below the
+2^-11 of one rounding.  The restatement, with the same chunked attention as the long form, shows it at 4096 tokens
+(global layers over all 4096 keys, windows at positions up to 4095): at most 0.31 of the bound on the plain,
+trained-like and wide families at H 768 and 384, as at 300 tokens.  A rope row read at fp16(position) or at
+position % 2048 leaves the bound by > 70x on the rows past 2048 (wide family, H 768).  Measured on an H100 80GB HBM3 at
+700 W, the engine's rows at 2049, 8192 and 32 768 tokens and in the 131 072-row batch reach at most 0.47 of the bound on
+the production path and 0.39 on the precise one.  The precise path's attention sums all keys of a global row in one fp32
+chain, whose rounding grows as sqrt(n) 2^-24; on the trained-like family its worst row goes from 0.14 of the bound at
+8192 tokens to 0.37 at 32 768, the longest position table of the mmBERT checkpoints.  Whether that chain is the cause
+is not established.
 
 The precise path (csrc/precise.cu) splits every GEMM operand into an fp16 pair and accumulates in fp32 on the tensor
 cores; everything between the GEMMs is fp32.  Its u is precise_u(cfg) = TAU_MEASURED * 0.64 sqrt(K), K = max(H, I) the
@@ -74,6 +95,7 @@ FP16_SAFE = 3e4                 # trained-like family: |q|, |k|, |v|, |ctx|, |Ge
 OUTLIER_CHANNELS = 4
 OUTLIER_ROW_SCALE = 4.0
 COMMON_SIGMA = 3.0
+Q_CHUNK = 256                   # query rows per attention chunk of the float64 forwards (chunked_attention)
 
 
 # --------------------------------------------------------------------------------------
@@ -155,6 +177,59 @@ def bert_hidden64(w64: Dict[str, torch.Tensor], cfg: eo.BertConfig, ids, real_le
     return [x[0] for x in out]
 
 
+class Hidden64:
+    """One sequence's float64 rows at some depths (1-based) and, per depth d, the [S] sum_{j <= d} s_j of row_bound"""
+
+    def __init__(self, rows: Dict[int, torch.Tensor], scale_sums: Dict[int, torch.Tensor]):
+        self.rows, self.scale_sums = rows, scale_sums
+
+
+def modernbert_hidden64_long(w64: Dict[str, torch.Tensor], cfg: eo.ModernBertConfig, ids, depths: Sequence[int],
+                             q_chunk: int = Q_CHUNK) -> List[Hidden64]:
+    """encoder_oracle.modernbert_forward on B sequences of S tokens each (ids [B, S]; unmasked), on the device of w64:
+    the float64 rows after each layer in `depths` and their row_bound scale sums, one Hidden64 per sequence.  Attention
+    runs per chunk of q_chunk queries over the keys the chunk sees (chunked_attention).  Peak memory is about
+    8 B S (7 H + 4 I) bytes for the activations plus 24 B heads q_chunk K bytes for one chunk's scores (K = S on a global
+    layer, q_chunk + local_attention on a local one), beside the rows kept: the caller bounds it with B and q_chunk."""
+    W = lambda name: eo._w(w64, name, eo.MODERNBERT_PREFIXES)
+    dev = next(iter(w64.values())).device
+    t = torch.as_tensor(np.asarray(ids, dtype=np.int64), device=dev)
+    t = t[None] if t.dim() == 1 else t
+    B, S = t.shape
+    H, heads, eps = cfg.hidden_size, cfg.num_attention_heads, cfg.layer_norm_eps
+    depths = sorted(set(depths))
+    tables = {local: tuple(c.to(dev).double()[None, :, None, :] for c in eo.rope_tables(64, theta, S))
+              for local, theta in ((False, cfg.global_rope_theta), (True, cfg.local_rope_theta))}
+
+    def rope(x, cos, sin):
+        x = x.reshape(B, S, heads, 64)
+        x1, x2 = x[..., :32], x[..., 32:]
+        return torch.cat([x1 * cos - x2 * sin, x1 * sin + x2 * cos], -1).reshape(B, S, H)
+
+    x = eo.layer_norm(W("embeddings.tok_embeddings.weight")[t], W("embeddings.norm.weight"), None, eps)
+    scale_sum = torch.zeros(B, S, dtype=torch.float64, device=dev)
+    rows, sums = {}, {}
+    for li in range(depths[-1]):
+        local = (li % cfg.global_attn_every_n_layers) != 0
+        g_an = W(f"layers.{li}.attn_norm.weight")
+        h = x if g_an is None else eo.layer_norm(x, g_an, None, eps)
+        qkv = h @ W(f"layers.{li}.attn.Wqkv.weight").t()
+        cos, sin = tables[local]
+        q, k, v = rope(qkv[..., :H], cos, sin), rope(qkv[..., H:2 * H], cos, sin), qkv[..., 2 * H:]
+        del qkv, h
+        ctx = chunked_attention(q, k, v, heads, cfg.local_attention // 2 if local else 0, q_chunk=q_chunk)
+        del q, k, v
+        x = ctx @ W(f"layers.{li}.attn.Wo.weight").t() + x
+        del ctx
+        a, b = (eo.layer_norm(x, W(f"layers.{li}.mlp_norm.weight"), None, eps) @ W(f"layers.{li}.mlp.Wi.weight").t()).chunk(2, dim=-1)
+        x = x + (eo.gelu_erf(a) * b) @ W(f"layers.{li}.mlp.Wo.weight").t()
+        del a, b
+        scale_sum = scale_sum + centred_rms(x)
+        if li + 1 in depths:
+            rows[li + 1], sums[li + 1] = x, scale_sum
+    return [Hidden64({d: rows[d][i] for d in depths}, {d: sums[d][i] for d in depths}) for i in range(B)]
+
+
 def precise_u(cfg) -> float:
     """u of the precise path for a ModernBertConfig (module docstring)"""
     return TAU_MEASURED * 0.64 * math.sqrt(max(cfg.hidden_size, cfg.intermediate_size))
@@ -165,26 +240,32 @@ def centred_rms(x: torch.Tensor) -> torch.Tensor:
     return (x - x.mean(-1, keepdim=True)).pow(2).mean(-1).sqrt()
 
 
-def row_bound(hidden64: Sequence[torch.Tensor], depth: int, u: float = U16) -> torch.Tensor:
+def row_bound(hidden64, depth: int, u: float = U16) -> torch.Tensor:
     """Bound [S] on every element of the rows after layer `depth` (1-based), given the float64 rows after layers 1 ...
-    depth (module docstring)."""
+    depth or a Hidden64 holding that depth (module docstring)."""
+    if isinstance(hidden64, Hidden64):
+        return GAIN * u * hidden64.scale_sums[depth]
     s = sum(centred_rms(hidden64[j]) for j in range(depth))
     return GAIN * u * s
 
 
-def worst_over_bound(got, hidden64: Sequence[torch.Tensor], depth: int, u: float = U16) -> float:
-    """max over rows of (largest element error) / bound; inf when `got` holds a NaN or inf"""
-    got = torch.as_tensor(got).to(hidden64[depth - 1].device).double()
+def worst_over_bound(got, hidden64, depth: int, u: float = U16, rows=slice(None)) -> float:
+    """max over `rows` of (largest element error) / bound; inf when `got` holds a NaN or inf.  hidden64: the float64 rows
+    after layers 1 ... depth, or a Hidden64 holding that depth."""
+    ref = hidden64.rows[depth] if isinstance(hidden64, Hidden64) else hidden64[depth - 1]
+    got = torch.as_tensor(got).to(ref.device).double()
     if not bool(torch.isfinite(got).all()):
         return math.inf
-    err = (got - hidden64[depth - 1]).abs().amax(-1)
-    return float((err / row_bound(hidden64, depth, u)).max())
+    err = (got - ref).abs().amax(-1)
+    return float((err / row_bound(hidden64, depth, u))[rows].max())
 
 
 # --------------------------------------------------------------------------------------
 # the engine restated in float64 with fp16 operands
 # --------------------------------------------------------------------------------------
 MUTATIONS = ("global_every", "rope_tables", "window", "geglu_halves", "fold_gamma", "stale_pivot", "stats_block", "stale_rows")
+# wrong engines that differ only at positions past 2048, config-wide: the rope row read at fp16(position), or at position % 2048
+FAR_POSITION_MUTATIONS = ("rope_pos_fp16", "rope_wrap_2048")
 
 
 def r16(t: torch.Tensor) -> torch.Tensor:
@@ -200,22 +281,34 @@ def _fold(w: torch.Tensor, gamma: torch.Tensor) -> torch.Tensor:
     return r16(row)
 
 
+def chunked_attention(q, k, v, heads: int, window: int, kv_len: Optional[int] = None, q_chunk: int = Q_CHUNK,
+                      p16: bool = False) -> torch.Tensor:
+    """softmax(0.125 q k^T) v on rows [B, S, heads * 64], a chunk of q_chunk query rows at a time over only the keys that
+    chunk can see: all of them (j < kv_len), or |i - j| <= window when window > 0.  No [S, S] tensor is built: one chunk's
+    scores are B * heads * q_chunk * K values, K = min(S, kv_len) or q_chunk + 2 window.  p16: P is rounded to fp16 for
+    P V while the denominator sums the unrounded weights, as attention_wgmma does."""
+    B, S, W = q.shape
+    sp = lambda t: t.reshape(B, S, heads, -1).transpose(1, 2)          # [B, heads, S, 64]
+    qh, kh, vh = sp(q), sp(k), sp(v)
+    keys = S if kv_len is None else min(S, kv_len)
+    out = torch.empty_like(qh)
+    for c0 in range(0, S, q_chunk):
+        c1 = min(S, c0 + q_chunk)
+        k0, k1 = (max(0, c0 - window), min(keys, c1 + window)) if window > 0 else (0, keys)
+        s = 0.125 * (qh[:, :, c0:c1] @ kh[:, :, k0:k1].transpose(-1, -2))
+        if window > 0:
+            i = torch.arange(c0, c1, device=q.device)
+            j = torch.arange(k0, k1, device=q.device)
+            s = s.masked_fill((j[None, :] - i[:, None]).abs() > window, -math.inf)
+        p = torch.exp(s - s.amax(-1, keepdim=True))
+        out[:, :, c0:c1] = ((r16(p) if p16 else p) @ vh[:, :, k0:k1]) / p.sum(-1, keepdim=True)
+    return out.transpose(1, 2).reshape(B, S, W)
+
+
 def _attention(q, k, v, heads: int, window: int, kv_len: Optional[int] = None) -> torch.Tensor:
     """attention_wgmma on fp16 q / k / v rows [S, heads * 64]: fp32 scores * 0.125, P rounded to fp16 for P V while the
     denominator sums the unrounded weights, fp16 context"""
-    S = q.shape[0]
-    sp = lambda t: t.reshape(S, heads, -1).transpose(0, 1)
-    s = 0.125 * (sp(q) @ sp(k).transpose(1, 2))
-    idx = torch.arange(S, device=q.device)
-    hide = torch.zeros(S, S, dtype=torch.bool, device=q.device)
-    if window > 0:
-        hide |= (idx[None, :] - idx[:, None]).abs() > window
-    if kv_len is not None:
-        hide |= idx[None, :] >= kv_len
-    s = s.masked_fill(hide[None], -math.inf)
-    p = torch.exp(s - s.amax(-1, keepdim=True))
-    o = (r16(p) @ sp(v)) / p.sum(-1, keepdim=True)
-    return r16(o.transpose(0, 1).reshape(S, -1))
+    return r16(chunked_attention(q[None], k[None], v[None], heads, window, kv_len, p16=True)[0])
 
 
 class _Pair:
@@ -275,7 +368,8 @@ def modernbert_restated(w64: Dict[str, torch.Tensor], cfg: eo.ModernBertConfig, 
                         mut: Optional[str] = None, mut_layer: int = 1, mut_row: int = 0, mut_block: int = 0,
                         probe: Optional[Dict[str, float]] = None) -> List[torch.Tensor]:
     """encoder_forward's ModernBERT branch on one sequence: [S, H] float64 rows (pivot + hi + lo) after each layer.
-    mut: one of MUTATIONS, applied at layer `mut_layer` (config-wide for the first three).  `probe` receives the largest
+    mut: one of MUTATIONS, applied at layer `mut_layer` (config-wide for the first three), or one of
+    FAR_POSITION_MUTATIONS (config-wide).  `probe` receives the largest
     |value| met at each place the engine stores fp16."""
     if mut == "global_every":
         cfg = replace(cfg, global_attn_every_n_layers=cfg.global_attn_every_n_layers + 1)
@@ -297,8 +391,14 @@ def modernbert_restated(w64: Dict[str, torch.Tensor], cfg: eo.ModernBertConfig, 
         x1, x2 = x[..., :32], x[..., 32:]
         return torch.cat([x1 * cos[:, None] - x2 * sin[:, None], x1 * sin[:, None] + x2 * cos[:, None]], -1).reshape(S, -1)
 
-    tables = {False: eo.rope_tables(64, cfg.global_rope_theta, S), True: eo.rope_tables(64, cfg.local_rope_theta, S)}
-    x0 = eo.layer_norm(W("embeddings.tok_embeddings.weight")[t], W("embeddings.norm.weight"), None, eps)
+    pos = torch.arange(S)
+    if mut == "rope_pos_fp16":          # the table row read at fp16(position): exact only up to 2048
+        pos = pos.to(torch.float16).long()
+    if mut == "rope_wrap_2048":
+        pos = pos % 2048
+    tables = {local: tuple(c[pos] for c in eo.rope_tables(64, theta, int(pos.max()) + 1))
+              for local, theta in ((False, cfg.global_rope_theta), (True, cfg.local_rope_theta))}
+    x0 =eo.layer_norm(W("embeddings.tok_embeddings.weight")[t], W("embeddings.norm.weight"), None, eps)
     st = _Pair(x0)
     out = []
     for li in range(num_layers):

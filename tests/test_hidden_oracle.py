@@ -15,8 +15,16 @@
       trained-like family at every geometry: > 10x at H 768, 384, 1024 / I 4096 and on the plain family at H 1024 / I 2624,
       and 4x - 9x at the other geometries, where one block of 3 or 6 moves rstd by less.  The factors are printed; > 4x at
       every geometry and > 10x at H 768 are asserted.
+* Long context (tests/test_encoder_long_context_gpu.py): the chunked float64 forward modernbert_hidden64_long equals the
+  dense one to float64 roundoff at S 1 - 1100 with chunks that divide no S and windows wider and narrower than a chunk,
+  batched = per sequence; at 4096 tokens the restatement keeps the margin >= 2 on every family at H 768 and 384; each wrong
+  engine of hidden_oracle.FAR_POSITION_MUTATIONS (the rope row of a position past 2048 read at fp16(position) or at
+  position % 2048) leaves the production bound by > 10x on the rows at positions >= 2048 (wide family, H 768, 4096
+  tokens), with the unmutated restatement inside it: the GPU test of long sequences can see an error confined to far
+  positions.
 Run with -s for the margins."""
 import functools
+from dataclasses import replace
 
 import numpy as np
 import pytest
@@ -169,3 +177,68 @@ def test_wrong_engine_leaves_the_bound(mut):
 
 def test_every_mutation_has_a_case():
     assert set(ho.MUTATIONS) == set(MUTATION_LAYER) | {"global_every", "rope_tables", "window", "stats_block"}
+
+
+# --------------------------------------------------------------------------------------
+# long context: the chunked float64 forward the GPU test of long sequences and large batches uses
+# --------------------------------------------------------------------------------------
+# H 384, global layers 0 and 3, window 32 (local_attention 64), the local theta above the global one
+LONG_CHECK_CFG = dict(local_attention=64, local_rope_theta=50000.0, global_rope_theta=7000.0, max_position_embeddings=2048)
+
+
+@pytest.mark.parametrize("S", [1, 63, 64, 65, 300, 1100])
+def test_long_form_equals_dense(S):
+    """modernbert_hidden64_long = modernbert_hidden64 to float64 roundoff, rows and scale sums, with query chunks of 23 (under
+    the window of 32) and 97 (over it) that divide no S; the [3, S] call = three [1, S] calls"""
+    cfg = replace(ho.modernbert_config("small-384", 4), **LONG_CHECK_CFG)
+    w = ho.to64(ho.modernbert_weights(cfg, "wide"))
+    seqs = np.stack(_seqs(cfg, [S] * 3, seed=S))
+    dense = [ho.modernbert_hidden64(w, cfg, s, 4) for s in seqs]
+    worst = 0.0
+    for q_chunk in (23, 97):
+        batched = ho.modernbert_hidden64_long(w, cfg, seqs, [1, 2, 3, 4], q_chunk=q_chunk)
+        for i, (ref, got) in enumerate(zip(dense, batched)):
+            alone = ho.modernbert_hidden64_long(w, cfg, seqs[i:i + 1], [1, 2, 3, 4], q_chunk=q_chunk)[0]
+            for d in range(1, 5):
+                scale = ho.centred_rms(ref[d - 1])[:, None]
+                sums = sum(ho.centred_rms(ref[j]) for j in range(d))
+                worst = max(worst, float(((got.rows[d] - ref[d - 1]).abs() / scale).max()),
+                            float(((got.scale_sums[d] - sums).abs() / sums).max()),
+                            float(((alone.rows[d] - got.rows[d]).abs() / scale).max()))
+    print(f"long form vs dense forward, S {S}: largest difference / row scale {worst:.1e}")
+    assert worst <= 1e-12
+
+
+@functools.lru_cache(maxsize=1)
+def _long_model(geo, family, S=4096):
+    cfg = replace(ho.modernbert_config(geo, 4), max_position_embeddings=S)
+    w = ho.to64(ho.modernbert_weights(cfg, family))
+    ids = _seqs(cfg, [S], seed=5)[0]
+    return cfg, w, ids, ho.modernbert_hidden64_long(w, cfg, ids[None], [1, 2, 3, 4])[0]
+
+
+def _long_worst(model, rows=slice(None), **mut):
+    cfg, w, ids, ref = model
+    got = ho.modernbert_restated(w, cfg, ids, 4, **mut)
+    return [ho.worst_over_bound(got[d - 1], ref, d, rows=rows) for d in range(1, 5)]
+
+
+@pytest.mark.parametrize("family", ho.FAMILIES)
+@pytest.mark.parametrize("geo", ["base-768", "small-384"])
+def test_restatement_inside_production_bound_at_4096(geo, family):
+    """Global layers over 4096 keys, local windows at positions up to 4095: the restated engine keeps the margin of 2"""
+    worst = _long_worst(_long_model(geo, family))
+    print(f"restatement {geo} {family} at 4096 tokens: worst error / bound per depth " + " ".join(f"{v:.3f}" for v in worst) +
+          f"  margin {1 / max(worst):.1f}x")
+    assert max(worst) <= 0.5
+
+
+@pytest.mark.parametrize("mut", ho.FAR_POSITION_MUTATIONS)
+def test_far_position_mutations_leave_the_bound(mut):
+    """Rope rows read at fp16(position) or at position % 2048 (wide family, base-768, 4096 tokens), over the rows at
+    positions >= 2048 they touch"""
+    model = _long_model("base-768", "wide")
+    ok = max(_long_worst(model))
+    bad = max(_long_worst(model, rows=slice(2048, None), mut=mut))
+    print(f"mutation {mut} (base-768 wide, 4096 tokens): {bad:.1f}x the production bound on rows >= 2048 (unmutated: {ok:.2f}x)")
+    assert ok <= 0.5 and bad > 10.0
