@@ -34,7 +34,10 @@ SR_API const char* sr_last_error(void);
 SR_API int sr_device_count(void);
 
 /* Load <dir>/config.json + <dir>/model.safetensors onto CUDA device `device`; a classifier found in the
- * checkpoint becomes head 0.  Replaces init_* of the reference (candle-binding/src/ffi/init.rs:154-877). */
+ * checkpoint becomes head 0.  Replaces init_* of the reference (candle-binding/src/ffi/init.rs:154-877).
+ * The directory is checked before the device: one that cannot be served is refused from its config.json and
+ * safetensors header alone, so on a host without a usable device its own error is reported, not the device's.  A
+ * servable directory still needs an sm_90 device ("no CUDA device available" without one). */
 SR_API int sr_model_load(const char* model_dir, int device, sr_model** out);
 /* Attach another head (head.*, classifier.*) from a second checkpoint sharing this encoder (BASELINE cfg 3).
  * token_level: 1 token classifier, 0 sequence classifier, -1 from config.json "architectures".  Returns head id. */

@@ -158,6 +158,16 @@ int finish(Model& m) {
   if (e != cudaSuccess) return fail(std::string("CUDA failure: ") + cudaGetErrorString(e));
   return 0;
 }
+
+// *out: the handle of the model a loader returned; m null: the loader's error after `what`
+int new_handle(const char* what, Model* m, const std::string& err, sr_model** out) {
+  if (!m) return fail(std::string(what) + ": " + err);
+  sr_model* h = new sr_model();
+  h->m = m;
+  h->private_stream = m->stream;
+  *out = h;
+  return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -174,12 +184,7 @@ int sr_model_load(const char* model_dir, int device, sr_model** out) {
   if (!model_dir || !out) return fail("bad arguments");
   std::string err;
   Model* m = model_load(model_dir, device, &err);
-  if (!m) return fail("sr_model_load(" + std::string(model_dir) + "): " + err);
-  sr_model* h = new sr_model();
-  h->m = m;
-  h->private_stream = m->stream;
-  *out = h;
-  return 0;
+  return new_handle("sr_model_load", m, err, out);
 }
 
 int sr_model_add_head(sr_model* h, const char* model_dir, int token_level) {
@@ -392,12 +397,7 @@ int load_grouped(const char* what, GroupedLoader load, const char* const* task_d
   }
   std::string err;
   Model* m = load(dirs, tl, device, &err);
-  if (!m) return fail(std::string(what) + ": " + err);
-  sr_model* h = new sr_model();
-  h->m = m;
-  h->private_stream = m->stream;
-  *out = h;
-  return 0;
+  return new_handle(what, m, err, out);
 }
 }  // namespace
 

@@ -116,6 +116,8 @@ struct SafeTensors {
   void* map = nullptr;
   size_t size = 0;
   std::map<std::string, StTensor> tensors;
+  SafeTensors() = default;
+  SafeTensors(const SafeTensors&) = delete;   // owns the mapping
   ~SafeTensors() {
     if (map) munmap(map, size);
     if (fd >= 0) close(fd);
@@ -131,10 +133,10 @@ struct SafeTensors {
     const uint8_t* base = static_cast<const uint8_t*>(map);
     uint64_t hlen;
     memcpy(&hlen, base, 8);
-    if (hlen > size - 8) { *err = "safetensors header exceeds file"; return false; }
+    if (hlen > size - 8) { *err = path + ": safetensors header exceeds file"; return false; }
     Json hdr;
     JsonParser jp(reinterpret_cast<const char*>(base + 8), hlen);
-    if (!jp.parse(hdr) || !hdr.is_obj()) { *err = "safetensors header is not JSON"; return false; }
+    if (!jp.parse(hdr) || !hdr.is_obj()) { *err = path + ": safetensors header is not JSON"; return false; }
     const uint8_t* data0 = base + 8 + hlen;
     for (const auto& kv : hdr.obj) {
       if (kv.first == "__metadata__") continue;
@@ -147,9 +149,9 @@ struct SafeTensors {
       for (const auto& d : sh->arr) t.shape.push_back(static_cast<int64_t>(d.num));
       const double bd = off->arr[0].num, ed = off->arr[1].num;
       const size_t room = size - 8 - static_cast<size_t>(hlen);
-      if (!(bd >= 0.0) || !(ed >= bd) || ed > static_cast<double>(room)) { *err = "tensor " + kv.first + " out of bounds"; return false; }
+      if (!(bd >= 0.0) || !(ed >= bd) || ed > static_cast<double>(room)) { *err = path + ": tensor " + kv.first + " out of bounds"; return false; }
       const size_t b = static_cast<size_t>(bd), e = static_cast<size_t>(ed);
-      if (e > room || e < b) { *err = "tensor " + kv.first + " out of bounds"; return false; }
+      if (e > room || e < b) { *err = path + ": tensor " + kv.first + " out of bounds"; return false; }
       t.data = data0 + b;
       t.bytes = e - b;
       tensors.emplace(kv.first, std::move(t));
@@ -292,11 +294,6 @@ struct Loader {
     if (!host_f32(name, v, shape, required)) return nullptr;
     return up_f32(v);
   }
-  __half* f16(const std::string& name, const std::vector<int64_t>& shape) {
-    std::vector<float> v;
-    if (!host_f32(name, v, shape)) return nullptr;
-    return up_f16(v);
-  }
 };
 
 void parse_id2label(const Json& cfg, std::map<int, std::string>& out) {
@@ -386,7 +383,7 @@ bool read_encoder_config(const Json& cfgj, const SafeTensors& st, EncoderConfig&
   return true;
 }
 
-// model_load's device requirements: an sm_90 device at index `device`, made current
+// The load's device step: an sm_90 device at index `device`, made current
 bool use_device(int device, std::string* err) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -553,15 +550,6 @@ void store_projection(Loader& ld, const Projection& pr, int p, const std::vector
   if (pr.bias) *biases[p] = ld.up_f32(b);
 }
 
-// The ordinary model: the four projections of one layer (and BERT's biases) from the loader's checkpoint
-void load_projections(Loader& ld, const std::array<Projection, 4>& pr, LayerWeights& lw) {
-  for (int p = 0; p < 4 && ld.ok; ++p) {
-    std::vector<float> w, b;
-    if (!device_weight(ld, pr[p], w, pr[p].bias ? &b : nullptr)) return;
-    store_projection(ld, pr[p], p, w, b, lw);
-  }
-}
-
 // ModernBERT's rotary tables for both thetas, max_position_embeddings rows
 void load_rope(Loader& ld, Model& m) {
   const EncoderConfig& c = m.cfg;
@@ -611,103 +599,6 @@ bool load_head(Loader& ld, const Json& cfgj, Arch arch, int H, const std::string
   return ld.ok;
 }
 
-}  // namespace
-
-// ------------------------------------------------------------------------------------------------
-// model load
-// ------------------------------------------------------------------------------------------------
-Model* model_load(const std::string& dir, int device, std::string* err) {
-  std::string e;
-  if (!use_device(device, err)) return nullptr;
-
-  Json cfgj;
-  if (!parse_json_file(dir + "/config.json", cfgj)) { *err = "cannot read " + dir + "/config.json"; return nullptr; }
-  SafeTensors st;
-  if (!st.open(dir + "/model.safetensors", &e)) { *err = e; return nullptr; }
-
-  Model* m = new Model();
-  m->device = device;
-  m->dir = dir;
-  Loader ld{m, &st};
-  ld.lora_alpha = lora_alpha_of(dir);
-  EncoderConfig& c = m->cfg;
-  std::string P;  // tensor-name prefix
-  if (!read_encoder_config(cfgj, st, c, P, &e)) ld.fail(e);
-
-  const int H = c.H;
-  if (ld.ok && c.arch == ARCH_MODERNBERT) {
-    m->emb_word = ld.f32(P + "embeddings.tok_embeddings.weight", {c.vocab, H});
-    m->emb_ln_w = ld.f32(P + "embeddings.norm.weight", {H});
-    m->layers.resize(c.L);
-    for (int li = 0; li < c.L && ld.ok; ++li) {
-      const std::string Lp = layer_prefix(c, P, li);
-      LayerWeights& lw = m->layers[li];
-      if (st.find(Lp + "attn_norm.weight")) lw.attn_norm_w = ld.f32(Lp + "attn_norm.weight", {H});
-      lw.mid_norm_w = ld.f32(Lp + "mlp_norm.weight", {H});
-      load_projections(ld, layer_projections(c, P, li, lw.attn_norm_w != nullptr), lw);
-    }
-    m->final_norm_w = ld.f32(P + "final_norm.weight", {H});
-    if (ld.ok) load_rope(ld, *m);
-  } else if (ld.ok) {
-    const std::string E = P + "embeddings.";
-    m->emb_word = ld.f32(E + "word_embeddings.weight", {c.vocab, H});
-    m->emb_pos = ld.f32(E + "position_embeddings.weight", {c.max_pos, H});
-    std::vector<float> tt;
-    if (ld.host_f32(E + "token_type_embeddings.weight", tt, {c.type_vocab, H})) {
-      tt.resize(H);  // token_type_ids are always zero (traditional/bert.rs:227)
-      m->emb_type0 = ld.up_f32(tt);
-    }
-    m->emb_ln_w = ld.f32(E + "LayerNorm.weight", {H});
-    m->emb_ln_b = ld.f32(E + "LayerNorm.bias", {H});
-    m->layers.resize(c.L);
-    for (int li = 0; li < c.L && ld.ok; ++li) {
-      const std::string Lp = layer_prefix(c, P, li);
-      LayerWeights& lw = m->layers[li];
-      load_projections(ld, layer_projections(c, P, li, false), lw);
-      lw.mid_norm_w = ld.f32(Lp + "attention.output.LayerNorm.weight", {H});
-      lw.mid_norm_b = ld.f32(Lp + "attention.output.LayerNorm.bias", {H});
-      lw.out_norm_w = ld.f32(Lp + "output.LayerNorm.weight", {H});
-      lw.out_norm_b = ld.f32(Lp + "output.LayerNorm.bias", {H});
-    }
-  }
-  if (ld.ok && st.find("classifier.weight")) {
-    Head hd;
-    if (load_head(ld, cfgj, c.arch, H, P, -1, hd)) m->heads.push_back(hd);
-  }
-  if (ld.ok && cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess) ld.fail("stream create failed");
-  if (!ld.ok) {
-    *err = ld.err;
-    model_free(m);
-    return nullptr;
-  }
-  cudaDeviceSynchronize();
-  return m;
-}
-
-int model_add_head(Model* m, const std::string& dir, int force_token_level, std::string* err) {
-  if (cudaSetDevice(m->device) != cudaSuccess) { *err = "cudaSetDevice failed"; return -1; }
-  Json cfgj;
-  if (!parse_json_file(dir + "/config.json", cfgj)) { *err = "cannot read " + dir + "/config.json"; return -1; }
-  SafeTensors st;
-  std::string e;
-  if (!st.open(dir + "/model.safetensors", &e)) { *err = e; return -1; }
-  Loader ld{m, &st};
-  Head hd;
-  std::string bp;
-  tensor_prefix(st, m->cfg.arch, bp);   // a head-only checkpoint has no embeddings: its pooler names the prefix
-  if (!load_head(ld, cfgj, m->cfg.arch, m->cfg.H, bp, force_token_level, hd) || !ld.ok) {
-    *err = ld.ok ? "no classifier.weight in " + dir : ld.err;
-    return -1;
-  }
-  m->heads.push_back(hd);
-  return static_cast<int>(m->heads.size()) - 1;
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// grouped model: several task checkpoints of one encoder in one pass (engine.h: Grouped)
-// ------------------------------------------------------------------------------------------------
-namespace {
 bool is_head_tensor(const std::string& n) {
   return n.compare(0, 11, "classifier.") == 0 || n.compare(0, 5, "head.") == 0 || n.find("pooler.") != std::string::npos;
 }
@@ -768,63 +659,61 @@ std::vector<float*> load_each(std::vector<Loader>& lt, const std::vector<std::st
   }
   return out;
 }
-}  // namespace
 
-Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
-                          std::string* err) {
-  const int T = static_cast<int>(dirs.size());
-  if (T < 1 || T > kMaxRowGroups) { *err = "a grouped model takes 1 to " + std::to_string(kMaxRowGroups) + " task checkpoints"; return nullptr; }
-  if (token_level.size() != dirs.size()) { *err = "one token_level per task checkpoint"; return nullptr; }
-  // every refusal of the directories first, on the host
-  std::vector<Json> cfgj(T);
-  std::vector<std::unique_ptr<SafeTensors>> sts;
-  std::vector<EncoderConfig> cfg(T);
-  std::vector<std::string> P(T);
-  for (int t = 0; t < T; ++t) {
-    const std::string& d = dirs[t];
-    if (!parse_json_file(d + "/config.json", cfgj[t])) { *err = "cannot read " + d + "/config.json"; return nullptr; }
-    sts.emplace_back(new SafeTensors());
-    std::string e;
-    if (!sts.back()->open(d + "/model.safetensors", &e)) { *err = e; return nullptr; }
-    if (!read_encoder_config(cfgj[t], *sts[t], cfg[t], P[t], &e)) { *err = d + ": " + e; return nullptr; }
-    if (cfg[t].attn_w != cfg[t].H) { *err = d + ": grouped serving is not available for padded-head (MiniLM) encoders"; return nullptr; }
-    const auto f0 = shape_fields(cfg[0]), ft = shape_fields(cfg[t]);
-    for (size_t i = 0; i < f0.size(); ++i)
-      if (f0[i].second != ft[i].second) {
-        *err = std::string("the checkpoints do not share one encoder shape: ") + f0[i].first + " is " + ft[i].second + " in " + d +
-               " and " + f0[i].second + " in " + dirs[0];
-        return nullptr;
-      }
-    if (!sts[t]->find("classifier.weight")) { *err = "no classifier.weight in " + d; return nullptr; }
-  }
-  if (!use_device(device, err)) return nullptr;
+// One checkpoint directory as the host reads it: config.json, the mapped safetensors file, the encoder shape and the
+// tensor-name prefix
+struct Checkpoint {
+  std::string dir;
+  Json cfgj;
+  SafeTensors st;
+  EncoderConfig cfg;
+  std::string P;
+};
 
+// The load's host step.  false: *err names the directory and says why it cannot be served.
+bool read_checkpoint(const std::string& dir, Checkpoint& ck, std::string* err) {
+  ck.dir = dir;
+  if (!parse_json_file(dir + "/config.json", ck.cfgj)) { *err = "cannot read " + dir + "/config.json"; return false; }
+  if (!ck.st.open(dir + "/model.safetensors", err)) return false;
+  if (read_encoder_config(ck.cfgj, ck.st, ck.cfg, ck.P, err)) return true;
+  *err = dir + ": " + *err;
+  return false;
+}
+
+// false: *err is the error of the first task whose upload failed, after its directory
+bool tasks_ok(const std::vector<Checkpoint>& ck, const std::vector<Loader>& lt, std::string* err) {
+  for (size_t t = 0; t < lt.size(); ++t)
+    if (!lt[t].ok) { *err = ck[t].dir + ": " + lt[t].err; return false; }
+  return true;
+}
+
+// The load's upload step, on the current device: a model of the tasks `ck` (host-read, one encoder shape) holding every
+// task's embeddings and norms (Model::task; a tensor bitwise equal in every task once), the rotary tables, and every
+// layer's projections -- each task's device weights (its own gamma folded in) and biases, stacked along N.  lt: one
+// loader per task, left to the caller's heads.  null: *err says why.
+Model* upload_tasks(const std::vector<Checkpoint>& ck, int device, std::vector<Loader>& lt, std::string* err) {
+  const int T = static_cast<int>(ck.size());
   Model* m = new Model();
   m->device = device;
-  m->dir = dirs[0];
-  m->cfg = cfg[0];
+  m->dir = ck[0].dir;
+  m->cfg = ck[0].cfg;
   const EncoderConfig& c = m->cfg;
   const int H = c.H;
-  std::vector<Loader> lt;
-  for (int t = 0; t < T; ++t) {
-    lt.push_back(Loader{m, sts[t].get()});
-    lt.back().lora_alpha = lora_alpha_of(dirs[t]);   // adapters are merged as model_load merges them
+  for (const Checkpoint& k : ck) {
+    lt.push_back(Loader{m, &k.st});
+    lt.back().lora_alpha = lora_alpha_of(k.dir);
   }
-  auto ok = [&]() {
-    for (const Loader& l : lt)
-      if (!l.ok) { *err = l.err; return false; }
-    return true;
-  };
+  auto ok = [&]() { return tasks_ok(ck, lt, err); };
   auto names = [&](const std::string& rest, int li = -1) {   // `rest` under every task's prefix (and layer li)
     std::vector<std::string> n(T);
-    for (int t = 0; t < T; ++t) n[t] = (li < 0 ? P[t] : layer_prefix(c, P[t], li)) + rest;
+    for (int t = 0; t < T; ++t) n[t] = (li < 0 ? ck[t].P : layer_prefix(c, ck[t].P, li)) + rest;
     return n;
   };
-  Grouped& g = m->group;
-  g.task.resize(T);
-  for (TaskTensors& tt : g.task) tt.layers.resize(c.L);
-  auto each = [&](std::vector<float*> v, float* TaskTensors::*f) { for (int t = 0; t < T; ++t) g.task[t].*f = v[t]; };
-  auto each_layer = [&](std::vector<float*> v, int li, float* TaskNorms::*f) { for (int t = 0; t < T; ++t) g.task[t].layers[li].*f = v[t]; };
+  std::vector<TaskTensors>& task = m->task;
+  task.resize(T);
+  for (TaskTensors& tt : task) tt.layers.resize(c.L);
+  auto each = [&](std::vector<float*> v, float* TaskTensors::*f) { for (int t = 0; t < T; ++t) task[t].*f = v[t]; };
+  auto each_layer = [&](std::vector<float*> v, int li, float* TaskNorms::*f) { for (int t = 0; t < T; ++t) task[t].layers[li].*f = v[t]; };
   if (c.arch == ARCH_MODERNBERT) {
     each(load_each(lt, names("embeddings.tok_embeddings.weight"), {c.vocab, H}), &TaskTensors::emb_word);
     each(load_each(lt, names("embeddings.norm.weight"), {H}), &TaskTensors::emb_ln_w);
@@ -832,9 +721,9 @@ Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vecto
       each_layer(load_each(lt, names("attn_norm.weight", li), {H}, false), li, &TaskNorms::attn_w);
       each_layer(load_each(lt, names("mlp_norm.weight", li), {H}), li, &TaskNorms::mid_w);
       for (int t = 1; t < T && ok(); ++t)
-        if ((g.task[t].layers[li].attn_w != nullptr) != (g.task[0].layers[li].attn_w != nullptr)) {
-          *err = "layer " + std::to_string(li) + " has an attn_norm in " + dirs[g.task[0].layers[li].attn_w ? 0 : t] +
-                 " but not in " + dirs[g.task[0].layers[li].attn_w ? t : 0];
+        if ((task[t].layers[li].attn_w != nullptr) != (task[0].layers[li].attn_w != nullptr)) {
+          *err = "layer " + std::to_string(li) + " has an attn_norm in " + ck[task[0].layers[li].attn_w ? 0 : t].dir +
+                 " but not in " + ck[task[0].layers[li].attn_w ? t : 0].dir;
           model_free(m);
           return nullptr;
         }
@@ -855,11 +744,10 @@ Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vecto
       each_layer(load_each(lt, names("output.LayerNorm.bias", li), {H}), li, &TaskNorms::out_b);
     }
   }
-  // projections: every task's device weights (its own gamma folded in) and biases, stacked along N
   m->layers.resize(c.L);
   for (int li = 0; li < c.L && ok(); ++li) {
     std::vector<std::array<Projection, 4>> pr;
-    for (int t = 0; t < T; ++t) pr.push_back(layer_projections(c, P[t], li, g.task[t].layers[li].attn_w != nullptr));
+    for (int t = 0; t < T; ++t) pr.push_back(layer_projections(c, ck[t].P, li, task[t].layers[li].attn_w != nullptr));
     for (int p = 0; p < 4 && ok(); ++p) {
       std::vector<float> stack, bstack, w, b;
       for (int t = 0; t < T && ok(); ++t) {
@@ -870,30 +758,97 @@ Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vecto
       if (ok()) store_projection(lt[0], pr[0][p], p, stack, bstack, m->layers[li]);
     }
   }
-  for (int t = 0; t < T && ok(); ++t) {
-    Head hd;
-    if (!load_head(lt[t], cfgj[t], c.arch, H, P[t], token_level[t], hd)) {
-      if (lt[t].ok) lt[t].fail("classifier.weight of " + dirs[t] + " does not fit hidden_size");
-      break;
-    }
-    hd.final_norm_w = g.task[t].final_norm_w;
-    m->heads.push_back(hd);
-    g.head_of_task.push_back(t);
-  }
-  if (ok() && cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess) lt[0].fail("stream create failed");
   if (!ok()) { model_free(m); return nullptr; }
-  // outside a grouped pass the model is task 0: its tensors, and the first matrix / bias of every stack
-  const TaskTensors& t0 = g.task[0];
-  m->emb_word = t0.emb_word; m->emb_pos = t0.emb_pos; m->emb_type0 = t0.emb_type0;
-  m->emb_ln_w = t0.emb_ln_w; m->emb_ln_b = t0.emb_ln_b; m->final_norm_w = t0.final_norm_w;
-  for (int li = 0; li < c.L; ++li) {
-    LayerWeights& lw = m->layers[li];
-    const TaskNorms& n = t0.layers[li];
-    lw.attn_norm_w = n.attn_w; lw.mid_norm_w = n.mid_w; lw.mid_norm_b = n.mid_b; lw.out_norm_w = n.out_w; lw.out_norm_b = n.out_b;
+  return m;
+}
+
+// The load's last step, after the caller's heads: the model with its stream, or null and *err (the model freed)
+Model* finish_load(Model* m, const std::vector<Checkpoint>& ck, const std::vector<Loader>& lt, std::string* err) {
+  if (!tasks_ok(ck, lt, err)) { model_free(m); return nullptr; }
+  if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess) {
+    *err = "stream create failed";
+    model_free(m);
+    return nullptr;
   }
-  g.tasks = T;
   cudaDeviceSynchronize();
   return m;
+}
+}  // namespace
+
+// ------------------------------------------------------------------------------------------------
+// model load: one checkpoint is a grouped model of one task (engine.h: Grouped).  Both entries read every directory on
+// the host (read_checkpoint), then take the device (use_device), upload (upload_tasks) and add their heads.
+// ------------------------------------------------------------------------------------------------
+Model* model_load(const std::string& dir, int device, std::string* err) {
+  std::vector<Checkpoint> ck(1);
+  if (!read_checkpoint(dir, ck[0], err) || !use_device(device, err)) return nullptr;
+  std::vector<Loader> lt;
+  Model* m = upload_tasks(ck, device, lt, err);
+  if (!m) return nullptr;
+  Head hd;   // none when the checkpoint has no classifier.weight or one that does not fit hidden_size
+  if (load_head(lt[0], ck[0].cfgj, m->cfg.arch, m->cfg.H, ck[0].P, -1, hd)) {
+    hd.final_norm_w = m->task[0].final_norm_w;
+    m->heads.push_back(hd);
+  }
+  return finish_load(m, ck, lt, err);
+}
+
+Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
+                          std::string* err) {
+  const int T = static_cast<int>(dirs.size());
+  if (T < 1 || T > kMaxRowGroups) { *err = "a grouped model takes 1 to " + std::to_string(kMaxRowGroups) + " task checkpoints"; return nullptr; }
+  if (token_level.size() != dirs.size()) { *err = "one token_level per task checkpoint"; return nullptr; }
+  // every refusal of the directories first, on the host
+  std::vector<Checkpoint> ck(T);
+  for (int t = 0; t < T; ++t) {
+    const std::string& d = dirs[t];
+    if (!read_checkpoint(d, ck[t], err)) return nullptr;
+    if (ck[t].cfg.attn_w != ck[t].cfg.H) { *err = d + ": grouped serving is not available for padded-head (MiniLM) encoders"; return nullptr; }
+    const auto f0 = shape_fields(ck[0].cfg), ft = shape_fields(ck[t].cfg);
+    for (size_t i = 0; i < f0.size(); ++i)
+      if (f0[i].second != ft[i].second) {
+        *err = std::string("the checkpoints do not share one encoder shape: ") + f0[i].first + " is " + ft[i].second + " in " + d +
+               " and " + f0[i].second + " in " + dirs[0];
+        return nullptr;
+      }
+    if (!ck[t].st.find("classifier.weight")) { *err = "no classifier.weight in " + d; return nullptr; }
+  }
+  if (!use_device(device, err)) return nullptr;
+  std::vector<Loader> lt;
+  Model* m = upload_tasks(ck, device, lt, err);
+  if (!m) return nullptr;
+  for (int t = 0; t < T; ++t) {
+    Head hd;
+    if (!load_head(lt[t], ck[t].cfgj, m->cfg.arch, m->cfg.H, ck[t].P, token_level[t], hd)) {
+      if (lt[t].ok) lt[t].fail("classifier.weight does not fit hidden_size");
+      break;
+    }
+    hd.final_norm_w = m->task[t].final_norm_w;
+    m->heads.push_back(hd);
+    m->group.head_of_task.push_back(t);
+  }
+  m->group.tasks = T;
+  return finish_load(m, ck, lt, err);
+}
+
+int model_add_head(Model* m, const std::string& dir, int force_token_level, std::string* err) {
+  if (cudaSetDevice(m->device) != cudaSuccess) { *err = "cudaSetDevice failed"; return -1; }
+  Json cfgj;
+  if (!parse_json_file(dir + "/config.json", cfgj)) { *err = "cannot read " + dir + "/config.json"; return -1; }
+  SafeTensors st;
+  std::string e;
+  if (!st.open(dir + "/model.safetensors", &e)) { *err = e; return -1; }
+  Loader ld{m, &st};
+  Head hd;
+  std::string bp;
+  tensor_prefix(st, m->cfg.arch, bp);   // a head-only checkpoint has no embeddings: its pooler names the prefix
+  if (!load_head(ld, cfgj, m->cfg.arch, m->cfg.H, bp, force_token_level, hd) || !ld.ok) {
+    *err = ld.ok ? "no classifier.weight in " + dir : ld.err;
+    return -1;
+  }
+  hd.final_norm_w = m->task[0].final_norm_w;
+  m->heads.push_back(hd);
+  return static_cast<int>(m->heads.size()) - 1;
 }
 
 Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
@@ -949,7 +904,7 @@ bool read_source_projections(Model& m, std::string* err,
   tensor_prefix(st, m.cfg.arch, P);
   std::vector<float> w;
   for (int li = 0; li < m.cfg.L; ++li) {
-    const auto pr = layer_projections(m.cfg, P, li, m.layers[li].attn_norm_w != nullptr);
+    const auto pr = layer_projections(m.cfg, P, li, m.task[0].layers[li].attn_w != nullptr);
     for (int p = 0; p < 4; ++p) {
       if (!read_projection(ld, pr[p], w, nullptr)) { *err = ld.err; return false; }
       if (!fn(li, p, w, pr[p].N, pr[p].K)) return false;
@@ -1092,15 +1047,16 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
     if (grouped) { gd.w_groups = gp.tasks; gd.w_group_rows = gp.rows_per_task; gd.bias_per_group = true; }
     return gemm_f16(s, gd);
   };
-  // a task tensor per row group; outside a grouped pass the model's own (task 0's)
-  auto per_task = [&](float* TaskTensors::*f, const float* own) {
-    RowGroups r = RowGroups::one(own);
-    for (int t = 0; grouped && t < gp.tasks; ++t) r.p[t] = gp.task[t].*f;
+  // a task tensor per row group; outside a grouped pass task 0's
+  const int row_groups = grouped ? gp.tasks : 1;
+  auto per_task = [&](float* TaskTensors::*f) {
+    RowGroups r;
+    for (int t = 0; t < row_groups; ++t) r.p[t] = m.task[t].*f;
     return r;
   };
-  auto per_task_norm = [&](int li, float* TaskNorms::*f, const float* own) {
-    RowGroups r = RowGroups::one(own);
-    for (int t = 0; grouped && t < gp.tasks; ++t) r.p[t] = gp.task[t].layers[li].*f;
+  auto per_task_norm = [&](int li, float* TaskNorms::*f) {
+    RowGroups r;
+    for (int t = 0; t < row_groups; ++t) r.p[t] = m.task[t].layers[li].*f;
     return r;
   };
   if (c.arch == ARCH_MODERNBERT) {
@@ -1109,10 +1065,10 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
     // GEMM also leaves the per-row (sum, sum of squares) of x - pivot in w.row_stats; the projection that consumes
     // LN(x) multiplies the raw rows w.h with W diag(gamma) and corrects per row in its epilogue -- no LayerNorm pass.
     // Layer 0's attn_norm (when the checkpoint has one) is the exception: it runs on the fp32 embedding output.
-    const bool ln0 = m.layers[0].attn_norm_w != nullptr;
+    const bool ln0 = m.task[0].layers[0].attn_w != nullptr;
     { ProfScope ps(m, PC_EMBED);
-      if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, per_task(&TaskTensors::emb_word, m.emb_word),
-                              per_task(&TaskTensors::emb_ln_w, m.emb_ln_w), group_rows, c.ln_eps, ln0 ? w.x : nullptr, w.h, w.lo))
+      if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, per_task(&TaskTensors::emb_word),
+                              per_task(&TaskTensors::emb_ln_w), group_rows, c.ln_eps, ln0 ? w.x : nullptr, w.h, w.lo))
         return -1; }
     // one statistics record [H/128][T][2] partials + [T] pivots, padded so that the second record keeps the float2
     // alignment of the partials; the residual GEMMs ping-pong between the two
@@ -1135,7 +1091,7 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
     for (int li = 0; li < L; ++li) {
       const LayerWeights& lw = m.layers[li];
       const bool local = (li % c.global_every) != 0;
-      const bool folded = lw.wqkv_f != nullptr;   // model_load: li > 0 with attn_norm
+      const bool folded = lw.wqkv_f != nullptr;   // layer_projections: li > 0 with attn_norm
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = 3 * H; g.K = H; g.A = w.h; g.W = lw.wqkv; g.out = w.qkv; g.ldo = 3 * H;
       if (folded) {
@@ -1145,7 +1101,7 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
         // this layer's attention has not written it yet)
         ProfScope ps(m, PC_NORM);
         if (li == 0) {
-          if (layernorm_rows(s, w.x, T, H, per_task_norm(0, &TaskNorms::attn_w, lw.attn_norm_w), RowGroups::one(nullptr),
+          if (layernorm_rows(s, w.x, T, H, per_task_norm(0, &TaskNorms::attn_w), RowGroups::one(nullptr),
                              group_rows, c.ln_eps, nullptr, w.ctx))
             return -1;
         } else {
@@ -1180,9 +1136,9 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
     }
   } else {
     ProfScope ps_embed(m, PC_EMBED);
-    if (embed_ln_bert(s, d_ids, w.pos, T, H, c.vocab, c.max_pos, per_task(&TaskTensors::emb_word, m.emb_word),
-                      per_task(&TaskTensors::emb_pos, m.emb_pos), per_task(&TaskTensors::emb_type0, m.emb_type0),
-                      per_task(&TaskTensors::emb_ln_w, m.emb_ln_w), per_task(&TaskTensors::emb_ln_b, m.emb_ln_b), group_rows,
+    if (embed_ln_bert(s, d_ids, w.pos, T, H, c.vocab, c.max_pos, per_task(&TaskTensors::emb_word),
+                      per_task(&TaskTensors::emb_pos), per_task(&TaskTensors::emb_type0),
+                      per_task(&TaskTensors::emb_ln_w), per_task(&TaskTensors::emb_ln_b), group_rows,
                       c.ln_eps, w.x, w.h))
       return -1;
     for (int li = 0; li < L; ++li) {
@@ -1198,8 +1154,8 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       g.epi = EPI_RESID; g.resid = w.x; g.ldr = H; g.bias = lw.bo;
       { ProfScope ps(m, PC_GEMM_WO); if (run_proj(g)) return -1; }
       { ProfScope ps(m, PC_NORM);
-        if (layernorm_rows(s, w.x, T, H, per_task_norm(li, &TaskNorms::mid_w, lw.mid_norm_w),
-                           per_task_norm(li, &TaskNorms::mid_b, lw.mid_norm_b), group_rows, c.ln_eps, w.x, w.h))
+        if (layernorm_rows(s, w.x, T, H, per_task_norm(li, &TaskNorms::mid_w),
+                           per_task_norm(li, &TaskNorms::mid_b), group_rows, c.ln_eps, w.x, w.h))
           return -1; }
       g = GemmDesc();
       g.M = T; g.a_rows = w.cap_tokens; g.N = I; g.K = H; g.A = w.h; g.W = lw.wi; g.out = w.mid; g.ldo = I;
@@ -1210,8 +1166,8 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
       g.epi = EPI_RESID; g.resid = w.x; g.ldr = H; g.bias = lw.bo2;
       { ProfScope ps(m, PC_GEMM_WO2); if (run_proj(g)) return -1; }
       { ProfScope ps(m, PC_NORM);
-        if (layernorm_rows(s, w.x, T, H, per_task_norm(li, &TaskNorms::out_w, lw.out_norm_w),
-                           per_task_norm(li, &TaskNorms::out_b, lw.out_norm_b), group_rows, c.ln_eps, w.x, w.h))
+        if (layernorm_rows(s, w.x, T, H, per_task_norm(li, &TaskNorms::out_w),
+                           per_task_norm(li, &TaskNorms::out_b), group_rows, c.ln_eps, w.x, w.h))
           return -1; }
     }
   }
@@ -1224,13 +1180,12 @@ int head_sequence(Model& m, int head, const int* d_cu, int B, int pooler_mode) {
   const EncoderConfig& c = m.cfg;
   Workspace& w = m.ws;
   if (static_cast<size_t>(B) * hd.num_classes > w.out_elems) return -1;
-  const float* final_norm = hd.final_norm_w ? hd.final_norm_w : m.final_norm_w;
   SeqHeadWeights sw;
   sw.cls_w = hd.cls_w; sw.cls_b = hd.cls_b; sw.num_classes = hd.num_classes;
   if (c.arch == ARCH_MODERNBERT) {
     // always MEAN pooling over final_norm(hidden) (traditional/modernbert.rs:818,1146-1169)
     const bool hf = m.head_flavor == 1;
-    if (pool_rows(m.stream, w.x, d_cu, B, c.H, (hf && c.cls_pooling == 0) ? POOL_CLS : POOL_MEAN, final_norm, nullptr,
+    if (pool_rows(m.stream, w.x, d_cu, B, c.H, (hf && c.cls_pooling == 0) ? POOL_CLS : POOL_MEAN, hd.final_norm_w, nullptr,
                   c.ln_eps, w.pooled, w.pool_part, w.pool_arrived))
       return -1;
     sw.dense_mode = hd.has_dense ? 1 : 0;
@@ -1256,11 +1211,10 @@ int head_tokens(Model& m, int head, int B, int T, int row0) {
   if (static_cast<size_t>(T) * hd.num_classes > w.out_elems || row0 < 0 || row0 + T > w.cap_tokens) return -1;
   const size_t off = static_cast<size_t>(row0) * c.H;   // the head reads rows [row0, row0 + T) of the hidden states
   const float* x = w.x + off;
-  const float* final_norm = hd.final_norm_w ? hd.final_norm_w : m.final_norm_w;
   if (c.arch == ARCH_MODERNBERT) {
     if (hd.has_dense) {
       // final_norm -> fp16, head.dense on the wgmma GEMM, then gelu/LN/classifier per token
-      if (layernorm_rows(m.stream, x, T, c.H, final_norm, nullptr, c.ln_eps, nullptr, w.h + off)) return -1;
+      if (layernorm_rows(m.stream, x, T, c.H, hd.final_norm_w, nullptr, c.ln_eps, nullptr, w.h + off)) return -1;
       GemmDesc g;
       g.M = T; g.a_rows = w.cap_tokens - row0; g.N = c.H; g.K = c.H; g.A = w.h + off; g.W = hd.dense_w16; g.out = w.ctx + off; g.ldo = c.H;
       g.epi = EPI_F16;
@@ -1269,7 +1223,7 @@ int head_tokens(Model& m, int head, int B, int T, int row0) {
       return token_head(m.stream, nullptr, w.ctx + off, T, c.H, hd.norm_w, nullptr, 0.f, hd.cls_w, hd.cls_b, hd.num_classes,
                         hf ? 1 : 0, w.logits, w.probs, w.cls, w.conf, hf ? 1 : 0, hf ? c.ln_eps : 1e-12f);
     }
-    return token_head(m.stream, x, nullptr, T, c.H, nullptr, final_norm, c.ln_eps, hd.cls_w, hd.cls_b,
+    return token_head(m.stream, x, nullptr, T, c.H, nullptr, hd.final_norm_w, c.ln_eps, hd.cls_w, hd.cls_b,
                       hd.num_classes, 0, w.logits, w.probs, w.cls, w.conf);
   }
   return token_head(m.stream, x, nullptr, T, c.H, nullptr, nullptr, 0.f, hd.cls_w, hd.cls_b, hd.num_classes, 1,
@@ -1281,7 +1235,7 @@ int head_embedding(Model& m, const int* d_cu, int B, int dim, float norm_eps) {
   Workspace& w = m.ws;
   if (dim <= 0 || dim > c.H) dim = c.H;
   if (c.arch == ARCH_MODERNBERT) {
-    if (pool_rows(m.stream, w.x, d_cu, B, c.H, POOL_MEAN, m.final_norm_w, nullptr, c.ln_eps, w.pooled, w.pool_part, w.pool_arrived)) return -1;
+    if (pool_rows(m.stream, w.x, d_cu, B, c.H, POOL_MEAN, m.task[0].final_norm_w, nullptr, c.ln_eps, w.pooled, w.pool_part, w.pool_arrived)) return -1;
   } else {
     if (pool_rows(m.stream, w.x, d_cu, B, c.H, POOL_MEAN, nullptr, nullptr, 0.f, w.pooled, w.pool_part, w.pool_arrived, m.cur_kv_lens)) return -1;
   }

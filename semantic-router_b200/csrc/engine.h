@@ -36,20 +36,15 @@ struct EncoderConfig {
   std::map<int, std::string> id2label;
 };
 
-struct LayerWeights {
-  float* attn_norm_w = nullptr;  // ModernBERT pre-attention LN (null on layer 0)
+struct LayerWeights {     // one layer's projections (its norms are per task: TaskNorms)
   __half* wqkv = nullptr;        // [3H, H]
   float* bqkv = nullptr;         // BERT only
   __half* wo = nullptr;          // [H, H]
   float* bo = nullptr;
-  float* mid_norm_w = nullptr;   // ModernBERT mlp_norm / BERT attention.output.LayerNorm
-  float* mid_norm_b = nullptr;
   __half* wi = nullptr;          // ModernBERT [2I, H] (GeGLU-interleaved) / BERT [I, H]
   float* bi = nullptr;
   __half* wo2 = nullptr;         // [H, I]
   float* bo2 = nullptr;
-  float* out_norm_w = nullptr;   // BERT output.LayerNorm
-  float* out_norm_b = nullptr;
   // LayerNorm fold (pre-LN models, gemm.h): W diag(gamma) with zero-sum rows, fp16, for the two projections that
   // consume a LayerNorm output; null when the fold is off or the layer has no such norm
   __half* wqkv_f = nullptr;      // Wqkv diag(attn_norm), rows centred
@@ -66,7 +61,7 @@ struct Head {
   float* norm_w = nullptr;
   float* cls_w = nullptr;
   float* cls_b = nullptr;
-  float* final_norm_w = nullptr;   // ModernBERT: this head's task's final_norm (grouped models); null: the model's
+  float* final_norm_w = nullptr;   // ModernBERT: the final_norm of this head's task (Model::task)
   std::map<int, std::string> id2label;
 };
 
@@ -138,21 +133,24 @@ struct PreciseState {
 // Several task checkpoints of one encoder served in ONE pass (model_load_grouped): merged or fully fine-tuned
 // checkpoints, or unmerged LoRA adapters over one base (model_load_lora_shared).  The T tasks' projection matrices are
 // stacked along N in Model::layers, each task's own LayerNorm gamma folded into its slice and BERT's biases stacked the
-// same way.  A batch runs ONCE as T copies of its rows (task-major, each copy padded to whole 256-row blocks): every row
-// block of a projection GEMM picks its task's matrix and bias (gemm.h: w_groups), every row kernel its task's embeddings
-// and norms (kernels.h: RowGroups), every task's head its task's final_norm -- the numerics of T separately loaded
-// models in one pass.  Outside such a pass the model is task 0.
+// same way; every task's embeddings and norms are Model::task[t].  A batch runs ONCE as T copies of its rows (task-major,
+// each copy padded to whole 256-row blocks): every row block of a projection GEMM picks its task's matrix and bias
+// (gemm.h: w_groups), every row kernel its task's embeddings and norms (kernels.h: RowGroups), every task's head its
+// task's final_norm -- the numerics of T separately loaded models in one pass.  Outside such a pass the model is task 0;
+// a model from model_load is a model of that one task.
 struct TaskNorms {      // one layer's norms of one task (null where the architecture has none)
-  float *attn_w = nullptr, *mid_w = nullptr, *mid_b = nullptr, *out_w = nullptr, *out_b = nullptr;
+  float* attn_w = nullptr;   // ModernBERT pre-attention LN (null on layer 0 and wherever the checkpoint has none)
+  float* mid_w = nullptr;    // ModernBERT mlp_norm / BERT attention.output.LayerNorm
+  float* mid_b = nullptr;
+  float *out_w = nullptr, *out_b = nullptr;   // BERT output.LayerNorm
 };
 struct TaskTensors {    // one task's tensors outside the projections; a tensor equal in every task is ONE allocation
   float *emb_word = nullptr, *emb_pos = nullptr, *emb_type0 = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
   float* final_norm_w = nullptr;
   std::vector<TaskNorms> layers;
 };
-struct Grouped {
-  int tasks = 0;        // 0: an ordinary model
-  std::vector<TaskTensors> task;
+struct Grouped {        // what describes a grouped pass
+  int tasks = 0;        // 0: a model from model_load
   std::vector<int> head_of_task;
   int rows_per_task = 0;   // set (under mu) for one forward: rows [t * rows_per_task, (t + 1) * rows_per_task) belong to task t
 };
@@ -164,13 +162,8 @@ struct Model {
   Profiler prof;
   EncoderConfig cfg;
   std::string dir;
-  float* emb_word = nullptr;
-  float* emb_pos = nullptr;
-  float* emb_type0 = nullptr;
-  float* emb_ln_w = nullptr;
-  float* emb_ln_b = nullptr;
+  std::vector<TaskTensors> task;   // at least one; task[0] outside a grouped pass
   std::vector<LayerWeights> layers;
-  float* final_norm_w = nullptr;
   float *rope_cos_g = nullptr, *rope_sin_g = nullptr, *rope_cos_l = nullptr, *rope_sin_l = nullptr;
   int rope_len = 0;
   std::vector<Head> heads;
@@ -187,10 +180,13 @@ struct Model {
   size_t weight_bytes = 0;    // bytes of those allocations (the loaded tensors)
 };
 
+// The loaders read every directory on the host first: a checkpoint that cannot be served is refused before a device is
+// touched.  Adapters a checkpoint carries are merged (lora_config.json alpha).
+// One checkpoint as a model of one task (Grouped::tasks stays 0); its classifier, when there is one of width H, is head 0
+// (token_level from config.json).
 Model* model_load(const std::string& dir, int device, std::string* err);
 // 1..8 task checkpoints of one encoder shape (every EncoderConfig field equal, no padded heads), each with its own head,
-// as one grouped model (engine.h: Grouped).  Adapters a checkpoint carries are merged as model_load merges them.
-// token_level[t]: 1 / 0 / -1 (from config.json).  Every refusal of the directories comes before a device is touched.
+// as one grouped model (engine.h: Grouped).  token_level[t]: 1 / 0 / -1 (from config.json).
 Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
                           std::string* err);
 // model_load_grouped for unmerged LoRA checkpoints over ONE base: refuses directories whose base tensors differ or that

@@ -228,7 +228,8 @@ int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, 
     return -1;
   const int L = (num_layers <= 0 || num_layers > c.L) ? c.L : num_layers;
   if (compute_positions(s, d_cu, B, w.pos)) return -1;
-  if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, m.emb_word, m.emb_ln_w, c.ln_eps, w.x, w.h)) return -1;
+  const TaskTensors& task = m.task[0];
+  if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, task.emb_word, task.emb_ln_w, c.ln_eps, w.x, w.h)) return -1;
   const int rows_grid = (T * 32 + 255) / 256;
   auto gemm = [&](const __half* a, const __half* wt, int n, int k, float* out, bool resid) {
     GemmDesc g;
@@ -239,11 +240,11 @@ int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, 
     return gemm_f16(s, g);
   };
   for (int li = 0; li < L; ++li) {
-    const LayerWeights& lw = m.layers[li];
+    const TaskNorms& norms = task.layers[li];
     const PreciseLayer& pl = p.layers[li];
     const bool local = (li % c.global_every) != 0;
     // attention input: LayerNorm (none on layer 0, modernbert.rs:266-271), split
-    if (lw.attn_norm_w) split_rows_kernel<true><<<rows_grid, 256, 0, s>>>(w.x, T, H, lw.attn_norm_w, c.ln_eps, p.split);
+    if (norms.attn_w) split_rows_kernel<true><<<rows_grid, 256, 0, s>>>(w.x, T, H, norms.attn_w, c.ln_eps, p.split);
     else split_rows_kernel<false><<<rows_grid, 256, 0, s>>>(w.x, T, H, nullptr, 0.f, p.split);
     if (gemm(p.split, pl.wqkv, 3 * H, H, p.qkv32, false)) return -1;
     {
@@ -258,7 +259,7 @@ int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, 
     }
     split_rows_kernel<false><<<rows_grid, 256, 0, s>>>(p.ctx32, T, H, nullptr, 0.f, p.split);
     if (gemm(p.split, pl.wo, H, H, w.x, true)) return -1;
-    split_rows_kernel<true><<<rows_grid, 256, 0, s>>>(w.x, T, H, lw.mid_norm_w, c.ln_eps, p.split);
+    split_rows_kernel<true><<<rows_grid, 256, 0, s>>>(w.x, T, H, norms.mid_w, c.ln_eps, p.split);
     if (gemm(p.split, pl.wi, 2 * I, H, p.mid32, false)) return -1;
     {
       const size_t n = static_cast<size_t>(T) * I;

@@ -1,7 +1,8 @@
-"""The grouped loader's refusals without a GPU (sr_model_load_grouped, binding.GroupedModel): directories that cannot be
-served as one grouped model are refused from their config.json and safetensors header alone, BEFORE any device is
-touched -- so a host without a GPU sees these messages, not the missing device.  And the text ABI's choice between one
-grouped model and three slots for merged checkpoints, on the mock engine."""
+"""The loaders' refusals without a GPU (sr_model_load_grouped, binding.GroupedModel, and sr_model_load for one
+directory): directories that cannot be served are refused from their config.json and safetensors header alone, BEFORE any
+device is touched -- so a host without a GPU sees these messages, not the missing device.  And the text ABI's choice
+between one grouped model and three slots for merged checkpoints, on the mock engine."""
+import ctypes as C
 import json
 import os
 import shutil
@@ -81,6 +82,42 @@ def test_servable_directories_reach_the_device(dirs):
         pytest.skip("a device is present")
     with pytest.raises(pkg.SrError, match="no CUDA device"):
         pkg.GroupedModel([dirs["a"], dirs["b"]], [0, 0], device=0)
+
+
+# ---- sr_model_load: one directory, refused on the host in the same way; its error names the directory once ----------
+def _single_load_error(d):
+    import semantic_router_b200 as pkg
+    h = C.c_void_p()
+    assert pkg.lib().sr_model_load(d.encode(), 0, C.byref(h)) != 0
+    assert not h.value                                           # no model returned
+    return pkg.lib().sr_last_error().decode()
+
+
+@pytest.mark.parametrize("fields,message", [
+    (dict(hidden_size=512, num_attention_heads=8), "hidden_size unsupported"),
+    (dict(intermediate_size=1136), "intermediate_size must be a multiple of 64"),
+    (dict(hidden_size=384, num_attention_heads=12, intermediate_size=1152), "head_dim 32 unsupported"),
+])
+def test_single_load_refuses_an_unservable_config(tmp_path, fields, message):
+    from oracle import encoder_oracle as eo
+    d = _dir(tmp_path / "m", eo.ModernBertConfig(vocab_size=1000, num_hidden_layers=2, max_position_embeddings=1024, pad_token_id=0,
+                                                 **fields))
+    err = _single_load_error(d)
+    assert message in err and err.count(d) == 1
+
+
+def test_single_load_of_a_missing_directory(dirs):
+    err = _single_load_error(dirs["missing"])
+    assert "cannot read " + dirs["missing"] + "/config.json" in err and err.count(dirs["missing"]) == 1
+
+
+@pytest.mark.parametrize("which", ["a", "bert", "minilm"])
+def test_single_load_of_a_servable_directory_reaches_the_device(dirs, which):
+    """padded-head (MiniLM) encoders included: only the grouped loader refuses them"""
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("a device is present")
+    assert "no CUDA device" in _single_load_error(dirs[which])
 
 
 # ---- text ABI on the mock engine: merged checkpoints as one grouped model, or three slots ----------------------------
