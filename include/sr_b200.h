@@ -90,11 +90,13 @@ SR_API int sr_classify_multi_ids(sr_model* m, const int* heads, int n_heads, con
  * (the reference publishes its LoRA classifiers merged, lora_*_model), full fine-tunes of one base, or anything else of
  * one encoder shape.  Every config.json field that shapes the encoder (architecture, hidden_size, num_hidden_layers,
  * num_attention_heads, intermediate_size, vocab_size, max_position_embeddings, global_attn_every_n_layers,
- * local_attention, both rope thetas, layer_norm_eps, classifier_pooling) must be equal, and padded-head (MiniLM) encoders
- * are refused; these refusals name the field and the directory and come before any device is touched.  A tensor that
+ * local_attention, both rope thetas, layer_norm_eps, classifier_pooling) must be equal, padded-head (MiniLM) encoders
+ * are refused, and so are two or more BERT tasks whose intermediate_size is not a multiple of 128; these refusals name
+ * the field and the directory and come before any device is touched.  A tensor that
  * is bitwise the same in every task is loaded once; one that differs gets a device copy per task.  Each task's
  * projection weights (its own LayerNorm gamma folded in, adapters a checkpoint still carries merged as sr_model_load
- * merges them) are stacked.  A batch then runs ONCE through the encoder as n_tasks copies of its rows: each 256-row block
+ * merges them) are stacked.  A batch then runs ONCE through the encoder as n_tasks copies of its rows, each padded to
+ * whole 256-row blocks by pad sequences of at most min(255, max_position_embeddings) rows: each 256-row block
  * of a projection GEMM picks its task's matrix and bias, every embedding and LayerNorm row its task's weights, every
  * task's head its task's final norm -- bitwise what n_tasks separately loaded models give.  The ordinary entries above
  * run task 0's encoder on such a model; sr_model_set_precise refuses it.  token_level[t]: 1 token head, 0 sequence head, -1

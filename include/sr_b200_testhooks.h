@@ -40,7 +40,8 @@ SR_API int sr_test_gemm_cluster(int epi, int n, int k, int* cluster_n, int* work
 /* Every field of the GEMM descriptor (csrc/gemm.h GemmDesc, same names and meaning; epi = GemmEpilogue value).  Zeroed
  * fields take GemmDesc's defaults.  EPI_ROPE / EPI_GEGLU with fold_stats (weights: W diag(gamma) with zero-sum rows)
  * scale the accumulator rows by the rstd computed from fold_stats over rows of length fold_h; the EPI_RESID_HL fields
- * mean what they mean for sr_test_gemm_resid_hl (out = hi). */
+ * mean what they mean for sr_test_gemm_resid_hl (out = hi).  bias_per_group (with w_groups > 1): bias holds w_groups
+ * vectors of n, and rows of group g add bias[g * n, (g + 1) * n). */
 typedef struct sr_gemm_desc {
   int m, n, k;
   const void* a;
@@ -69,6 +70,7 @@ typedef struct sr_gemm_desc {
   float fold_eps;
   int fold_h;
   int w_groups, w_group_rows;
+  int bias_per_group;
 } sr_gemm_desc;
 /* gemm_f16 on the legacy default stream with every descriptor field; EPI_TOPK's list count goes to *topk_lists. */
 SR_API int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists);

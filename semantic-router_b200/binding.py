@@ -108,7 +108,7 @@ class GemmDesc(C.Structure):
         ("topk_score", C.c_void_p), ("topk_valid", C.c_void_p), ("topk_n", C.c_int), ("row_stats", C.c_void_p),
         ("lo16", C.c_void_p), ("pivot_out", C.c_void_p), ("pivot_in", C.c_void_p),
         ("pivot_in_stats", C.c_void_p), ("fold_stats", C.c_void_p), ("fold_eps", C.c_float), ("fold_h", C.c_int),
-        ("w_groups", C.c_int), ("w_group_rows", C.c_int)]
+        ("w_groups", C.c_int), ("w_group_rows", C.c_int), ("bias_per_group", C.c_int)]
 
 
 def run_gemm(**fields):

@@ -428,15 +428,20 @@ int sr_classify_lora_shared_ids(sr_model* h, const int32_t* ids, const int32_t* 
   const int T1 = cu[batch];
   if (T1 <= 0 || static_cast<long long>(T1) * nt > (1ll << 30)) return fail("bad arguments");
   // the batch once per task, task-major: rows [t * T1p, t * T1p + T1) run with task t's weights.  Every copy is padded to
-  // whole 256-row GEMM blocks (a block multiplies ONE task's matrices); the pad rows form one extra sequence per copy that
-  // runs through the encoder and is read by nobody.
+  // whole 256-row GEMM blocks (a block multiplies ONE task's matrices); the pad rows form extra sequences per copy that
+  // run through the encoder and are read by nobody.  A pad sequence is at most min(255, max_position_embeddings) rows, so
+  // it never exceeds the position range of a prompt the model serves alone: one sequence when max_position_embeddings
+  // >= 256, several below.  Their number depends on T1 alone for a given model, which the graph key holds.
   const int T1p = (T1 + 255) / 256 * 256;
   const int pad = T1p - T1;
-  const int Bp = batch + (pad > 0 ? 1 : 0);
+  const int piece = std::max(1, std::min(255, m.cfg.max_pos));
+  const int pieces = (pad + piece - 1) / piece;
+  const int Bp = batch + pieces;
   std::vector<int32_t> rids(static_cast<size_t>(T1p) * nt, 0), rcu(static_cast<size_t>(Bp) * nt + 1);
   for (int t = 0; t < nt; ++t) {
     memcpy(rids.data() + static_cast<size_t>(t) * T1p, ids, sizeof(int32_t) * T1);
     for (int b = 0; b <= batch; ++b) rcu[static_cast<size_t>(t) * Bp + b] = t * T1p + cu[b];
+    for (int k = 1; k < pieces; ++k) rcu[static_cast<size_t>(t) * Bp + batch + k] = t * T1p + T1 + k * piece;
   }
   rcu[static_cast<size_t>(Bp) * nt] = nt * T1p;
   size_t cseq = 0, ctok = 0;
@@ -589,7 +594,7 @@ int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
   g.row_stats = d->row_stats; g.lo16 = d->lo16;
   g.pivot_out = d->pivot_out; g.pivot_in = d->pivot_in; g.pivot_in_stats = d->pivot_in_stats;
   g.fold_stats = d->fold_stats; g.fold_eps = d->fold_eps; g.fold_h = d->fold_h;
-  g.w_groups = d->w_groups; g.w_group_rows = d->w_group_rows;
+  g.w_groups = d->w_groups; g.w_group_rows = d->w_group_rows; g.bias_per_group = d->bias_per_group != 0;
   return gemm_f16(nullptr, g);
 }
 int sr_test_cache_plan(int b, int n, int dim, int k, int* route, int* chunks, int* candidates) {

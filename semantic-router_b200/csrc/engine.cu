@@ -812,6 +812,12 @@ Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vecto
         return nullptr;
       }
     if (!ck[t].st.find("classifier.weight")) { *err = "no classifier.weight in " + d; return nullptr; }
+    // BERT's Wi has N = intermediate_size, and gemm_f16 picks a task's matrix per row block only when N is whole
+    // 128-column tiles (ModernBERT's Wi, N = 2 I with I % 64 == 0, always is)
+    if (T > 1 && ck[t].cfg.arch == ARCH_BERT && ck[t].cfg.I % 128 != 0) {
+      *err = d + ": intermediate_size " + std::to_string(ck[t].cfg.I) + " must be a multiple of 128 to serve several BERT tasks in one pass";
+      return nullptr;
+    }
   }
   if (!use_device(device, err)) return nullptr;
   std::vector<Loader> lt;

@@ -139,7 +139,7 @@ class Problem:
 
 
 def problem(epi, M, N, K, seed, *, bias=False, resid=True, fold=False, rope_cols=0, w_groups=0, w_group_rows=0,
-            stale=True, w_scale=0.05):
+            stale=True, w_scale=0.05, bias_per_group=False):
     dev = torch.device(DEV)
     g = torch.Generator(device=dev).manual_seed(seed)
     a_rows = _up(M, 128) + 64 if stale else M
@@ -148,9 +148,11 @@ def problem(epi, M, N, K, seed, *, bias=False, resid=True, fold=False, rope_cols
     d = dict(m=M, n=N, k=K, a=A, a_rows=a_rows, w=W, epi=epi)
     o = {}
     _stale(A, M)
-    if bias:
-        b = torch.randn(N, generator=g, device=dev)
+    if bias:                                   # bias_per_group: one vector per stacked matrix
+        b = torch.randn(N * (w_groups if bias_per_group else 1), generator=g, device=dev)
         d["bias"] = o["bias"] = b
+        if bias_per_group:
+            d["bias_per_group"], o["bias_per_group"] = 1, True
     if epi == EPI_ROPE:
         cos, sin = _rope_tables()
         pos = torch.randint(0, 1024, (M,), generator=g, device=dev, dtype=torch.int32)
@@ -249,21 +251,30 @@ def test_layernorm_fold(lib, epi, N, M):
     check_parity(p, tag=go.EPI_NAMES[epi] + "+fold")
 
 
-GROUPED = [(EPI_F16, 384, 200, False), (EPI_ROPE, 2304, 768, False), (EPI_ROPE, 2304, 768, True),
-           (EPI_ROPE, 1152, 768, False), (EPI_ROPE, 1152, 768, True), (EPI_GEGLU, 2304, 768, False),
-           (EPI_GEGLU, 2304, 768, True), (EPI_RESID_HL, 768, 768, False)]
+# (epi, N, K, fold, a bias per group).  GeGLU N = 640 / 2176 / 5248 (I = 320 / 1088 / 2624): the wide kernel's last
+# 192-column tile of a group reaches into the next group's matrix, which must be clipped.  The per-group biases are
+# BERT's grouped epilogues: Wqkv (EPI_F16), Wi (EPI_GELU), Wo and Wo2 (EPI_RESID in place).
+GROUPED = [(EPI_F16, 384, 200, False, False), (EPI_ROPE, 2304, 768, False, False), (EPI_ROPE, 2304, 768, True, False),
+           (EPI_ROPE, 1152, 768, False, False), (EPI_ROPE, 1152, 768, True, False), (EPI_GEGLU, 2304, 768, False, False),
+           (EPI_GEGLU, 2304, 768, True, False), (EPI_RESID_HL, 768, 768, False, False),
+           (EPI_GEGLU, 640, 384, False, False), (EPI_GEGLU, 640, 384, True, False),
+           (EPI_GEGLU, 2176, 768, False, False), (EPI_GEGLU, 2176, 768, True, False),
+           (EPI_GEGLU, 5248, 1024, False, False), (EPI_GEGLU, 5248, 1024, True, False),
+           (EPI_F16, 2304, 768, False, True), (EPI_GELU, 3072, 768, False, True), (EPI_GELU, 1536, 384, False, True),
+           (EPI_RESID, 768, 3072, False, True), (EPI_RESID, 1024, 4096, False, True)]
 
 
 @pytest.mark.parametrize("rows", [128, 256])
-@pytest.mark.parametrize("epi,N,K,fold", GROUPED,
-                         ids=[f"{e}-{n}-{k}" + ("-fold" if f else "") for e, n, k, f in GROUPED])
-def test_grouped_weights(lib, epi, N, K, fold, rows):
+@pytest.mark.parametrize("epi,N,K,fold,gbias", GROUPED,
+                         ids=[f"{e}-{n}-{k}" + ("-fold" if f else "") + ("-gbias" if b else "") for e, n, k, f, b in GROUPED])
+def test_grouped_weights(lib, epi, N, K, fold, gbias, rows):
     """w_groups = 3 stacked matrices; the last group is partly empty.  Row blocks of 128 never straddle two groups
     when w_group_rows is a multiple of 128, which is what gemm_f16 accepts.  The LayerNorm-fold projections run in
-    pairs at N = 2304 and unclustered at N = 1152 (the shared-LoRA serving shapes)."""
+    pairs at N = 2304 and unclustered at N = 1152 (the shared-LoRA serving shapes).  gbias: each group adds its own
+    bias (EPI_RESID in place over a residual)."""
     p = problem(epi, 3 * rows - 5, N, K, seed=rows + epi, w_groups=3, w_group_rows=rows, rope_cols=ROPE_COLS.get(N, 0),
-                bias=epi == EPI_F16, fold=fold, w_scale=0.01 if fold else 0.05)
-    check_parity(p, tag=go.EPI_NAMES[epi] + ("+grp+fold" if fold else "+grp"))
+                bias=epi == EPI_F16 or gbias, bias_per_group=gbias, fold=fold, w_scale=0.01 if fold else 0.05)
+    check_parity(p, tag=go.EPI_NAMES[epi] + ("+grp+fold" if fold else "+grp") + ("+gbias" if gbias else ""))
 
 
 # ---- the cache scan: GEMV (B <= 4), fused top-8 epilogue (one row block, and the grouped schedule), two-pass (k > 8)
@@ -353,16 +364,25 @@ def test_cluster_pair_equals_unclustered_halves(lib, epi, fold):
 
 
 @pytest.mark.parametrize("rows", [128, 256])
-@pytest.mark.parametrize("epi", [EPI_RESID, EPI_F16], ids=["resid", "f16"])
-def test_grouped_weights_are_per_group_gemms(lib, epi, rows):
+@pytest.mark.parametrize("epi,gbias", [(EPI_RESID, False), (EPI_F16, False), (EPI_RESID, True), (EPI_F16, True),
+                                       (EPI_GELU, True)],
+                         ids=["resid", "f16", "resid-gbias", "f16-gbias", "gelu-gbias"])
+def test_grouped_weights_are_per_group_gemms(lib, epi, gbias, rows):
+    """gbias: each group's GEMM gets its own bias (EPI_RESID over a residual, in place)"""
     M, N, K = 3 * rows, 384, 200
-    p = problem(epi, M, N, K, seed=rows, w_groups=3, w_group_rows=rows, resid=False)
+    p = problem(epi, M, N, K, seed=rows, w_groups=3, w_group_rows=rows, resid=gbias, bias=gbias, bias_per_group=gbias)
     d = p.desc
+    out0 = p.out.clone()
     assert run(**d)[0] == 0
     grouped = p.out[:M].clone()
+    p.out.copy_(out0)
     for g in range(3):
-        dg = {k: v for k, v in d.items() if k not in ("w_groups", "w_group_rows")}
+        dg = {k: v for k, v in d.items() if k not in ("w_groups", "w_group_rows", "bias_per_group")}
         dg.update(m=rows, a=d["a"][g * rows:], a_rows=rows, w=d["w"][g * N:(g + 1) * N], out=p.out[g * rows:])
+        if gbias:
+            dg["bias"] = d["bias"][g * N:(g + 1) * N]
+        if "resid" in d:
+            dg["resid"] = dg["out"]
         assert run(**dg)[0] == 0
     assert torch.equal(_bits(grouped), _bits(p.out[:M]))
 

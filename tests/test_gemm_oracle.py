@@ -108,6 +108,28 @@ def test_grouped_weights():
         torch.testing.assert_close(r.value[sl], a[sl].double() @ w[i * N:(i + 1) * N].double().t(), rtol=1e-14, atol=0)
 
 
+@pytest.mark.parametrize("epi", [go.EPI_F16, go.EPI_GELU, go.EPI_RESID])
+def test_grouped_weights_with_a_bias_per_group(epi):
+    """bias_per_group: rows of group g are group g's GEMM with group g's bias (the last group partly empty), and one
+    bias for every group -- a group's rows adding group 0's vector -- is far outside the bound"""
+    g = _gen(7)
+    rows, G, K, N = 128, 3, 64, 128
+    M = G * rows - 7
+    a, w = _f16((M, K), g), _f16((G * N, K), g, 0.1)
+    bias = torch.randn(G * N, generator=g)
+    resid = torch.randn(M, N, generator=g) if epi == go.EPI_RESID else None
+    r = go.gemm(epi, a, w, N, bias=bias, resid=resid, w_groups=G, w_group_rows=rows, bias_per_group=True)
+    for i in range(G):
+        sl = slice(i * rows, min((i + 1) * rows, M))
+        one = go.gemm(epi, a[sl], w[i * N:(i + 1) * N], N, bias=bias[i * N:(i + 1) * N],
+                      resid=None if resid is None else resid[sl])
+        for x, y in ((r.value, one.value), (r.coef, one.coef), (r.eps, one.eps)):
+            torch.testing.assert_close(x[sl], y, rtol=0, atol=0)
+    shared = go.gemm(epi, a, w, N, bias=bias, resid=resid, w_groups=G, w_group_rows=rows)
+    assert torch.equal(shared.value[:rows], r.value[:rows])
+    assert ((shared.value[rows:] - r.value[rows:]).abs() > r.bound()[rows:]).any()
+
+
 def test_gelu_derivative_and_bound_covers_rounding():
     x = torch.linspace(-8, 8, 2001, dtype=torch.float64)
     h = 1e-6

@@ -62,6 +62,22 @@ def test_task_count_outside_one_to_eight(dirs, n):
         pkg.GroupedModel([dirs["a"]] * n, [0] * n, device=0)
 
 
+def test_several_bert_tasks_need_whole_128_column_wi_tiles(tmp_path):
+    """BERT's Wi has N = intermediate_size, and a grouped GEMM picks a task's matrix only over whole 128-column tiles:
+    I = 1088 is refused for two tasks, from config.json alone.  One task reaches the device like any single load."""
+    import torch
+    import semantic_router_b200 as pkg
+    from oracle import encoder_oracle as eo
+    cfg = eo.BertConfig(vocab_size=1000, num_hidden_layers=2, intermediate_size=1088)
+    d0, d1 = _dir(tmp_path / "bert0", cfg, "bert"), _dir(tmp_path / "bert1", cfg, "bert")
+    with pytest.raises(pkg.SrError, match=f"{d0}: intermediate_size 1088 must be a multiple of 128"):
+        pkg.GroupedModel([d0, d1], [0, 0], device=0)
+    if torch.cuda.is_available():
+        return
+    with pytest.raises(pkg.SrError, match="no CUDA device"):
+        pkg.GroupedModel([d0], [0], device=0)
+
+
 def test_token_level_count_must_match(dirs):
     import semantic_router_b200 as pkg
     with pytest.raises(pkg.SrError, match="3 token_level values for 2 task checkpoints"):
