@@ -83,6 +83,16 @@ SR_API int sr_test_hl_to_f32(const void* hi_f16, const void* lo_f16, const float
 /* attention_wgmma_fwd (csrc/kernels.h: same arguments and meaning; window 0 = global, kv_lens [batch] or null) */
 SR_API int sr_test_attention_wgmma(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int max_len,
                                    int num_heads, int head_dim, int window, const int32_t* kv_lens);
+/* ---- the precise path's row kernels (csrc/precise.cu), one hook per launcher (csrc/engine.h: same arguments and meaning) */
+/* x [t, h] fp32 -> out [t, 3h] fp16 rows [hi | lo | hi]; gamma non-null: the no-bias LayerNorm with eps first */
+SR_API int sr_test_precise_split(const float* x, int t, int h, const float* gamma, float eps, void* out_f16);
+/* rotate-half RoPE in place on the q and k thirds of qkv [t, 3 * heads * 64] fp32 with the [*, 32] tables at pos[t] */
+SR_API int sr_test_precise_rope(float* qkv, const int32_t* pos, int t, int heads, const float* cos_t, const float* sin_t);
+/* out [t, i] = gelu_erf(a) * b, ab [t, 2i] fp32 */
+SR_API int sr_test_precise_geglu(const float* ab, int t, int i, float* out);
+/* fp32 attention over packed qkv [T, 3 * heads * 64] -> out [T, heads * 64]; window 0 = global */
+SR_API int sr_test_precise_attention(const float* qkv, float* out, const int32_t* cu_seqlens, int batch, int max_len,
+                                     int heads, int window);
 SR_API int sr_test_layernorm(const float* x, int t, int h, const float* w, const float* b, float eps, float* y32,
                       void* y16);
 

@@ -16,6 +16,14 @@ output rounds).  TAU = 2^-20 is 2.1x that.  Longer sums reach more: the grouped 
 group at K = 3072 and 4096 (BERT's Wo2) reach 7.0e-7 = 2^-20.44, 1.4x under TAU.  It must stay <= 2^-16: then at
 K <= 4096 one missing k-term of average size (S / K >= 2^-12 S) is 16x the bound, so a dropped k-column or k-block
 cannot pass.
+
+The precise path's GEMMs (gemm(..., split=True)) sum three times as deep, K' = 3K up to 3 x 4096 = 12 288, and there the
+error per unit of S' grows with the depth: over tests/test_precise_kernels_gpu.py on an H100 80GB HBM3 at 700 W the
+largest (|err| - eps) / S' was 4.7e-7 at K' = 1152, 7.2e-7 - 7.6e-7 at K' = 2304 - 3456, 1.6e-6 at K' = 7872 and
+1.8e-6 = 2^-19.1 at K' = 12 288 (M 17 370, N 1024): beyond TAU, close to the sqrt(K) growth of a sum of
+roundings of either sign.  So the split form carries TAU depth_scale(K') = 2^-20 sqrt(K' / 1024), 3.3e-6 at K' = 12 288,
+1.8x the measured value (1.0e-6 at K' <= 1024, 2.2x the 4.47e-7 above).  One missing k-term of average size is still
+S' / K' = 8e-5 S' at K' = 12 288, 25x the bound.
 """
 from __future__ import annotations
 
@@ -100,15 +108,58 @@ def accumulate(a, w, n, w_groups=0, w_group_rows=0):
     return acc, s
 
 
+def depth_scale(k: int) -> float:
+    """TAU's growth with the depth of the sum beyond K = 1024: sqrt(K / 1024) (module docstring)"""
+    return max(1.0, math.sqrt(k / 1024.0))
+
+
+def split_pair(x: torch.Tensor):
+    """(hi, lo) fp16 of fp32 x: hi = fp16_rn(x), lo = fp16_rn(x - hi), as precise.cu's split_weight and split_rows_kernel"""
+    x = x.float()
+    hi = x.half()
+    return hi, (x - hi.float()).half()
+
+
+def split3(a: torch.Tensor, w: torch.Tensor):
+    """the precise path's triple-depth operands of fp32 A [M, K] and W [N, K]: A' = [A_hi | A_lo | A_hi] and
+    W' = [W_hi | W_hi | W_lo], fp16 [*, 3K], so that A' W'^T = A_hi W_hi^T + A_lo W_hi^T + A_hi W_lo^T"""
+    ah, al = split_pair(a)
+    wh, wl = split_pair(w)
+    return torch.cat([ah, al, ah], 1).contiguous(), torch.cat([wh, wh, wl], 1).contiguous()
+
+
+def _split_terms(a, w, n):
+    """(A W^T of the unsplit fp32 operands, S' = |A'| |W'|^T, the split's own error) in float64: the dropped A_lo W_lo^T
+    and the residuals |x - hi - lo| of both operands (half an fp16 ulp of x - hi: 2^-25 where lo is subnormal)"""
+    w = w[:n]
+    (ah, al), (wh, wl) = split_pair(a), split_pair(w)
+    a64, w64 = a.double(), w.double()
+    ra, rw = (a64 - ah.double() - al.double()).abs(), (w64 - wh.double() - wl.double()).abs()
+    ah, al, wh, wl = (t.double().abs() for t in (ah, al, wh, wl))
+    acc = a64 @ w64.t()
+    s = ah @ wh.t() + al @ wh.t() + ah @ wl.t()
+    own = al @ wl.t() + ra @ w64.abs().t() + a64.abs() @ rw.t()
+    return acc, s, own
+
+
 def gemm(epi: int, a: torch.Tensor, w: torch.Tensor, n: Optional[int] = None, *, bias=None, resid=None, pos=None,
          rope_cos=None, rope_sin=None, rope_cols: int = 0, fold_stats=None, fold_eps: float = 0.0, fold_h: int = 0,
-         w_groups: int = 0, w_group_rows: int = 0, bias_per_group: bool = False) -> Ref:
+         w_groups: int = 0, w_group_rows: int = 0, bias_per_group: bool = False, split: bool = False) -> Ref:
     """Reference of gemm_f16 for a = A [M, K] (only the M rows the GEMM computes), w = W [N, K] (grouped: the stack),
     n = N.  EPI_RESID / EPI_RESID_HL: resid = the stream before the GEMM (the fp16 pair as hi + lo), or None.
     EPI_GEGLU: w rows interleaved in 32-row (a | b) groups; the result is [M, N / 2].  bias_per_group (grouped
-    weights): bias is w_groups vectors of n stacked like the matrices, and rows of group g add bias[g n:(g + 1) n]."""
+    weights): bias is w_groups vectors of n stacked like the matrices, and rows of group g add bias[g n:(g + 1) n].
+    split (EPI_RESID only): a and w are the fp32 operands of the precise path, which multiplies split3(a, w) at depth 3K;
+    the value is the float64 product of the UNSPLIT a and w, coef is S' over the three parts, and eps also carries the
+    dropped A_lo W_lo^T and the split residuals."""
     n = w.shape[0] if n is None else n
     m = a.shape[0]
+    if split:
+        assert epi == EPI_RESID and w_groups <= 1 and bias is None
+        acc, s, own = _split_terms(a, w, n)
+        r = resid.double()[:m, :n] if resid is not None else torch.zeros_like(acc)
+        v = r + acc
+        return Ref(v, s * depth_scale(3 * a.shape[1]), 2 * U32 * (r.abs() + v.abs()) + own)
     acc, s = accumulate(a, w, n, w_groups, w_group_rows)
     if bias is None:
         b = torch.zeros(n, dtype=torch.float64, device=acc.device)

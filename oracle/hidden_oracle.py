@@ -55,10 +55,14 @@ The fp32 denominator summed over n / 64 key blocks adds (n / 64) 2^-24 at worst,
 trained-like and wide families at H 768 and 384, as at 300 tokens.  A rope row read at fp16(position) or at
 position % 2048 leaves the bound by > 70x on the rows past 2048 (wide family, H 768).  Measured on an H100 80GB HBM3 at
 700 W, the engine's rows at 2049, 8192 and 32 768 tokens and in the 131 072-row batch reach at most 0.47 of the bound on
-the production path and 0.39 on the precise one.  The precise path's attention sums all keys of a global row in one fp32
-chain, whose rounding grows as sqrt(n) 2^-24; on the trained-like family its worst row goes from 0.14 of the bound at
-8192 tokens to 0.37 at 32 768, the longest position table of the mmBERT checkpoints.  Whether that chain is the cause
-is not established.
+the production path and 0.39 on the precise one.  The precise path's attention used to sum all keys of a global row in
+one fp32 chain; on the trained-like family its worst row went from 0.14 of the bound at 8192 tokens to 0.37 at 32 768,
+the longest position table of the mmBERT checkpoints.  That chain was the cause.  Its rounding grows linearly in n where
+the terms are correlated: on constant V columns under uniform scores at 32 768 keys the chained kernel was 4.9e-4
+relative off (3.9x the bound of oracle/precise_oracle.py for per-tile sums, 2.4x at 8192 keys; the same numbers as the
+float32 restatement), the kernel that sums each 32-key tile first and then adds it to the running sums 1.0e-5 (0.08 of
+that bound).  With per-tile sums the trained-like rows are at 0.15 of the bound at 8192 tokens and 0.16 at 32 768 (plain
+family 0.045 at both; H100 80GB HBM3, 700 W).
 
 The precise path (csrc/precise.cu) splits every GEMM operand into an fp16 pair and accumulates in fp32 on the tensor
 cores; everything between the GEMMs is fp32.  Its u is precise_u(cfg) = TAU_MEASURED * 0.64 sqrt(K), K = max(H, I) the

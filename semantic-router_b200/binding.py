@@ -139,6 +139,10 @@ def hooks():
         H.sr_test_gemm_cluster.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp]
         H.sr_test_attention_wgmma.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         H.sr_test_layernorm.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_float, vp, vp]
+        H.sr_test_precise_split.argtypes = [vp, C.c_int, C.c_int, vp, C.c_float, vp]
+        H.sr_test_precise_rope.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp]
+        H.sr_test_precise_geglu.argtypes = [vp, C.c_int, C.c_int, vp]
+        H.sr_test_precise_attention.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
         H.sr_test_hl_to_f32.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
         H.sr_test_cache_plan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
         ci, cf = C.c_int, C.c_float

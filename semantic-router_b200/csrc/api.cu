@@ -612,6 +612,16 @@ int sr_test_attention_wgmma(const void* qkv, void* out, const int32_t* cu, int b
   return attention_wgmma_fwd(nullptr, static_cast<const __half*>(qkv), static_cast<__half*>(out), cu, batch, max_len,
                              num_heads, head_dim, window, kv_lens);
 }
+int sr_test_precise_split(const float* x, int t, int hdim, const float* gamma, float eps, void* out) {
+  return precise_split_rows(nullptr, x, t, hdim, gamma, eps, static_cast<__half*>(out));
+}
+int sr_test_precise_rope(float* qkv, const int32_t* pos, int t, int heads, const float* cos_t, const float* sin_t) {
+  return precise_rope(nullptr, qkv, pos, t, heads, cos_t, sin_t);
+}
+int sr_test_precise_geglu(const float* ab, int t, int i, float* out) { return precise_geglu(nullptr, ab, t, i, out); }
+int sr_test_precise_attention(const float* qkv, float* out, const int32_t* cu, int batch, int max_len, int heads, int window) {
+  return precise_attention(nullptr, qkv, out, cu, batch, max_len, heads, window);
+}
 int sr_test_layernorm(const float* x, int t, int hdim, const float* w, const float* b, float eps, float* y32, void* y16) {
   return layernorm_rows(nullptr, x, t, hdim, w, b, eps, y32, static_cast<__half*>(y16));
 }

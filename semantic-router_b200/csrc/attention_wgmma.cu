@@ -256,11 +256,15 @@ int attention_wgmma_fwd(cudaStream_t stream, const __half* qkv, __half* out, con
     return -1;
   }
   if (batch <= 0 || max_len <= 0) return 0;
-  const dim3 grid((max_len + kBQ - 1) / kBQ, num_heads, batch);
   const float scale_log2 = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e)
-  attn_wgmma_kernel<<<grid, 128, 0, stream>>>(qkv, out, cu_seqlens, num_heads, window, scale_log2, kv_lens);
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
+  for (int b0 = 0; b0 < batch; b0 += kMaxGridZ) {   // the kernel reads absolute row offsets from cu_seqlens
+    const int nb = batch - b0 < kMaxGridZ ? batch - b0 : kMaxGridZ;
+    const dim3 grid((max_len + kBQ - 1) / kBQ, num_heads, nb);
+    attn_wgmma_kernel<<<grid, 128, 0, stream>>>(qkv, out, cu_seqlens + b0, num_heads, window, scale_log2,
+                                                kv_lens ? kv_lens + b0 : nullptr);
+    SRB_CUDA_CHECK(cudaGetLastError());
+    note_launch();
+  }
   return 0;
 }
 

@@ -214,6 +214,18 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
 int precise_prepare(Model& m, std::string* err);
 int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers);
 void precise_free(Model& m);
+// The precise path's four row kernels, one launcher each (device pointers, asynchronous on s):
+// x [T, H] fp32 -> out [T, 3H] fp16 rows [hi | lo | hi], hi = fp16(v), lo = fp16(v - hi), v = x or (gamma non-null) the
+// no-bias LayerNorm (x - mean) rsqrt(var + eps) gamma
+int precise_split_rows(cudaStream_t s, const float* x, int T, int H, const float* gamma, float eps, __half* out);
+// rotate-half RoPE in place on the q and k thirds of qkv [T, 3 * heads * 64] fp32, row pos[t] of the [*, 32] tables
+int precise_rope(cudaStream_t s, float* qkv, const int* pos, int T, int heads, const float* cos_t, const float* sin_t);
+// out [T, I] = gelu_erf(a) * b over ab [T, 2I] fp32 (a = the first I columns, b = the last I)
+int precise_geglu(cudaStream_t s, const float* ab, int T, int I, float* out);
+// fp32 softmax(0.125 q k^T) v per head over packed qkv [T, 3 * heads * 64] -> out [T, heads * 64]; window 0: global,
+// else |i - j| <= window; any batch (slices of kMaxGridZ sequences)
+int precise_attention(cudaStream_t s, const float* qkv, float* out, const int* cu_seqlens, int batch, int max_len, int heads,
+                      int window);
 // Sequence classification with head `head`: writes ws.logits/probs [B,C], ws.cls, ws.conf.
 int head_sequence(Model& m, int head, const int* d_cu, int B, int pooler_mode);
 // Token classification with head `head`: writes ws.logits/probs [T,C], ws.cls [T], ws.conf [T].

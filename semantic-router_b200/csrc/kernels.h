@@ -13,6 +13,10 @@ void note_launch(int n = 1);
 bool pdl_enabled();
 long long launches_total();
 
+// Sequences one attention launch takes: they sit in gridDim.z, whose limit is 65 535; the attention launchers (here and in
+// precise.cu) run larger packs as slices of at most this many sequences.
+constexpr int kMaxGridZ = 65535;
+
 // ---- attention_wgmma.cu (wgmma flash attention, head dim 64, optional sliding window |i - j| <= window; every layer)
 // kv_lens [batch] (optional, global attention only): keys >= kv_lens[b] of sequence b are masked for EVERY query row while
 // all rows stay queries -- right-padded sequences whose pads are queries, as candle's BertModel sees them under a

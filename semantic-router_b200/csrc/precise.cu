@@ -84,6 +84,10 @@ __global__ void geglu_f32_kernel(const float* __restrict__ ab, int T, int I, flo
 
 // ---- fp32 softmax attention on the CUDA cores: one thread per query row, K / V tiles of 32 keys through shared memory,
 // online softmax per tile (expf).  window = 0: global; else |i - j| <= window.  Padding never exists (packed rows).
+// Each tile's weighted values are summed on their own and only then added to the running sums, o = o alpha + sum_j p_j v_j
+// (one fmaf per tile): every term passes through at most 32 + tiles roundings.  One chain over every key would pass the
+// first terms through n + n / 32 roundings, an error that grows linearly in n where the terms are correlated (constant
+// V columns, near-uniform scores): oracle/precise_oracle.py.
 constexpr int kARows = 64, kAKeys = 32;
 __global__ void __launch_bounds__(kARows)
 attention_f32_kernel(const float* __restrict__ qkv, float* __restrict__ out, const int* __restrict__ cu, int heads, int window,
@@ -130,15 +134,19 @@ attention_f32_kernel(const float* __restrict__ qkv, float* __restrict__ out, con
     if (tm == -INFINITY) continue;          // (uniform control flow is not required: no barrier inside)
     const float mn = fmaxf(m, tm);
     const float alpha = (m == -INFINITY) ? 0.f : expf(m - mn);
-    l *= alpha;
+    float lt = 0.f;
 #pragma unroll
-    for (int d = 0; d < 64; ++d) o[d] *= alpha;
+    for (int j = 0; j < kAKeys; ++j) {      // s[j] becomes the weight p_j
+      s[j] = (s[j] == -INFINITY) ? 0.f : expf(s[j] - mn);
+      lt += s[j];
+    }
+    l = fmaf(l, alpha, lt);
 #pragma unroll
-    for (int j = 0; j < kAKeys; ++j) {
-      const float p = (s[j] == -INFINITY) ? 0.f : expf(s[j] - mn);
-      l += p;
+    for (int d = 0; d < 64; ++d) {
+      float acc = 0.f;
 #pragma unroll
-      for (int d = 0; d < 64; ++d) o[d] = fmaf(p, vs[j][d], o[d]);
+      for (int j = 0; j < kAKeys; ++j) acc = fmaf(s[j], vs[j][d], acc);
+      o[d] = fmaf(o[d], alpha, acc);
     }
     m = mn;
   }
@@ -181,6 +189,44 @@ int grow(T*& p, size_t& cap, size_t n) {
 }
 
 }  // namespace
+
+int precise_split_rows(cudaStream_t s, const float* x, int T, int H, const float* gamma, float eps, __half* out) {
+  if (T <= 0) return 0;
+  const unsigned grid = static_cast<unsigned>((static_cast<size_t>(T) * 32 + 255) / 256);
+  if (gamma) split_rows_kernel<true><<<grid, 256, 0, s>>>(x, T, H, gamma, eps, out);
+  else split_rows_kernel<false><<<grid, 256, 0, s>>>(x, T, H, nullptr, 0.f, out);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int precise_rope(cudaStream_t s, float* qkv, const int* pos, int T, int heads, const float* cos_t, const float* sin_t) {
+  const size_t n = static_cast<size_t>(T) * 2 * heads * 32;
+  if (n == 0) return 0;
+  rope_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(qkv, pos, T, heads, cos_t, sin_t);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int precise_geglu(cudaStream_t s, const float* ab, int T, int I, float* out) {
+  const size_t n = static_cast<size_t>(T) * I;
+  if (n == 0) return 0;
+  geglu_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(ab, T, I, out);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int precise_attention(cudaStream_t s, const float* qkv, float* out, const int* cu_seqlens, int batch, int max_len, int heads,
+                      int window) {
+  if (batch <= 0 || max_len <= 0) return 0;
+  // gridDim.z holds at most 65 535 sequences: larger packs run as slices (the kernel reads absolute offsets from cu)
+  for (int b0 = 0; b0 < batch; b0 += kMaxGridZ) {
+    const int nb = batch - b0 < kMaxGridZ ? batch - b0 : kMaxGridZ;
+    const dim3 grid((max_len + kARows - 1) / kARows, heads, nb);
+    attention_f32_kernel<<<grid, kARows, 0, s>>>(qkv, out, cu_seqlens + b0, heads, window, 0.125f);
+    SRB_CUDA_CHECK(cudaGetLastError());
+  }
+  return 0;
+}
 
 int precise_prepare(Model& m, std::string* err) {
   if (m.cfg.arch != ARCH_MODERNBERT) { *err = "the precise path covers ModernBERT / mmBERT encoders"; return -1; }
@@ -230,7 +276,6 @@ int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, 
   if (compute_positions(s, d_cu, B, w.pos)) return -1;
   const TaskTensors& task = m.task[0];
   if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, task.emb_word, task.emb_ln_w, c.ln_eps, w.x, w.h)) return -1;
-  const int rows_grid = (T * 32 + 255) / 256;
   auto gemm = [&](const __half* a, const __half* wt, int n, int k, float* out, bool resid) {
     GemmDesc g;
     g.M = T; g.a_rows = static_cast<int>(Tp); g.N = n; g.K = 3 * k; g.A = a; g.W = wt; g.out = out; g.ldo = n;
@@ -244,28 +289,17 @@ int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, 
     const PreciseLayer& pl = p.layers[li];
     const bool local = (li % c.global_every) != 0;
     // attention input: LayerNorm (none on layer 0, modernbert.rs:266-271), split
-    if (norms.attn_w) split_rows_kernel<true><<<rows_grid, 256, 0, s>>>(w.x, T, H, norms.attn_w, c.ln_eps, p.split);
-    else split_rows_kernel<false><<<rows_grid, 256, 0, s>>>(w.x, T, H, nullptr, 0.f, p.split);
+    if (precise_split_rows(s, w.x, T, H, norms.attn_w, c.ln_eps, p.split)) return -1;
     if (gemm(p.split, pl.wqkv, 3 * H, H, p.qkv32, false)) return -1;
-    {
-      const size_t n = static_cast<size_t>(T) * 2 * c.heads * 32;
-      rope_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(p.qkv32, w.pos, T, c.heads,
-                                                                            local ? m.rope_cos_l : m.rope_cos_g,
-                                                                            local ? m.rope_sin_l : m.rope_sin_g);
-    }
-    {
-      const dim3 grid((max_len + kARows - 1) / kARows, c.heads, B);
-      attention_f32_kernel<<<grid, kARows, 0, s>>>(p.qkv32, p.ctx32, d_cu, c.heads, local ? c.local_attention / 2 : 0, 0.125f);
-    }
-    split_rows_kernel<false><<<rows_grid, 256, 0, s>>>(p.ctx32, T, H, nullptr, 0.f, p.split);
+    if (precise_rope(s, p.qkv32, w.pos, T, c.heads, local ? m.rope_cos_l : m.rope_cos_g, local ? m.rope_sin_l : m.rope_sin_g))
+      return -1;
+    if (precise_attention(s, p.qkv32, p.ctx32, d_cu, B, max_len, c.heads, local ? c.local_attention / 2 : 0)) return -1;
+    if (precise_split_rows(s, p.ctx32, T, H, nullptr, 0.f, p.split)) return -1;
     if (gemm(p.split, pl.wo, H, H, w.x, true)) return -1;
-    split_rows_kernel<true><<<rows_grid, 256, 0, s>>>(w.x, T, H, norms.mid_w, c.ln_eps, p.split);
+    if (precise_split_rows(s, w.x, T, H, norms.mid_w, c.ln_eps, p.split)) return -1;
     if (gemm(p.split, pl.wi, 2 * I, H, p.mid32, false)) return -1;
-    {
-      const size_t n = static_cast<size_t>(T) * I;
-      geglu_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(p.mid32, T, I, p.act32);
-    }
-    split_rows_kernel<false><<<rows_grid, 256, 0, s>>>(p.act32, T, I, nullptr, 0.f, p.split);
+    if (precise_geglu(s, p.mid32, T, I, p.act32)) return -1;
+    if (precise_split_rows(s, p.act32, T, I, nullptr, 0.f, p.split)) return -1;
     if (gemm(p.split, pl.wo2, H, I, w.x, true)) return -1;
     note_launch(7);
   }

@@ -79,7 +79,7 @@ def _long_case(srlib, name, cfg, w, seqs, depths, paths=tuple(PATHS)):
 ])
 def test_mmbert_long_sequence(srlib, cuda, S, max_pos, family):
     """One sequence up to max_position_embeddings: rope rows and windows at every far position, global layers over all keys
-    (the precise path's attention sums every key of a row in one fp32 chain)"""
+    (the precise path's attention sums each 32-key tile and then adds it to the running sums of the row)"""
     cfg = _mmbert(max_pos)
     seqs = synth.make_ids(np.random.default_rng(S + 31), [S], cfg.vocab_size)
     _long_case(srlib, f"mmBERT {family} S {S} (max_position_embeddings {max_pos})", cfg, ho.modernbert_weights(cfg, family),
