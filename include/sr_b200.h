@@ -49,12 +49,16 @@ SR_API int sr_head_num_classes(const sr_model* m, int head);
  * always, tanh GELU, LayerNorm eps 1e-12, first max).  1: the HF graph an ONNX export carries, which onnx-binding
  * runs (mmbert_classifier.rs:796-830 -- pooling per config "classifier_pooling", erf GELU, eps = norm_eps, last max). */
 SR_API int sr_model_set_head_flavor(sr_model* m, int flavor);
-/* Encoder arithmetic of a ModernBERT / mmBERT model.  0 (default): the production path -- fp16 operands on the tensor cores,
- * fp32 accumulation, residual stream and statistics (logits of the x8-scaled synthetic heads within ~3e-4 RELATIVE of the
+/* Encoder arithmetic of a model.  0 (default): the production path -- fp16 operands on the tensor cores, fp32
+ * accumulation, residual stream and statistics (logits of the x8-scaled synthetic heads within ~3e-4 RELATIVE of the
  * fp32 reference).  1: the "precise" path -- every GEMM operand as an fp16 hi + lo pair (three wgmma passes in one GEMM of
  * triple depth, fp32-equivalent products), fp32 LayerNorm / RoPE / GeGLU / attention in between: logits and embeddings
- * within the 1e-3 ABSOLUTE bound of BASELINE's north star, at about five times the cost.  Parity mode, not a serving mode.
- * Returns -1 for other architectures. */
+ * within the 1e-3 ABSOLUTE bound of BASELINE's north star, at several times the cost.  Parity mode, not a serving mode.
+ * ModernBERT / mmBERT and BERT / MiniLM encoders: for BERT the post-LN layers run with fp32 biases added in the GEMM
+ * epilogue, fp32 erf GELU and fp32 attention over the model's own heads (64, or MiniLM's 32: no zero-padded heads), and
+ * every entry that runs the encoder (sr_classify_ids under both pooler modes, sr_classify_tokens_ids,
+ * sr_classify_multi_ids, sr_embed_ids, sr_embed_ids_padded with its key lengths) takes it.  Returns -1 for grouped
+ * models (sr_model_load_grouped / sr_model_load_lora_shared). */
 SR_API int sr_model_set_precise(sr_model* m, int on);
 
 /* ---- host-buffer entries (synchronous; H2D of ids and D2H of results inside the call) ---------------- */

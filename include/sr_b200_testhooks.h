@@ -93,6 +93,13 @@ SR_API int sr_test_precise_geglu(const float* ab, int t, int i, float* out);
 /* fp32 attention over packed qkv [T, 3 * heads * 64] -> out [T, heads * 64]; window 0 = global */
 SR_API int sr_test_precise_attention(const float* qkv, float* out, const int32_t* cu_seqlens, int batch, int max_len,
                                      int heads, int window);
+/* the same over heads of head_dim 32 or 64 (qkv [T, 3 * heads * head_dim] -> out [T, heads * head_dim], scores scaled by
+ * head_dim^-1/2); kv_lens [batch] or null (global attention only): keys >= kv_lens[b] are masked for every query row of
+ * sequence b, and every row stays a query */
+SR_API int sr_test_precise_attention_kv(const float* qkv, float* out, const int32_t* cu_seqlens, int batch, int max_len,
+                                        int heads, int head_dim, int window, const int32_t* kv_lens);
+/* x = gelu_erf(x) in place over fp32 [t, i] */
+SR_API int sr_test_precise_gelu(float* x, int t, int i);
 SR_API int sr_test_layernorm(const float* x, int t, int h, const float* w, const float* b, float eps, float* y32,
                       void* y16);
 

@@ -143,6 +143,8 @@ def hooks():
         H.sr_test_precise_rope.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp]
         H.sr_test_precise_geglu.argtypes = [vp, C.c_int, C.c_int, vp]
         H.sr_test_precise_attention.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
+        H.sr_test_precise_attention_kv.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+        H.sr_test_precise_gelu.argtypes = [vp, C.c_int, C.c_int]
         H.sr_test_hl_to_f32.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
         H.sr_test_cache_plan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
         ci, cf = C.c_int, C.c_float

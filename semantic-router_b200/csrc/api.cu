@@ -620,8 +620,13 @@ int sr_test_precise_rope(float* qkv, const int32_t* pos, int t, int heads, const
 }
 int sr_test_precise_geglu(const float* ab, int t, int i, float* out) { return precise_geglu(nullptr, ab, t, i, out); }
 int sr_test_precise_attention(const float* qkv, float* out, const int32_t* cu, int batch, int max_len, int heads, int window) {
-  return precise_attention(nullptr, qkv, out, cu, batch, max_len, heads, window);
+  return precise_attention(nullptr, qkv, out, cu, batch, max_len, heads, 64, window);
 }
+int sr_test_precise_attention_kv(const float* qkv, float* out, const int32_t* cu, int batch, int max_len, int heads, int head_dim,
+                                 int window, const int32_t* kv_lens) {
+  return precise_attention(nullptr, qkv, out, cu, batch, max_len, heads, head_dim, window, kv_lens);
+}
+int sr_test_precise_gelu(float* x, int t, int i) { return precise_gelu(nullptr, x, t, i); }
 int sr_test_layernorm(const float* x, int t, int hdim, const float* w, const float* b, float eps, float* y32, void* y16) {
   return layernorm_rows(nullptr, x, t, hdim, w, b, eps, y32, static_cast<__half*>(y16));
 }

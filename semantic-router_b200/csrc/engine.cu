@@ -901,19 +901,21 @@ int checkpoint_has_adapters(const std::string& dir) {
 }
 
 bool read_source_projections(Model& m, std::string* err,
-                             const std::function<bool(int li, int p, const std::vector<float>& w, int N, int K)>& fn) {
+                             const std::function<bool(int li, int p, const std::vector<float>& w,
+                                                      const std::vector<float>& bias, int N, int K)>& fn) {
   SafeTensors st;
   if (!st.open(m.dir + "/model.safetensors", err)) return false;
   Loader ld{&m, &st};
   ld.lora_alpha = lora_alpha_of(m.dir);
   std::string P;
   tensor_prefix(st, m.cfg.arch, P);
-  std::vector<float> w;
+  std::vector<float> w, b;
   for (int li = 0; li < m.cfg.L; ++li) {
     const auto pr = layer_projections(m.cfg, P, li, m.task[0].layers[li].attn_w != nullptr);
     for (int p = 0; p < 4; ++p) {
-      if (!read_projection(ld, pr[p], w, nullptr)) { *err = ld.err; return false; }
-      if (!fn(li, p, w, pr[p].N, pr[p].K)) return false;
+      b.clear();
+      if (!read_projection(ld, pr[p], w, pr[p].bias ? &b : nullptr)) { *err = ld.err; return false; }
+      if (!fn(li, p, w, b, pr[p].N, pr[p].K)) return false;
     }
   }
   return true;

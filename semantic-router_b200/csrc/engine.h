@@ -112,12 +112,14 @@ struct Profiler {
   int count[PC_COUNT] = {0};
 };
 
-// "Precise" path (precise.cu): split-fp16 weights [W_hi | W_hi | W_lo] per projection and fp32 intermediates.
+// "Precise" path (precise.cu): split-fp16 weights [W_hi | W_hi | W_lo] per projection, in source order (BERT / MiniLM:
+// no padded heads, no scaled query rows), their fp32 biases (BERT; null for ModernBERT) and fp32 intermediates.
 struct PreciseLayer {
   __half* wqkv = nullptr;   // [3H, 3H]
   __half* wo = nullptr;     // [H, 3H]
-  __half* wi = nullptr;     // [2I, 3H] (original row order: a rows, then b rows)
+  __half* wi = nullptr;     // ModernBERT [2I, 3H] (original row order: a rows, then b rows) / BERT [I, 3H]
   __half* wo2 = nullptr;    // [H, 3I]
+  float *bqkv = nullptr, *bo = nullptr, *bi = nullptr, *bo2 = nullptr;
 };
 struct PreciseState {
   bool on = false;
@@ -125,8 +127,8 @@ struct PreciseState {
   __half* split = nullptr;  // [T, 3 * max(H, I)]  A operand [hi | lo | hi]
   float* qkv32 = nullptr;   // [T, 3H]
   float* ctx32 = nullptr;   // [T, H]
-  float* mid32 = nullptr;   // [T, 2I]
-  float* act32 = nullptr;   // [T, I]
+  float* mid32 = nullptr;   // ModernBERT [T, 2I] / BERT [T, I]
+  float* act32 = nullptr;   // ModernBERT [T, I]
   size_t split_cap = 0, qkv_cap = 0, ctx_cap = 0, mid_cap = 0, act_cap = 0;
 };
 
@@ -195,10 +197,11 @@ Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::v
                               std::string* err);
 int checkpoint_has_adapters(const std::string& dir);
 // Opens <m.dir>/model.safetensors afresh and passes every layer's four projections (qkv, attention output, intermediate,
-// output) to fn as source-order fp32 [N, K] host weights, adapters merged as model_load merges them.  fn returning false
-// stops the walk (and leaves *err to fn).
+// output) to fn as source-order fp32 [N, K] host weights, adapters merged as model_load merges them, with their
+// source-order [N] biases (BERT; empty for ModernBERT).  fn returning false stops the walk (and leaves *err to fn).
 bool read_source_projections(Model& m, std::string* err,
-                             const std::function<bool(int li, int p, const std::vector<float>& w, int N, int K)>& fn);
+                             const std::function<bool(int li, int p, const std::vector<float>& w,
+                                                      const std::vector<float>& bias, int N, int K)>& fn);
 int model_add_head(Model* m, const std::string& dir, int force_token_level, std::string* err);
 void model_free(Model* m);
 
@@ -214,7 +217,7 @@ int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, i
 int precise_prepare(Model& m, std::string* err);
 int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers);
 void precise_free(Model& m);
-// The precise path's four row kernels, one launcher each (device pointers, asynchronous on s):
+// The precise path's row kernels, one launcher each (device pointers, asynchronous on s):
 // x [T, H] fp32 -> out [T, 3H] fp16 rows [hi | lo | hi], hi = fp16(v), lo = fp16(v - hi), v = x or (gamma non-null) the
 // no-bias LayerNorm (x - mean) rsqrt(var + eps) gamma
 int precise_split_rows(cudaStream_t s, const float* x, int T, int H, const float* gamma, float eps, __half* out);
@@ -222,10 +225,14 @@ int precise_split_rows(cudaStream_t s, const float* x, int T, int H, const float
 int precise_rope(cudaStream_t s, float* qkv, const int* pos, int T, int heads, const float* cos_t, const float* sin_t);
 // out [T, I] = gelu_erf(a) * b over ab [T, 2I] fp32 (a = the first I columns, b = the last I)
 int precise_geglu(cudaStream_t s, const float* ab, int T, int I, float* out);
-// fp32 softmax(0.125 q k^T) v per head over packed qkv [T, 3 * heads * 64] -> out [T, heads * 64]; window 0: global,
-// else |i - j| <= window; any batch (slices of kMaxGridZ sequences)
+// x = gelu_erf(x) in place over fp32 [T, I]
+int precise_gelu(cudaStream_t s, float* x, int T, int I);
+// fp32 softmax(D^-1/2 q k^T) v per head of D = head_dim (32 or 64) over packed qkv [T, 3 * heads * D] -> out
+// [T, heads * D]; window 0: global, else |i - j| <= window; kv_lens [batch] (optional, global attention only): keys
+// >= kv_lens[b] of sequence b are masked for every query row while all rows stay queries (attention_wgmma_fwd's kv_lens);
+// any batch (slices of kMaxGridZ sequences)
 int precise_attention(cudaStream_t s, const float* qkv, float* out, const int* cu_seqlens, int batch, int max_len, int heads,
-                      int window);
+                      int head_dim, int window, const int* kv_lens = nullptr);
 // Sequence classification with head `head`: writes ws.logits/probs [B,C], ws.cls, ws.conf.
 int head_sequence(Model& m, int head, const int* d_cu, int B, int pooler_mode);
 // Token classification with head `head`: writes ws.logits/probs [T,C], ws.cls [T], ws.conf [T].

@@ -1,4 +1,4 @@
-// "Precise" encoder path (ModernBERT / mmBERT): fp32-equivalent arithmetic on the same wgmma GEMM, for the strict
+// "Precise" encoder path (ModernBERT / mmBERT, BERT / MiniLM): fp32-equivalent arithmetic on the same wgmma GEMM, for the strict
 // parity bound BASELINE's north star states ("logits and embeddings within 1e-3 fp32").
 //
 // The production path multiplies fp16 operands (2^-11 relative rounding of every activation and weight, fp16 q / k / v /
@@ -10,11 +10,12 @@
 //
 // and runs it as ONE wgmma GEMM of three times the depth: A' = [A_hi | A_lo | A_hi] (K' = 3K), W' = [W_hi | W_hi | W_lo].
 // fp16 x fp16 products are exact in fp32 and the accumulator is fp32 in registers, so the result carries fp32-accumulation
-// error only.  Everything between the GEMMs is plain fp32 (LayerNorm, RoPE, GeGLU with erff, softmax attention on the CUDA
-// cores with expf): nothing is rounded to fp16 except through the split.  ~5x the time of the production path; selected
+// error only.  Everything between the GEMMs is plain fp32 (LayerNorm, RoPE, GeGLU / GELU with erff, softmax attention on the
+// CUDA cores with expf, heads of 64 or MiniLM's 32): nothing is rounded to fp16 except through the split.  ~5x the time of the production path; selected
 // per model with sr_model_set_precise() -- it exists for parity, not for serving.
 //
-// Replaces the same reference code as engine.cu's encoder_forward (candle_models/modernbert.rs:61-86,121-213,234-240,283-305).
+// Replaces the same reference code as engine.cu's encoder_forward (candle_models/modernbert.rs:61-86,121-213,234-240,283-305;
+// candle-transformers bert.rs for BERT, whose biases the GEMM epilogue adds in fp32).
 #include <cuda_fp16.h>
 
 #include <cmath>
@@ -82,39 +83,51 @@ __global__ void geglu_f32_kernel(const float* __restrict__ ab, int T, int I, flo
   out[i] = 0.5f * a * (1.0f + erff(a * 0.70710678118654752440f)) * b;
 }
 
+// ---- gelu_erf in place over fp32 [T, I] (BERT's HiddenAct::Gelu; the GEMM has added the bias)
+__global__ void gelu_f32_kernel(float* __restrict__ x, size_t n) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float a = x[i];
+  x[i] = 0.5f * a * (1.0f + erff(a * 0.70710678118654752440f));
+}
+
 // ---- fp32 softmax attention on the CUDA cores: one thread per query row, K / V tiles of 32 keys through shared memory,
-// online softmax per tile (expf).  window = 0: global; else |i - j| <= window.  Padding never exists (packed rows).
+// online softmax per tile (expf).  Heads of D = 32 or 64: qkv rows [T, 3 heads D], out rows [T, heads D], scores scaled
+// by D^-1/2 on q.  window = 0: global, keys j < kv_lens[b] (kv_lens null: the whole sequence; every row stays a query);
+// else |i - j| <= window.
 // Each tile's weighted values are summed on their own and only then added to the running sums, o = o alpha + sum_j p_j v_j
 // (one fmaf per tile): every term passes through at most 32 + tiles roundings.  One chain over every key would pass the
 // first terms through n + n / 32 roundings, an error that grows linearly in n where the terms are correlated (constant
 // V columns, near-uniform scores): oracle/precise_oracle.py.
 constexpr int kARows = 64, kAKeys = 32;
+template <int D>
 __global__ void __launch_bounds__(kARows)
 attention_f32_kernel(const float* __restrict__ qkv, float* __restrict__ out, const int* __restrict__ cu, int heads, int window,
-                     float scale) {
-  __shared__ float ks[kAKeys][64], vs[kAKeys][64];
+                     float scale, const int* __restrict__ kv_lens) {
+  __shared__ float ks[kAKeys][D], vs[kAKeys][D];
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * kARows;
   const int seq0 = cu[b], len = cu[b + 1] - seq0;
   if (q0 >= len) return;
-  const int H = heads * 64;
+  const int klen = kv_lens ? min(len, kv_lens[b]) : len;   // keys >= klen are invisible to every query row
+  const int H = heads * D;
   const int qi = q0 + threadIdx.x;
   const bool live = qi < len;
-  float q[64], o[64];
-  const float* qp = qkv + static_cast<size_t>(seq0 + (live ? qi : q0)) * 3 * H + h * 64;
+  float q[D], o[D];
+  const float* qp = qkv + static_cast<size_t>(seq0 + (live ? qi : q0)) * 3 * H + h * D;
 #pragma unroll
-  for (int d = 0; d < 64; ++d) { q[d] = qp[d] * scale; o[d] = 0.f; }
+  for (int d = 0; d < D; ++d) { q[d] = qp[d] * scale; o[d] = 0.f; }
   float m = -INFINITY, l = 0.f;
-  int k_lo = 0, k_hi = len;
+  int k_lo = 0, k_hi = klen;
   if (window > 0) {
     k_lo = q0 - window > 0 ? q0 - window : 0;
     k_hi = q0 + kARows - 1 + window + 1 < len ? q0 + kARows + window : len;
   }
   for (int k0 = k_lo; k0 < k_hi; k0 += kAKeys) {
     __syncthreads();
-    for (int e = threadIdx.x; e < kAKeys * 64; e += kARows) {
-      const int j = e >> 6, d = e & 63;
-      const bool ok = k0 + j < len;
-      const float* base = qkv + static_cast<size_t>(seq0 + (ok ? k0 + j : 0)) * 3 * H + h * 64 + d;
+    for (int e = threadIdx.x; e < kAKeys * D; e += kARows) {
+      const int j = e / D, d = e % D;
+      const bool ok = k0 + j < klen;
+      const float* base = qkv + static_cast<size_t>(seq0 + (ok ? k0 + j : 0)) * 3 * H + h * D + d;
       ks[j][d] = ok ? base[H] : 0.f;
       vs[j][d] = ok ? base[2 * H] : 0.f;
     }
@@ -125,9 +138,9 @@ attention_f32_kernel(const float* __restrict__ qkv, float* __restrict__ out, con
     for (int j = 0; j < kAKeys; ++j) {
       float acc = 0.f;
 #pragma unroll
-      for (int d = 0; d < 64; ++d) acc = fmaf(q[d], ks[j][d], acc);
+      for (int d = 0; d < D; ++d) acc = fmaf(q[d], ks[j][d], acc);
       const int kj = k0 + j;
-      const bool vis = live && kj < len && (window == 0 || (kj - qi <= window && qi - kj <= window));
+      const bool vis = live && kj < klen && (window == 0 || (kj - qi <= window && qi - kj <= window));
       s[j] = vis ? acc : -INFINITY;
       tm = fmaxf(tm, s[j]);
     }
@@ -142,7 +155,7 @@ attention_f32_kernel(const float* __restrict__ qkv, float* __restrict__ out, con
     }
     l = fmaf(l, alpha, lt);
 #pragma unroll
-    for (int d = 0; d < 64; ++d) {
+    for (int d = 0; d < D; ++d) {
       float acc = 0.f;
 #pragma unroll
       for (int j = 0; j < kAKeys; ++j) acc = fmaf(s[j], vs[j][d], acc);
@@ -151,10 +164,10 @@ attention_f32_kernel(const float* __restrict__ qkv, float* __restrict__ out, con
     m = mn;
   }
   if (live) {
-    float* op = out + static_cast<size_t>(seq0 + qi) * H + h * 64;
+    float* op = out + static_cast<size_t>(seq0 + qi) * H + h * D;
     const float inv = 1.0f / l;
 #pragma unroll
-    for (int d = 0; d < 64; ++d) op[d] = o[d] * inv;
+    for (int d = 0; d < D; ++d) op[d] = o[d] * inv;
   }
 }
 
@@ -174,6 +187,14 @@ __half* split_weight(Model& m, const std::vector<float>& w, int n, int k) {
   if (cudaMalloc(reinterpret_cast<void**>(&d), h.size() * 2) != cudaSuccess) return nullptr;
   m.allocs.push_back(d);
   if (cudaMemcpy(d, h.data(), h.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
+  return d;
+}
+
+float* upload_f32(Model& m, const std::vector<float>& v) {
+  float* d = nullptr;
+  if (cudaMalloc(reinterpret_cast<void**>(&d), v.size() * 4) != cudaSuccess) return nullptr;
+  m.allocs.push_back(d);
+  if (cudaMemcpy(d, v.data(), v.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
   return d;
 }
 
@@ -215,30 +236,55 @@ int precise_geglu(cudaStream_t s, const float* ab, int T, int I, float* out) {
   return 0;
 }
 
+int precise_gelu(cudaStream_t s, float* x, int T, int I) {
+  const size_t n = static_cast<size_t>(T) * I;
+  if (n == 0) return 0;
+  gelu_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(x, n);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
 int precise_attention(cudaStream_t s, const float* qkv, float* out, const int* cu_seqlens, int batch, int max_len, int heads,
-                      int window) {
+                      int head_dim, int window, const int* kv_lens) {
+  if (head_dim != 32 && head_dim != 64) {
+    fprintf(stderr, "[srb200] precise_attention: head_dim %d (32 or 64)\n", head_dim);
+    return -1;
+  }
+  if (kv_lens && window > 0) {
+    fprintf(stderr, "[srb200] precise_attention: kv_lens applies to global attention only\n");
+    return -1;
+  }
   if (batch <= 0 || max_len <= 0) return 0;
+  // D^-1/2: 0.125 exactly for D = 64, fp32(32^-1/2) for D = 32
+  const float scale = head_dim == 64 ? 0.125f : 0.17677669529663688110f;
   // gridDim.z holds at most 65 535 sequences: larger packs run as slices (the kernel reads absolute offsets from cu)
   for (int b0 = 0; b0 < batch; b0 += kMaxGridZ) {
     const int nb = batch - b0 < kMaxGridZ ? batch - b0 : kMaxGridZ;
     const dim3 grid((max_len + kARows - 1) / kARows, heads, nb);
-    attention_f32_kernel<<<grid, kARows, 0, s>>>(qkv, out, cu_seqlens + b0, heads, window, 0.125f);
+    const int* kl = kv_lens ? kv_lens + b0 : nullptr;
+    if (head_dim == 64) attention_f32_kernel<64><<<grid, kARows, 0, s>>>(qkv, out, cu_seqlens + b0, heads, window, scale, kl);
+    else attention_f32_kernel<32><<<grid, kARows, 0, s>>>(qkv, out, cu_seqlens + b0, heads, window, scale, kl);
     SRB_CUDA_CHECK(cudaGetLastError());
   }
   return 0;
 }
 
 int precise_prepare(Model& m, std::string* err) {
-  if (m.cfg.arch != ARCH_MODERNBERT) { *err = "the precise path covers ModernBERT / mmBERT encoders"; return -1; }
   if (!m.precise.layers.empty()) return 0;
   if (cudaSetDevice(m.device) != cudaSuccess) { *err = "cudaSetDevice failed"; return -1; }
   std::vector<PreciseLayer> layers(m.cfg.L);
-  const bool ok = read_source_projections(m, err, [&](int li, int p, const std::vector<float>& w, int n, int k) {
+  const bool ok = read_source_projections(m, err, [&](int li, int p, const std::vector<float>& w, const std::vector<float>& b,
+                                                      int n, int k) {
     PreciseLayer& pl = layers[li];
     __half** slot[] = {&pl.wqkv, &pl.wo, &pl.wi, &pl.wo2};
+    float** bias[] = {&pl.bqkv, &pl.bo, &pl.bi, &pl.bo2};
     *slot[p] = split_weight(m, w, n, k);
-    if (!*slot[p]) *err = "allocation of the split weights failed";
-    return *slot[p] != nullptr;
+    if (*slot[p] && !b.empty()) *bias[p] = upload_f32(m, b);
+    if (!*slot[p] || (!b.empty() && !*bias[p])) {
+      *err = "allocation of the split weights failed";
+      return false;
+    }
+    return true;
   });
   if (!ok) return -1;
   m.precise.layers.swap(layers);
@@ -261,46 +307,76 @@ int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, 
   PreciseState& p = m.precise;
   cudaStream_t s = m.stream;
   const int H = c.H, I = c.I;
+  const bool bert = c.arch == ARCH_BERT;
   if (p.layers.empty() || T > w.cap_tokens || B > w.cap_seqs) return -1;
-  if (max_len > m.rope_len) {
-    fprintf(stderr, "[srb200] sequence length %d exceeds max_position_embeddings %d\n", max_len, m.rope_len);
+  const int max_pos = bert ? c.max_pos : m.rope_len;
+  if (max_len > max_pos) {
+    fprintf(stderr, "[srb200] sequence length %d exceeds max_position_embeddings %d\n", max_len, max_pos);
     return -1;
   }
   const size_t Tp = (static_cast<size_t>(T) + 127) / 128 * 128;   // TMA boxes of 128 rows stay inside the allocations
   const int wide = I > H ? I : H;
   cudaStreamSynchronize(s);   // the buffers below may be regrown: nothing queued may still use the old ones
   if (grow(p.split, p.split_cap, Tp * 3 * wide) || grow(p.qkv32, p.qkv_cap, Tp * 3 * H) || grow(p.ctx32, p.ctx_cap, Tp * H) ||
-      grow(p.mid32, p.mid_cap, Tp * 2 * I) || grow(p.act32, p.act_cap, Tp * I))
+      grow(p.mid32, p.mid_cap, Tp * (bert ? 1 : 2) * I) || grow(p.act32, p.act_cap, bert ? 0 : Tp * I))
     return -1;
   const int L = (num_layers <= 0 || num_layers > c.L) ? c.L : num_layers;
   if (compute_positions(s, d_cu, B, w.pos)) return -1;
   const TaskTensors& task = m.task[0];
-  if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, task.emb_word, task.emb_ln_w, c.ln_eps, w.x, w.h)) return -1;
-  auto gemm = [&](const __half* a, const __half* wt, int n, int k, float* out, bool resid) {
+  // out = [out +] split(A) W'^T [+ bias] in fp32 (EPI_RESID; resid null: a plain store)
+  auto gemm = [&](const __half* a, const __half* wt, int n, int k, float* out, bool resid, const float* bias) {
     GemmDesc g;
     g.M = T; g.a_rows = static_cast<int>(Tp); g.N = n; g.K = 3 * k; g.A = a; g.W = wt; g.out = out; g.ldo = n;
     g.epi = EPI_RESID;
     g.resid = resid ? out : nullptr;
     g.ldr = n;
+    g.bias = bias;
     return gemm_f16(s, g);
   };
+  if (bert) {
+    // candle's post-LN BertLayer: x = LN(x + attn(x) Wo + bo), then x = LN(x + gelu(x Wi + bi) Wo2 + bo2)
+    if (embed_ln_bert(s, d_ids, w.pos, T, H, c.vocab, c.max_pos, task.emb_word, task.emb_pos, task.emb_type0, task.emb_ln_w,
+                      task.emb_ln_b, c.ln_eps, w.x, w.h))
+      return -1;
+    for (int li = 0; li < L; ++li) {
+      const TaskNorms& norms = task.layers[li];
+      const PreciseLayer& pl = p.layers[li];
+      if (precise_split_rows(s, w.x, T, H, nullptr, 0.f, p.split)) return -1;
+      if (gemm(p.split, pl.wqkv, 3 * H, H, p.qkv32, false, pl.bqkv)) return -1;
+      if (precise_attention(s, p.qkv32, p.ctx32, d_cu, B, max_len, c.heads, H / c.heads, 0, m.cur_kv_lens)) return -1;
+      if (precise_split_rows(s, p.ctx32, T, H, nullptr, 0.f, p.split)) return -1;
+      if (gemm(p.split, pl.wo, H, H, w.x, true, pl.bo)) return -1;
+      if (layernorm_rows(s, w.x, T, H, norms.mid_w, norms.mid_b, c.ln_eps, w.x, nullptr)) return -1;
+      if (precise_split_rows(s, w.x, T, H, nullptr, 0.f, p.split)) return -1;
+      if (gemm(p.split, pl.wi, I, H, p.mid32, false, pl.bi)) return -1;
+      if (precise_gelu(s, p.mid32, T, I)) return -1;
+      if (precise_split_rows(s, p.mid32, T, I, nullptr, 0.f, p.split)) return -1;
+      if (gemm(p.split, pl.wo2, H, I, w.x, true, pl.bo2)) return -1;
+      if (layernorm_rows(s, w.x, T, H, norms.out_w, norms.out_b, c.ln_eps, w.x, nullptr)) return -1;
+      note_launch(6);   // the split, attention and GELU launches (the GEMMs and LayerNorms count their own)
+    }
+    SRB_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  }
+  if (embed_ln_modernbert(s, d_ids, T, H, c.vocab, task.emb_word, task.emb_ln_w, c.ln_eps, w.x, w.h)) return -1;
   for (int li = 0; li < L; ++li) {
     const TaskNorms& norms = task.layers[li];
     const PreciseLayer& pl = p.layers[li];
     const bool local = (li % c.global_every) != 0;
     // attention input: LayerNorm (none on layer 0, modernbert.rs:266-271), split
     if (precise_split_rows(s, w.x, T, H, norms.attn_w, c.ln_eps, p.split)) return -1;
-    if (gemm(p.split, pl.wqkv, 3 * H, H, p.qkv32, false)) return -1;
+    if (gemm(p.split, pl.wqkv, 3 * H, H, p.qkv32, false, nullptr)) return -1;
     if (precise_rope(s, p.qkv32, w.pos, T, c.heads, local ? m.rope_cos_l : m.rope_cos_g, local ? m.rope_sin_l : m.rope_sin_g))
       return -1;
-    if (precise_attention(s, p.qkv32, p.ctx32, d_cu, B, max_len, c.heads, local ? c.local_attention / 2 : 0)) return -1;
+    if (precise_attention(s, p.qkv32, p.ctx32, d_cu, B, max_len, c.heads, 64, local ? c.local_attention / 2 : 0, nullptr))
+      return -1;
     if (precise_split_rows(s, p.ctx32, T, H, nullptr, 0.f, p.split)) return -1;
-    if (gemm(p.split, pl.wo, H, H, w.x, true)) return -1;
+    if (gemm(p.split, pl.wo, H, H, w.x, true, nullptr)) return -1;
     if (precise_split_rows(s, w.x, T, H, norms.mid_w, c.ln_eps, p.split)) return -1;
-    if (gemm(p.split, pl.wi, 2 * I, H, p.mid32, false)) return -1;
+    if (gemm(p.split, pl.wi, 2 * I, H, p.mid32, false, nullptr)) return -1;
     if (precise_geglu(s, p.mid32, T, I, p.act32)) return -1;
     if (precise_split_rows(s, p.act32, T, I, nullptr, 0.f, p.split)) return -1;
-    if (gemm(p.split, pl.wo2, H, I, w.x, true)) return -1;
+    if (gemm(p.split, pl.wo2, H, I, w.x, true, nullptr)) return -1;
     note_launch(7);
   }
   SRB_CUDA_CHECK(cudaGetLastError());
