@@ -490,6 +490,10 @@ int sr_model_set_precise(sr_model* h, int on) {
   }
   cudaStreamSynchronize(h->m->stream);
   h->m->precise.on = on != 0;
+  if (on && precise_reserve(*h->m)) {
+    h->m->precise.on = false;
+    return fail("sr_model_set_precise: workspace allocation failed");
+  }
   return 0;
 }
 

@@ -553,7 +553,6 @@ void store_projection(Loader& ld, const Projection& pr, int p, const std::vector
 // ModernBERT's rotary tables for both thetas, max_position_embeddings rows
 void load_rope(Loader& ld, Model& m) {
   const EncoderConfig& c = m.cfg;
-  m.rope_len = c.max_pos;
   std::vector<float> cs, sn;
   rope_tables(64, c.theta_global, c.max_pos, cs, sn);
   m.rope_cos_g = ld.up_f32(cs);
@@ -900,35 +899,55 @@ int checkpoint_has_adapters(const std::string& dir) {
   return 0;
 }
 
-bool read_source_projections(Model& m, std::string* err,
-                             const std::function<bool(int li, int p, const std::vector<float>& w,
-                                                      const std::vector<float>& bias, int N, int K)>& fn) {
+int precise_prepare(Model& m, std::string* err) {
+  if (!m.precise.layers.empty()) return 0;
+  if (cudaSetDevice(m.device) != cudaSuccess) { *err = "cudaSetDevice failed"; return -1; }
   SafeTensors st;
-  if (!st.open(m.dir + "/model.safetensors", err)) return false;
+  if (!st.open(m.dir + "/model.safetensors", err)) return -1;
   Loader ld{&m, &st};
   ld.lora_alpha = lora_alpha_of(m.dir);
   std::string P;
   tensor_prefix(st, m.cfg.arch, P);
-  std::vector<float> w, b;
-  for (int li = 0; li < m.cfg.L; ++li) {
+  const size_t loaded = m.weight_bytes;
+  std::vector<PreciseLayer> layers(m.cfg.L);
+  std::vector<float> w, b, split;
+  for (int li = 0; li < m.cfg.L && ld.ok; ++li) {
     const auto pr = layer_projections(m.cfg, P, li, m.task[0].layers[li].attn_w != nullptr);
-    for (int p = 0; p < 4; ++p) {
-      b.clear();
-      if (!read_projection(ld, pr[p], w, pr[p].bias ? &b : nullptr)) { *err = ld.err; return false; }
-      if (!fn(li, p, w, b, pr[p].N, pr[p].K)) return false;
+    PreciseLayer& pl = layers[li];
+    __half** slot[] = {&pl.wqkv, &pl.wo, &pl.wi, &pl.wo2};
+    float** bias[] = {&pl.bqkv, &pl.bo, &pl.bi, &pl.bo2};
+    for (int p = 0; p < 4 && ld.ok; ++p) {
+      if (!read_projection(ld, pr[p], w, pr[p].bias ? &b : nullptr)) break;
+      // W [N, K] -> [W_hi | W_hi | W_lo] [N, 3K], hi = fp16(w), lo = fp16(w - hi): both are fp16 values, which up_f16
+      // stores unchanged
+      const int n = pr[p].N, k = pr[p].K;
+      split.resize(static_cast<size_t>(n) * 3 * k);
+      for (int r = 0; r < n; ++r)
+        for (int c = 0; c < k; ++c) {
+          const float v = w[static_cast<size_t>(r) * k + c];
+          const float hi = __half2float(__float2half_rn(v));
+          float* o = split.data() + static_cast<size_t>(r) * 3 * k + c;
+          o[0] = o[k] = hi;
+          o[2 * k] = __half2float(__float2half_rn(v - hi));
+        }
+      *slot[p] = ld.up_f16(split);
+      if (pr[p].bias) *bias[p] = ld.up_f32(b);
     }
   }
-  return true;
+  m.weight_bytes = loaded;   // derived from the loaded weights, not loaded: sr_model_device_bytes leaves them out
+  if (!ld.ok) { *err = ld.err; return -1; }
+  m.precise.layers.swap(layers);
+  return 0;
 }
 
 void model_free(Model* m) {
   if (!m) return;
   cudaSetDevice(m->device);
   if (m->stream) { cudaStreamSynchronize(m->stream); cudaStreamDestroy(m->stream); }
-  precise_free(*m);
   for (void* p : m->allocs) cudaFree(p);
   Workspace& w = m->ws;
-  void* dev[] = {w.x, w.h, w.lo, w.qkv, w.ctx, w.mid, w.ids, w.pos, w.cu, w.pooled, w.pool_part, w.pool_arrived, w.logits, w.probs, w.cls, w.conf, w.emb, w.row_stats, w.kv_lens};
+  void* dev[] = {w.x, w.h, w.lo, w.qkv, w.ctx, w.mid, w.ids, w.pos, w.cu, w.pooled, w.pool_part, w.pool_arrived, w.logits,
+                 w.probs, w.cls, w.conf, w.emb, w.row_stats, w.kv_lens, w.split, w.qkv32, w.ctx32, w.mid32, w.act32};
   for (void* p : dev) if (p) cudaFree(p);
   void* host[] = {w.h_ids, w.h_cu, w.h_out, w.h_cls, w.h_conf};
   for (void* p : host) if (p) cudaFreeHost(p);
@@ -1018,7 +1037,25 @@ int workspace_reserve(Model& m, int tokens, int seqs, size_t out_elems) {
     rc |= regrow_host(w.h_out, 2 * want_out);
     w.h_out_elems = rc ? 0 : want_out;
   }
+  if (m.precise.on) rc |= precise_reserve(m);
   if (rc) fprintf(stderr, "[srb200] workspace allocation failed (tokens=%d seqs=%d)\n", tokens, seqs);
+  return rc;
+}
+
+int precise_reserve(Model& m) {
+  Workspace& w = m.ws;
+  if (w.cap_tokens <= w.cap_precise) return 0;
+  cudaStreamSynchronize(m.stream);
+  ++w.generation;
+  const size_t T = static_cast<size_t>(w.cap_tokens), H = m.cfg.H, I = m.cfg.I;
+  const bool bert = m.cfg.arch == ARCH_BERT;
+  int rc = regrow(w.split, T * 3 * std::max(H, I));
+  rc |= regrow(w.qkv32, T * 3 * H);
+  rc |= regrow(w.ctx32, T * H);
+  rc |= regrow(w.mid32, T * (bert ? 1 : 2) * I);
+  if (!bert) rc |= regrow(w.act32, T * I);
+  w.cap_precise = rc ? 0 : w.cap_tokens;
+  if (rc) w.cap_tokens = 0;
   return rc;
 }
 
@@ -1026,22 +1063,18 @@ int workspace_reserve(Model& m, int tokens, int seqs, size_t out_elems) {
 // forward
 // ------------------------------------------------------------------------------------------------
 int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers) {
-  if (m.precise.on) return encoder_forward_precise(m, d_ids, d_cu, B, T, max_len, num_layers);
   const EncoderConfig& c = m.cfg;
   Workspace& w = m.ws;
   cudaStream_t s = m.stream;
   const int H = c.H, I = c.I;
   if (T > w.cap_tokens || B > w.cap_seqs) return -1;
-  if (c.arch == ARCH_MODERNBERT && max_len > m.rope_len) {
-    fprintf(stderr, "[srb200] sequence length %d exceeds max_position_embeddings %d\n", max_len, m.rope_len);
-    return -1;
-  }
-  if (c.arch == ARCH_BERT && max_len > c.max_pos) {
+  if (max_len > c.max_pos) {   // BERT's position embeddings and ModernBERT's rotary tables have max_pos rows
     fprintf(stderr, "[srb200] sequence length %d exceeds max_position_embeddings %d\n", max_len, c.max_pos);
     return -1;
   }
   const int L = (num_layers <= 0 || num_layers > c.L) ? c.L : num_layers;
   if (compute_positions(s, d_cu, B, w.pos)) return -1;
+  if (m.precise.on) return encoder_forward_precise(m, d_ids, d_cu, B, T, max_len, L);
   GemmDesc g;
   g.M = T;
   g.a_rows = w.cap_tokens;

@@ -7,7 +7,6 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
-#include <functional>
 #include <map>
 #include <mutex>
 #include <string>
@@ -89,6 +88,13 @@ struct Workspace {
   float* conf = nullptr;
   float* emb = nullptr;     // [B,H]
   size_t out_elems = 0;
+  // precise path (precise.cu), sized for cap_tokens rows while Model::precise.on
+  int cap_precise = 0;      // rows the buffers below hold
+  __half* split = nullptr;  // [T, 3 * max(H, I)]  A operand [hi | lo | hi]
+  float* qkv32 = nullptr;   // [T, 3H]
+  float* ctx32 = nullptr;   // [T, H]
+  float* mid32 = nullptr;   // ModernBERT [T, 2I] / BERT [T, I]
+  float* act32 = nullptr;   // ModernBERT [T, I]
   // pinned host staging
   int* h_ids = nullptr;
   int* h_cu = nullptr;
@@ -113,7 +119,8 @@ struct Profiler {
 };
 
 // "Precise" path (precise.cu): split-fp16 weights [W_hi | W_hi | W_lo] per projection, in source order (BERT / MiniLM:
-// no padded heads, no scaled query rows), their fp32 biases (BERT; null for ModernBERT) and fp32 intermediates.
+// no padded heads, no scaled query rows) and their fp32 biases (BERT; null for ModernBERT).  Its fp32 intermediates are
+// workspace buffers (Workspace::split ... act32).
 struct PreciseLayer {
   __half* wqkv = nullptr;   // [3H, 3H]
   __half* wo = nullptr;     // [H, 3H]
@@ -124,12 +131,6 @@ struct PreciseLayer {
 struct PreciseState {
   bool on = false;
   std::vector<PreciseLayer> layers;
-  __half* split = nullptr;  // [T, 3 * max(H, I)]  A operand [hi | lo | hi]
-  float* qkv32 = nullptr;   // [T, 3H]
-  float* ctx32 = nullptr;   // [T, H]
-  float* mid32 = nullptr;   // ModernBERT [T, 2I] / BERT [T, I]
-  float* act32 = nullptr;   // ModernBERT [T, I]
-  size_t split_cap = 0, qkv_cap = 0, ctx_cap = 0, mid_cap = 0, act_cap = 0;
 };
 
 // Several task checkpoints of one encoder served in ONE pass (model_load_grouped): merged or fully fine-tuned
@@ -166,8 +167,7 @@ struct Model {
   std::string dir;
   std::vector<TaskTensors> task;   // at least one; task[0] outside a grouped pass
   std::vector<LayerWeights> layers;
-  float *rope_cos_g = nullptr, *rope_sin_g = nullptr, *rope_cos_l = nullptr, *rope_sin_l = nullptr;
-  int rope_len = 0;
+  float *rope_cos_g = nullptr, *rope_sin_g = nullptr, *rope_cos_l = nullptr, *rope_sin_l = nullptr;   // cfg.max_pos rows
   std::vector<Head> heads;
   // 0: candle semantics (MEAN pooling always, tanh GELU, eps 1e-12, first-max; traditional/modernbert.rs:303-329,818)
   // 1: HF / ONNX-export semantics (pooling per config, erf GELU, eps = norm_eps, last-max;
@@ -196,16 +196,16 @@ Model* model_load_grouped(const std::vector<std::string>& dirs, const std::vecto
 Model* model_load_lora_shared(const std::vector<std::string>& dirs, const std::vector<int>& token_level, int device,
                               std::string* err);
 int checkpoint_has_adapters(const std::string& dir);
-// Opens <m.dir>/model.safetensors afresh and passes every layer's four projections (qkv, attention output, intermediate,
-// output) to fn as source-order fp32 [N, K] host weights, adapters merged as model_load merges them, with their
-// source-order [N] biases (BERT; empty for ModernBERT).  fn returning false stops the walk (and leaves *err to fn).
-bool read_source_projections(Model& m, std::string* err,
-                             const std::function<bool(int li, int p, const std::vector<float>& w,
-                                                      const std::vector<float>& bias, int N, int K)>& fn);
+// The precise path's split weights (PreciseLayer), built once from <m.dir>/model.safetensors opened afresh: every layer's
+// four projections in source order, adapters merged as model_load merges them.  Not counted in m.weight_bytes.
+int precise_prepare(Model& m, std::string* err);
 int model_add_head(Model* m, const std::string& dir, int force_token_level, std::string* err);
 void model_free(Model* m);
 
 int workspace_reserve(Model& m, int tokens, int seqs, size_t out_elems);
+// The precise path's workspace buffers for ws.cap_tokens rows (workspace_reserve calls it while m.precise.on).  On
+// failure ws.cap_tokens drops to 0, so no forward runs until a reservation succeeds.
+int precise_reserve(Model& m);
 void profile_enable(Model& m, bool on);
 // synchronises the stream, folds the recorded event pairs into prof.ms / prof.count
 int profile_collect(Model& m);
@@ -213,11 +213,10 @@ int profile_collect(Model& m);
 // All of the following enqueue on m.stream and do NOT synchronise.
 // ids/cu are device pointers (int32); T = cu[B]; max_len = longest sequence.
 int encoder_forward(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers);
-// precise.cu: builds the split weights (read_source_projections), the fp32-equivalent forward, buffer release
-int precise_prepare(Model& m, std::string* err);
-int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers);
-void precise_free(Model& m);
-// The precise path's row kernels, one launcher each (device pointers, asynchronous on s):
+// precise.cu: encoder_forward's embedding and first L layers while m.precise.on (encoder_forward has checked the
+// capacity and the positions and computed ws.pos)
+int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int L);
+// The precise path's row kernels, one launcher each (device pointers, asynchronous on s; note_launch per launch):
 // x [T, H] fp32 -> out [T, 3H] fp16 rows [hi | lo | hi], hi = fp16(v), lo = fp16(v - hi), v = x or (gamma non-null) the
 // no-bias LayerNorm (x - mean) rsqrt(var + eps) gamma
 int precise_split_rows(cudaStream_t s, const float* x, int T, int H, const float* gamma, float eps, __half* out);

@@ -19,7 +19,6 @@
 #include <cuda_fp16.h>
 
 #include <cmath>
-#include <vector>
 
 #include "common.cuh"
 #include "engine.h"
@@ -97,7 +96,7 @@ __global__ void gelu_f32_kernel(float* __restrict__ x, size_t n) {
 // else |i - j| <= window.
 // Each tile's weighted values are summed on their own and only then added to the running sums, o = o alpha + sum_j p_j v_j
 // (one fmaf per tile): every term passes through at most 32 + tiles roundings.  One chain over every key would pass the
-// first terms through n + n / 32 roundings, an error that grows linearly in n where the terms are correlated (constant
+// first terms through n + n / 32 roundings, an error that increases linearly in n where the terms are correlated (constant
 // V columns, near-uniform scores): oracle/precise_oracle.py.
 constexpr int kARows = 64, kAKeys = 32;
 template <int D>
@@ -171,44 +170,6 @@ attention_f32_kernel(const float* __restrict__ qkv, float* __restrict__ out, con
   }
 }
 
-// W [N, K] fp32 -> [W_hi | W_hi | W_lo] fp16 [N, 3K]
-__half* split_weight(Model& m, const std::vector<float>& w, int n, int k) {
-  std::vector<__half> h(static_cast<size_t>(n) * 3 * k);
-  for (int r = 0; r < n; ++r)
-    for (int c = 0; c < k; ++c) {
-      const float v = w[static_cast<size_t>(r) * k + c];
-      const __half hi = __float2half_rn(v);
-      const __half lo = __float2half_rn(v - __half2float(hi));
-      h[static_cast<size_t>(r) * 3 * k + c] = hi;
-      h[static_cast<size_t>(r) * 3 * k + k + c] = hi;
-      h[static_cast<size_t>(r) * 3 * k + 2 * k + c] = lo;
-    }
-  __half* d = nullptr;
-  if (cudaMalloc(reinterpret_cast<void**>(&d), h.size() * 2) != cudaSuccess) return nullptr;
-  m.allocs.push_back(d);
-  if (cudaMemcpy(d, h.data(), h.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
-  return d;
-}
-
-float* upload_f32(Model& m, const std::vector<float>& v) {
-  float* d = nullptr;
-  if (cudaMalloc(reinterpret_cast<void**>(&d), v.size() * 4) != cudaSuccess) return nullptr;
-  m.allocs.push_back(d);
-  if (cudaMemcpy(d, v.data(), v.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
-  return d;
-}
-
-template <typename T>
-int grow(T*& p, size_t& cap, size_t n) {
-  if (n <= cap) return 0;
-  if (p) cudaFree(p);
-  p = nullptr;
-  cap = 0;
-  if (cudaMalloc(reinterpret_cast<void**>(&p), n * sizeof(T)) != cudaSuccess) return -1;
-  cap = n;
-  return 0;
-}
-
 }  // namespace
 
 int precise_split_rows(cudaStream_t s, const float* x, int T, int H, const float* gamma, float eps, __half* out) {
@@ -217,6 +178,7 @@ int precise_split_rows(cudaStream_t s, const float* x, int T, int H, const float
   if (gamma) split_rows_kernel<true><<<grid, 256, 0, s>>>(x, T, H, gamma, eps, out);
   else split_rows_kernel<false><<<grid, 256, 0, s>>>(x, T, H, nullptr, 0.f, out);
   SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
   return 0;
 }
 
@@ -225,6 +187,7 @@ int precise_rope(cudaStream_t s, float* qkv, const int* pos, int T, int heads, c
   if (n == 0) return 0;
   rope_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(qkv, pos, T, heads, cos_t, sin_t);
   SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
   return 0;
 }
 
@@ -233,6 +196,7 @@ int precise_geglu(cudaStream_t s, const float* ab, int T, int I, float* out) {
   if (n == 0) return 0;
   geglu_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(ab, T, I, out);
   SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
   return 0;
 }
 
@@ -241,6 +205,7 @@ int precise_gelu(cudaStream_t s, float* x, int T, int I) {
   if (n == 0) return 0;
   gelu_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(x, n);
   SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
   return 0;
 }
 
@@ -265,68 +230,23 @@ int precise_attention(cudaStream_t s, const float* qkv, float* out, const int* c
     if (head_dim == 64) attention_f32_kernel<64><<<grid, kARows, 0, s>>>(qkv, out, cu_seqlens + b0, heads, window, scale, kl);
     else attention_f32_kernel<32><<<grid, kARows, 0, s>>>(qkv, out, cu_seqlens + b0, heads, window, scale, kl);
     SRB_CUDA_CHECK(cudaGetLastError());
+    note_launch();
   }
   return 0;
 }
 
-int precise_prepare(Model& m, std::string* err) {
-  if (!m.precise.layers.empty()) return 0;
-  if (cudaSetDevice(m.device) != cudaSuccess) { *err = "cudaSetDevice failed"; return -1; }
-  std::vector<PreciseLayer> layers(m.cfg.L);
-  const bool ok = read_source_projections(m, err, [&](int li, int p, const std::vector<float>& w, const std::vector<float>& b,
-                                                      int n, int k) {
-    PreciseLayer& pl = layers[li];
-    __half** slot[] = {&pl.wqkv, &pl.wo, &pl.wi, &pl.wo2};
-    float** bias[] = {&pl.bqkv, &pl.bo, &pl.bi, &pl.bo2};
-    *slot[p] = split_weight(m, w, n, k);
-    if (*slot[p] && !b.empty()) *bias[p] = upload_f32(m, b);
-    if (!*slot[p] || (!b.empty() && !*bias[p])) {
-      *err = "allocation of the split weights failed";
-      return false;
-    }
-    return true;
-  });
-  if (!ok) return -1;
-  m.precise.layers.swap(layers);
-  return 0;
-}
-
-void precise_free(Model& m) {
-  PreciseState& p = m.precise;
-  if (p.split) cudaFree(p.split);
-  if (p.qkv32) cudaFree(p.qkv32);
-  if (p.ctx32) cudaFree(p.ctx32);
-  if (p.mid32) cudaFree(p.mid32);
-  if (p.act32) cudaFree(p.act32);
-  p = PreciseState();
-}
-
-int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int num_layers) {
+int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, int T, int max_len, int L) {
   const EncoderConfig& c = m.cfg;
   Workspace& w = m.ws;
   PreciseState& p = m.precise;
   cudaStream_t s = m.stream;
   const int H = c.H, I = c.I;
   const bool bert = c.arch == ARCH_BERT;
-  if (p.layers.empty() || T > w.cap_tokens || B > w.cap_seqs) return -1;
-  const int max_pos = bert ? c.max_pos : m.rope_len;
-  if (max_len > max_pos) {
-    fprintf(stderr, "[srb200] sequence length %d exceeds max_position_embeddings %d\n", max_len, max_pos);
-    return -1;
-  }
-  const size_t Tp = (static_cast<size_t>(T) + 127) / 128 * 128;   // TMA boxes of 128 rows stay inside the allocations
-  const int wide = I > H ? I : H;
-  cudaStreamSynchronize(s);   // the buffers below may be regrown: nothing queued may still use the old ones
-  if (grow(p.split, p.split_cap, Tp * 3 * wide) || grow(p.qkv32, p.qkv_cap, Tp * 3 * H) || grow(p.ctx32, p.ctx_cap, Tp * H) ||
-      grow(p.mid32, p.mid_cap, Tp * (bert ? 1 : 2) * I) || grow(p.act32, p.act_cap, bert ? 0 : Tp * I))
-    return -1;
-  const int L = (num_layers <= 0 || num_layers > c.L) ? c.L : num_layers;
-  if (compute_positions(s, d_cu, B, w.pos)) return -1;
   const TaskTensors& task = m.task[0];
   // out = [out +] split(A) W'^T [+ bias] in fp32 (EPI_RESID; resid null: a plain store)
   auto gemm = [&](const __half* a, const __half* wt, int n, int k, float* out, bool resid, const float* bias) {
     GemmDesc g;
-    g.M = T; g.a_rows = static_cast<int>(Tp); g.N = n; g.K = 3 * k; g.A = a; g.W = wt; g.out = out; g.ldo = n;
+    g.M = T; g.a_rows = w.cap_tokens; g.N = n; g.K = 3 * k; g.A = a; g.W = wt; g.out = out; g.ldo = n;
     g.epi = EPI_RESID;
     g.resid = resid ? out : nullptr;
     g.ldr = n;
@@ -341,19 +261,18 @@ int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, 
     for (int li = 0; li < L; ++li) {
       const TaskNorms& norms = task.layers[li];
       const PreciseLayer& pl = p.layers[li];
-      if (precise_split_rows(s, w.x, T, H, nullptr, 0.f, p.split)) return -1;
-      if (gemm(p.split, pl.wqkv, 3 * H, H, p.qkv32, false, pl.bqkv)) return -1;
-      if (precise_attention(s, p.qkv32, p.ctx32, d_cu, B, max_len, c.heads, H / c.heads, 0, m.cur_kv_lens)) return -1;
-      if (precise_split_rows(s, p.ctx32, T, H, nullptr, 0.f, p.split)) return -1;
-      if (gemm(p.split, pl.wo, H, H, w.x, true, pl.bo)) return -1;
+      if (precise_split_rows(s, w.x, T, H, nullptr, 0.f, w.split)) return -1;
+      if (gemm(w.split, pl.wqkv, 3 * H, H, w.qkv32, false, pl.bqkv)) return -1;
+      if (precise_attention(s, w.qkv32, w.ctx32, d_cu, B, max_len, c.heads, H / c.heads, 0, m.cur_kv_lens)) return -1;
+      if (precise_split_rows(s, w.ctx32, T, H, nullptr, 0.f, w.split)) return -1;
+      if (gemm(w.split, pl.wo, H, H, w.x, true, pl.bo)) return -1;
       if (layernorm_rows(s, w.x, T, H, norms.mid_w, norms.mid_b, c.ln_eps, w.x, nullptr)) return -1;
-      if (precise_split_rows(s, w.x, T, H, nullptr, 0.f, p.split)) return -1;
-      if (gemm(p.split, pl.wi, I, H, p.mid32, false, pl.bi)) return -1;
-      if (precise_gelu(s, p.mid32, T, I)) return -1;
-      if (precise_split_rows(s, p.mid32, T, I, nullptr, 0.f, p.split)) return -1;
-      if (gemm(p.split, pl.wo2, H, I, w.x, true, pl.bo2)) return -1;
+      if (precise_split_rows(s, w.x, T, H, nullptr, 0.f, w.split)) return -1;
+      if (gemm(w.split, pl.wi, I, H, w.mid32, false, pl.bi)) return -1;
+      if (precise_gelu(s, w.mid32, T, I)) return -1;
+      if (precise_split_rows(s, w.mid32, T, I, nullptr, 0.f, w.split)) return -1;
+      if (gemm(w.split, pl.wo2, H, I, w.x, true, pl.bo2)) return -1;
       if (layernorm_rows(s, w.x, T, H, norms.out_w, norms.out_b, c.ln_eps, w.x, nullptr)) return -1;
-      note_launch(6);   // the split, attention and GELU launches (the GEMMs and LayerNorms count their own)
     }
     SRB_CUDA_CHECK(cudaGetLastError());
     return 0;
@@ -364,20 +283,19 @@ int encoder_forward_precise(Model& m, const int* d_ids, const int* d_cu, int B, 
     const PreciseLayer& pl = p.layers[li];
     const bool local = (li % c.global_every) != 0;
     // attention input: LayerNorm (none on layer 0, modernbert.rs:266-271), split
-    if (precise_split_rows(s, w.x, T, H, norms.attn_w, c.ln_eps, p.split)) return -1;
-    if (gemm(p.split, pl.wqkv, 3 * H, H, p.qkv32, false, nullptr)) return -1;
-    if (precise_rope(s, p.qkv32, w.pos, T, c.heads, local ? m.rope_cos_l : m.rope_cos_g, local ? m.rope_sin_l : m.rope_sin_g))
+    if (precise_split_rows(s, w.x, T, H, norms.attn_w, c.ln_eps, w.split)) return -1;
+    if (gemm(w.split, pl.wqkv, 3 * H, H, w.qkv32, false, nullptr)) return -1;
+    if (precise_rope(s, w.qkv32, w.pos, T, c.heads, local ? m.rope_cos_l : m.rope_cos_g, local ? m.rope_sin_l : m.rope_sin_g))
       return -1;
-    if (precise_attention(s, p.qkv32, p.ctx32, d_cu, B, max_len, c.heads, 64, local ? c.local_attention / 2 : 0, nullptr))
+    if (precise_attention(s, w.qkv32, w.ctx32, d_cu, B, max_len, c.heads, 64, local ? c.local_attention / 2 : 0, nullptr))
       return -1;
-    if (precise_split_rows(s, p.ctx32, T, H, nullptr, 0.f, p.split)) return -1;
-    if (gemm(p.split, pl.wo, H, H, w.x, true, nullptr)) return -1;
-    if (precise_split_rows(s, w.x, T, H, norms.mid_w, c.ln_eps, p.split)) return -1;
-    if (gemm(p.split, pl.wi, 2 * I, H, p.mid32, false, nullptr)) return -1;
-    if (precise_geglu(s, p.mid32, T, I, p.act32)) return -1;
-    if (precise_split_rows(s, p.act32, T, I, nullptr, 0.f, p.split)) return -1;
-    if (gemm(p.split, pl.wo2, H, I, w.x, true, nullptr)) return -1;
-    note_launch(7);
+    if (precise_split_rows(s, w.ctx32, T, H, nullptr, 0.f, w.split)) return -1;
+    if (gemm(w.split, pl.wo, H, H, w.x, true, nullptr)) return -1;
+    if (precise_split_rows(s, w.x, T, H, norms.mid_w, c.ln_eps, w.split)) return -1;
+    if (gemm(w.split, pl.wi, 2 * I, H, w.mid32, false, nullptr)) return -1;
+    if (precise_geglu(s, w.mid32, T, I, w.act32)) return -1;
+    if (precise_split_rows(s, w.act32, T, I, nullptr, 0.f, w.split)) return -1;
+    if (gemm(w.split, pl.wo2, H, I, w.x, true, nullptr)) return -1;
   }
   SRB_CUDA_CHECK(cudaGetLastError());
   return 0;

@@ -17,8 +17,12 @@ references and bounds of oracle/precise_oracle.py and gemm_oracle.gemm(split=Tru
     most 65 535), and 70 000 sequences through sr_forward_dev on both paths, bitwise the same rows as two calls.
   * The triple-depth GEMM at every (N, K') encoder_forward_precise launches at those geometries, K' up to 12 288,
     M = 1, 127, 128, 129 and 17 370, EPI_RESID plain and in place.
+  * The precise forward of a small ModernBERT and a small BERT model on a caller's stream (sr_model_set_stream): no
+    device-bytes change from set_precise, launch counts exact at 1 and 2 attention slices per layer, and a CUDA graph
+    capture of sr_forward_dev whose replay is bitwise the eager call.
 Outputs start as NaN and rows past the launch hold sentinels that must survive.  Run with -s for the worst error / bound
 of each kernel and where it occurs."""
+import ctypes as C
 import math
 
 import numpy as np
@@ -304,6 +308,66 @@ def test_forward_beyond_grid_z_equals_two_calls(srlib, cuda, precise):
         second = _forward(srlib, m, seqs[65535:], 2)
         m.set_precise(False)
     assert _same(whole, torch.cat([first, second]))
+
+
+# ---- the precise forward on a caller's stream ------------------------------------------------------------------------
+def _small_model(arch):
+    if arch == "modernbert":
+        cfg = ho.modernbert_config("small-384", 2)
+        return cfg, ho.modernbert_weights(cfg, "plain")
+    cfg = eo.BertConfig(vocab_size=ho.VOCAB, hidden_size=384, num_hidden_layers=2, num_attention_heads=12,
+                        intermediate_size=1536)
+    return cfg, synth.make_bert_weights(cfg, 0, seed=31, with_pooler=False)
+
+
+@pytest.mark.parametrize("lens", [PACK, [1] * 70000], ids=["pack", "70000-ones"])
+@pytest.mark.parametrize("arch", ["modernbert", "bert"])
+def test_forward_on_caller_stream_replays_as_a_graph(srlib, cuda, arch, lens):
+    """sr_reserve, then set_precise(True), on a caller's stream: set_precise leaves device_bytes() unchanged, one eager
+    forward counts exactly the kernels it launches (attention once per slice of at most 65 535 sequences), and the
+    forward captures as a CUDA graph whose replay writes the eager call's hidden rows bitwise"""
+    from test_encoder_hidden_conformance_gpu import _hidden, _load, _same
+    cfg, w = _small_model(arch)
+    L = srlib.lib()
+    L.sr_launch_count.restype = C.c_longlong
+    ids, cu = srlib.pack(synth.make_ids(np.random.default_rng(32), lens, cfg.vocab_size))
+    T, B, max_len = len(ids), len(lens), max(lens)
+    d_ids, d_cu = torch.from_numpy(ids).to(DEV), torch.from_numpy(cu).to(DEV)
+    stream = torch.cuda.Stream()
+    torch.cuda.synchronize()
+    layers = cfg.num_hidden_layers
+    slices = (B + 65534) // 65535
+    # positions + embedding, then per layer 4 splits, 4 GEMMs, the attention slices and
+    # ModernBERT: RoPE + GeGLU / BERT: GELU + 2 LayerNorms
+    expected = 2 + layers * (8 + slices + (2 if arch == "modernbert" else 3))
+    with _load(srlib, cfg, w) as m:
+        h = m.handle
+        assert L.sr_model_set_stream(h, C.c_void_p(stream.cuda_stream)) == 0
+        assert L.sr_reserve(h, T, B, B) == 0
+        loaded = m.device_bytes()
+        m.set_precise(True)
+        assert m.device_bytes() == loaded
+        forward = lambda: L.sr_forward_dev(h, d_ids.data_ptr(), d_cu.data_ptr(), B, T, max_len, 0)
+        with torch.cuda.stream(stream):
+            n0 = L.sr_launch_count()
+            assert forward() == 0
+            assert L.sr_launch_count() - n0 == expected
+        stream.synchronize()
+        eager = _hidden(srlib, m, T)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, stream=stream, capture_error_mode="thread_local"):
+            assert forward() == 0
+
+        class _Rows:
+            __cuda_array_interface__ = {"data": (int(L.sr_dev_hidden(h)), False), "shape": (T, m.hidden),
+                                        "typestr": "<f4", "version": 3}
+        rows = torch.as_tensor(_Rows(), device=DEV)    # the model's hidden rows, not a copy
+        with torch.cuda.stream(stream):
+            rows.fill_(float("nan"))
+            graph.replay()
+        stream.synchronize()
+        assert _same(rows.clone(), eager)
+        assert L.sr_model_set_stream(h, None) == 0
 
 
 # ---- the triple-depth GEMM -----------------------------------------------------------------------------------------
