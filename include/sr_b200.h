@@ -155,6 +155,21 @@ SR_API const float* sr_dev_hidden(const sr_model* m);   /* fp32 residual stream 
 typedef struct sr_cache sr_cache;
 /* capacity rows of dimension dim on `device`; id_offset = global id of local row 0 (sharded caches). */
 SR_API int sr_cache_create(int device, int capacity, int dim, int id_offset, sr_cache** out);
+/* An exact cache: sr_cache_topk and sr_cache_lookup_ids return, per query, the scores of the reference's
+ * embeddingDotProduct (pkg/cache/inmemory_cache_search.go:14-20: dot = 0, dot += q[i] * c[i] in index order) on the fp32
+ * query and the fp32 rows exactly as passed to sr_cache_add, bit for bit, and the ids in descending score order, lower
+ * index first on ties, with the same -1 / -inf padding.  sum_rule picks how each term is accumulated: 0 rounds the product
+ * to fp32, then adds (Go on amd64 at the default GOAMD64=v1); 1 is one fused multiply-add (Go on arm64, ppc64le, s390x and
+ * on amd64 at GOAMD64=v3 or higher); any other value is refused.  The store keeps every row twice, fp32 beside the fp16
+ * copy (6 bytes per element instead of 2).  The fp16 scan stays the filter: it picks k' candidates per query (k' = 32 for
+ * k <= 32 and 64 above, where the two-stage selection takes that many, else 16 or k), a certified band of them is rescored in Go order, and a query
+ * whose band does not fit in k' is scanned exhaustively in Go order on the CUDA cores.  Limits: 1 <= k <= 64 and
+ * ceil(size / 8192) * k <= 25600 for every b (the fallback selects through the two-stage selection; there is no fused
+ * route), and the scan synchronises once in the middle.  Refused (-1, outputs untouched): rows (sr_cache_add) or queries
+ * (sr_cache_topk) with a non-finite component or one of magnitude above 65504; sr_cache_topk_dev and
+ * sr_cache_topk_packed_dev, which see only fp16 queries -- scan each shard with sr_cache_topk and merge the lists with
+ * sr_cache_merge_topk, which is exact on exact scores.  Lifecycle calls keep both stores in step. */
+SR_API int sr_cache_create_exact(int device, int capacity, int dim, int id_offset, int sum_rule, sr_cache** out);
 SR_API void sr_cache_free(sr_cache* c);
 /* Append n rows (float32 host, rounded to fp16 on upload); returns first local row index or -1. */
 SR_API int sr_cache_add(sr_cache* c, const float* rows, int n);

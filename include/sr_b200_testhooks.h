@@ -79,6 +79,13 @@ SR_API int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists);
  * two-stage selection; chunks = score chunks of the two-stage routes (0 otherwise); candidates = stage-2 candidates per
  * query (fused: the upper bound).  Returns -1 (route -1) wherever sr_cache_topk refuses the shape. */
 SR_API int sr_test_cache_plan(int b, int n, int dim, int k, int* route, int* chunks, int* candidates);
+/* The last scan of an exact cache (sr_cache_create_exact) over b queries, per query: path 0 when its band of possible
+ * winners was certified inside the candidates of the fp16 scan, 1 when it fell back to the exhaustive exact scan; band = the
+ * candidates at or above s16_(k) - 2 eps (for a fallback query: all of them); eps = the bound on |fp16-operand score - Go
+ * score| (csrc/cache_scan.cu exact_eps).  candidates = k' of that scan, fallback = its fallback queries (either may be
+ * null).  -1 for a cache that is not exact or whose last scan had another b. */
+SR_API int sr_test_cache_exact_stats(sr_cache* c, int b, int32_t* path, int32_t* band, double* eps, int* candidates,
+                                     int* fallback);
 SR_API int sr_test_hl_to_f32(const void* hi_f16, const void* lo_f16, const float* pivot, int t, int hdim, float* x);
 /* attention_wgmma_fwd (csrc/kernels.h: same arguments and meaning; window 0 = global, kv_lens [batch] or null) */
 SR_API int sr_test_attention_wgmma(const void* qkv_f16, void* out_f16, const int32_t* cu_seqlens, int batch, int max_len,

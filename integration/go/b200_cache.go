@@ -4,8 +4,10 @@
 //
 // Drop this file into src/semantic-router/pkg/cache/ of the reference and build with `-tags b200`.  It implements the
 // reference's CacheBackend interface (cache_interface.go) on top of the B200 library's cache entry points
-// (include/sr_b200.h: sr_cache_*): the embeddings of the entries live in HBM as fp16 rows, one row per element of the
-// entries slice in slice order, and FindSimilar asks the GPU for the best row instead of running
+// (include/sr_b200.h: sr_cache_*): the embeddings of the entries live in HBM, one row per element of the entries slice in
+// slice order, in an exact store (sr_cache_create_exact: the fp32 rows beside an fp16 copy, scores bitwise those of
+// embeddingDotProduct as this binary's Go compiler evaluates it, goSumRule), and FindSimilar asks the GPU for the best
+// row instead of running
 // scanLinearForSimilarity (inmemory_cache_search.go:65-89) over a Go slice under a read lock.  Everything that is not
 // arithmetic is the reference's own bookkeeping and reuses its types: CacheEntry, the FIFO / LRU / LFU policies and the
 // ExpirationHeap of eviction_policy.go.  Each slice mutation has its device form:
@@ -25,7 +27,7 @@ package cache
 #include <stdint.h>
 #include <stdlib.h>
 typedef struct sr_cache sr_cache;
-int sr_cache_create(int device, int capacity, int dim, int id_offset, sr_cache** out);
+int sr_cache_create_exact(int device, int capacity, int dim, int id_offset, int sum_rule, sr_cache** out);
 void sr_cache_free(sr_cache* c);
 int sr_cache_add(sr_cache* c, const float* rows, int n);
 int sr_cache_set_valid(sr_cache* c, int local_row, int valid);
@@ -90,8 +92,8 @@ func NewB200Cache(options InMemoryCacheOptions, device int, dim int, embed func(
 	default:
 		c.fifo = NewFIFOPolicy()
 	}
-	if rc := C.sr_cache_create(C.int(device), C.int(capacity), C.int(dim), 0, &c.store); rc != 0 {
-		return nil, fmt.Errorf("sr_cache_create failed (no sm_100 GPU?)")
+	if rc := C.sr_cache_create_exact(C.int(device), C.int(capacity), C.int(dim), 0, C.int(goSumRule), &c.store); rc != 0 {
+		return nil, fmt.Errorf("sr_cache_create_exact failed (no sm_90 GPU?)")
 	}
 	return c, nil
 }

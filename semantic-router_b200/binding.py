@@ -67,6 +67,7 @@ def load_library(path: Optional[str] = None):
         getattr(L, f).argtypes = [vp]
         getattr(L, f).restype = vp
     L.sr_cache_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
+    L.sr_cache_create_exact.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
     L.sr_cache_free.argtypes = [vp]
     L.sr_cache_free.restype = None
     L.sr_cache_add.argtypes = [vp, vp, C.c_int]
@@ -147,6 +148,7 @@ def hooks():
         H.sr_test_precise_gelu.argtypes = [vp, C.c_int, C.c_int]
         H.sr_test_hl_to_f32.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp]
         H.sr_test_cache_plan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
+        H.sr_test_cache_exact_stats.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
         ci, cf = C.c_int, C.c_float
         H.sr_test_embed_ln_modernbert.argtypes = [vp, ci, ci, ci, vp, vp, cf, vp, vp, vp]
         H.sr_test_embed_ln_bert.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, cf, vp, vp]
@@ -348,13 +350,22 @@ class GroupedModel(LoraSharedModel):
 
 
 class Cache:
-    """Device-resident semantic cache shard (mirror of pkg/cache/inmemory_cache.go's lookup side)."""
+    """Device-resident semantic cache shard (mirror of pkg/cache/inmemory_cache.go's lookup side).
 
-    def __init__(self, capacity: int, dim: int, device: int = 0, id_offset: int = 0):
+    exact=True (sr_cache_create_exact): scores bitwise those of the reference's fp32 embeddingDotProduct on the rows and
+    queries as given, under sum_rule 0 (product rounded, then added: Go amd64 v1) or 1 (fused multiply-add: Go arm64,
+    amd64 v3+)."""
+
+    def __init__(self, capacity: int, dim: int, device: int = 0, id_offset: int = 0, exact: bool = False,
+                 sum_rule: int = 0):
         self._h = C.c_void_p()
-        if lib().sr_cache_create(device, capacity, dim, id_offset, C.byref(self._h)) != 0:
+        if exact:
+            if lib().sr_cache_create_exact(device, capacity, dim, id_offset, sum_rule, C.byref(self._h)) != 0:
+                raise SrError("sr_cache_create_exact failed")
+        elif lib().sr_cache_create(device, capacity, dim, id_offset, C.byref(self._h)) != 0:
             raise SrError("sr_cache_create failed")
         self.dim = dim
+        self.exact = exact
 
     def close(self):
         if self._h:
@@ -412,6 +423,17 @@ class Cache:
         if lib().sr_cache_topk(self._h, _p(q), q.shape[0], k, _p(idx), _p(sc)) != 0:
             raise SrError("sr_cache_topk failed")
         return idx, sc
+
+    def exact_stats(self, b: int):
+        """The last scan of an exact cache over b queries (test hook): (path [b] 0 certified / 1 fallback, band [b],
+        eps [b] float64, k', fallback count)."""
+        path = np.empty(b, np.int32)
+        band = np.empty(b, np.int32)
+        eps = np.empty(b, np.float64)
+        kc, nf = C.c_int(0), C.c_int(0)
+        if hooks().sr_test_cache_exact_stats(self._h, b, _p(path), _p(band), _p(eps), C.byref(kc), C.byref(nf)) != 0:
+            raise SrError("sr_test_cache_exact_stats failed")
+        return path, band, eps, kc.value, nf.value
 
 
     def lookup_ids(self, model: "Model", seqs: Sequence[np.ndarray], k: int, target_layer: int = 0):

@@ -93,7 +93,7 @@ class B200SemanticCache:
 
     def __init__(self, dim: int, similarity_threshold: float, max_entries: int, ttl_seconds: int, eviction_policy: str = "fifo",
                  embed: Optional[Callable[[str], np.ndarray]] = None, device: int = 0, clock: Callable[[], float] = time.time,
-                 capacity: Optional[int] = None):
+                 capacity: Optional[int] = None, exact: bool = False, sum_rule: int = 0):
         self.dim = dim
         self.threshold = np.float32(similarity_threshold)
         self.max_entries = max_entries
@@ -101,7 +101,8 @@ class B200SemanticCache:
         self.embed = embed
         self.clock = clock
         cap = capacity or (max_entries if max_entries > 0 else 1 << 16)
-        self.store = Cache(cap, dim, device=device)
+        # exact: hit decisions on the reference's own fp32 scores (sr_cache_create_exact) under the Go build's sum rule
+        self.store = Cache(cap, dim, device=device, exact=exact, sum_rule=sum_rule)
         self.evictor = _Evictor(eviction_policy)
         # entries[i] <-> device row i
         self.request_id: List[str] = []

@@ -16,7 +16,9 @@ using namespace srb;
 
 namespace srb {   // cache_api.cu
 std::mutex& cache_mutex(sr_cache* c);
-int cache_topk_dev_locked(sr_cache* c, const void* d_queries_f16, int b, int k, void* cuda_stream);
+int cache_topk_dev_locked(sr_cache* c, const void* d_queries_f16, const float* d_queries_f32, int b, int k,
+                          void* cuda_stream);
+int cache_exact_stats(sr_cache* c, int b, int32_t* path, int32_t* band, double* eps, int* candidates, int* fallback);
 }
 
 // A captured forward (+ sequence head) for one launch geometry.  Small calls -- one prompt, the reference's operating
@@ -342,7 +344,8 @@ int sr_cache_lookup_ids(sr_model* h, sr_cache* c, const int32_t* ids, const int3
     h->q16_elems = n;
   }
   if (cast_rows_f16(m.stream, w.emb, n, h->q16)) return fail("cast failed");
-  if (cache_topk_dev_locked(c, h->q16, batch, k, m.stream)) return fail("cache scan failed");
+  // an exact cache scores the fp32 embedding itself; the fp16 copy only feeds its candidate scan
+  if (cache_topk_dev_locked(c, h->q16, w.emb, batch, k, m.stream)) return fail("cache scan failed");
   cudaMemcpyAsync(out_idx, sr_cache_dev_idx(c), static_cast<size_t>(batch) * k * 4, cudaMemcpyDeviceToHost, m.stream);
   cudaMemcpyAsync(out_score, sr_cache_dev_score(c), static_cast<size_t>(batch) * k * 4, cudaMemcpyDeviceToHost, m.stream);
   return finish(m);
@@ -600,6 +603,10 @@ int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists) {
   g.fold_stats = d->fold_stats; g.fold_eps = d->fold_eps; g.fold_h = d->fold_h;
   g.w_groups = d->w_groups; g.w_group_rows = d->w_group_rows; g.bias_per_group = d->bias_per_group != 0;
   return gemm_f16(nullptr, g);
+}
+int sr_test_cache_exact_stats(sr_cache* c, int b, int32_t* path, int32_t* band, double* eps, int* candidates, int* fallback) {
+  if (!c || b <= 0 || !path || !band || !eps) return -1;
+  return cache_exact_stats(c, b, path, band, eps, candidates, fallback);
 }
 int sr_test_cache_plan(int b, int n, int dim, int k, int* route, int* chunks, int* candidates) {
   const CachePlan p = cache_topk_plan(b, n, dim, k);

@@ -2,6 +2,7 @@
 // (src/semantic-router/pkg/cache/inmemory_cache.go:192-234, inmemory_cache_search.go:65-89):
 // entries are appended, may be invalidated (expired / evicted), and are scanned exhaustively.
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -26,6 +27,17 @@ struct sr_cache {
   int q_cap = 0, res_cap = 0;
   cudaStream_t stream = nullptr;
   std::mutex mu;
+  // exact caches (sr_cache_create_exact): the rows as passed to sr_cache_add, bit for bit, beside the fp16 copy the scan
+  // reads; the largest L2 norm any row ever added had (removing rows leaves it an upper bound); the record of the last
+  // scan per query (sr_test_cache_exact_stats)
+  bool exact = false;
+  int sum_rule = 0;
+  float* rows32 = nullptr;
+  double rmax = 0;
+  int* d_path = nullptr;
+  int* d_band = nullptr;
+  double* d_eps = nullptr;
+  int last_b = 0, last_kc = 0, last_fallback = 0;
 };
 
 namespace {
@@ -33,10 +45,26 @@ int cfail(const char* msg) {
   fprintf(stderr, "[srb200] %s\n", msg);
   return -1;
 }
+// What the exact scan's bound covers (cache_scan.cu): finite components that round to a finite fp16 value.  Returns the
+// largest L2 norm of the n rows of dim values, or -1 when a component falls outside.
+double checked_max_norm(const float* x, size_t n, int dim) {
+  double best = 0;
+  for (size_t r = 0; r < n; ++r) {
+    double ss = 0;
+    for (int i = 0; i < dim; ++i) {
+      const float v = x[r * dim + i];
+      if (!(std::fabs(v) <= 65504.f)) return -1;   // NaN fails the comparison too
+      ss += static_cast<double>(v) * v;
+    }
+    best = std::max(best, std::sqrt(ss));
+  }
+  return best;
+}
 // Grows the per-cache scratch.  Caller holds c->mu.  Buffers may still be referenced by work queued on the cache's
 // stream or on a caller's stream (sr_cache_topk_dev), so everything on the device drains before anything is freed.
 int ensure(sr_cache* c, int b, int k) {
-  const size_t need = cache_topk_workspace_bytes(b, c->size > 0 ? c->size : 1, c->dim, k);
+  const int n = c->size > 0 ? c->size : 1;
+  const size_t need = c->exact ? cache_topk_exact_workspace_bytes(b, n, c->dim, k) : cache_topk_workspace_bytes(b, n, c->dim, k);
   if (b > c->q_cap || b * k > c->res_cap || need > c->ws_bytes) cudaDeviceSynchronize();
   if (b > c->q_cap) {
     if (c->d_q) cudaFree(c->d_q);
@@ -44,6 +72,15 @@ int ensure(sr_cache* c, int b, int k) {
     c->d_q = nullptr; c->d_q32 = nullptr; c->q_cap = 0;
     if (cudaMalloc(reinterpret_cast<void**>(&c->d_q), static_cast<size_t>(b) * c->dim * 2) != cudaSuccess) return -1;
     if (cudaMalloc(reinterpret_cast<void**>(&c->d_q32), static_cast<size_t>(b) * c->dim * 4) != cudaSuccess) return -1;
+    if (c->exact) {
+      for (void* p : {static_cast<void*>(c->d_path), static_cast<void*>(c->d_band), static_cast<void*>(c->d_eps)})
+        if (p) cudaFree(p);
+      c->d_path = nullptr; c->d_band = nullptr; c->d_eps = nullptr;
+      if (cudaMalloc(reinterpret_cast<void**>(&c->d_path), static_cast<size_t>(b) * 4) != cudaSuccess ||
+          cudaMalloc(reinterpret_cast<void**>(&c->d_band), static_cast<size_t>(b) * 4) != cudaSuccess ||
+          cudaMalloc(reinterpret_cast<void**>(&c->d_eps), static_cast<size_t>(b) * 8) != cudaSuccess)
+        return -1;
+    }
     c->q_cap = b;
   }
   if (b * k > c->res_cap) {
@@ -62,35 +99,62 @@ int ensure(sr_cache* c, int b, int k) {
   }
   return 0;
 }
-int topk_dev_locked(sr_cache* c, const void* d_queries_f16, int b, int k, void* cuda_stream) {
+// d_queries_f32: the queries before their fp16 rounding, which an exact cache scores with (null: refused there)
+int topk_dev_locked(sr_cache* c, const void* d_queries_f16, const float* d_queries_f32, int b, int k, void* cuda_stream) {
+  if (c->exact && !d_queries_f32) return cfail("sr_cache_topk: an exact cache needs the fp32 queries (sr_cache_topk)");
   cudaSetDevice(c->device);
   if (ensure(c, b, k)) return cfail("sr_cache_topk: allocation failed");
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : c->stream;
-  return cache_topk(s, static_cast<const __half*>(d_queries_f16), b, c->rows, c->valid, c->size, c->dim, k, c->id_offset,
-                    c->d_idx, c->d_score, c->ws, c->ws_bytes);
+  const __half* q16 = static_cast<const __half*>(d_queries_f16);
+  if (!c->exact)
+    return cache_topk(s, q16, b, c->rows, c->valid, c->size, c->dim, k, c->id_offset, c->d_idx, c->d_score, c->ws,
+                      c->ws_bytes);
+  int fallback = 0;
+  if (cache_topk_exact(s, d_queries_f32, q16, b, c->rows, c->rows32, c->valid, c->size, c->dim, c->rmax, k, c->sum_rule,
+                       c->id_offset, c->d_idx, c->d_score, c->ws, c->ws_bytes, c->d_path, c->d_band, c->d_eps, &fallback))
+    return -1;
+  c->last_b = b;
+  c->last_kc = cache_exact_candidates(b, c->size, c->dim, k);
+  c->last_fallback = fallback;
+  return 0;
 }
 }  // namespace
 
 namespace srb {
 // api.cu (sr_cache_lookup_ids) holds the cache's mutex from the scan until its D2H copies have landed
 std::mutex& cache_mutex(sr_cache* c) { return c->mu; }
-int cache_topk_dev_locked(sr_cache* c, const void* d_queries_f16, int b, int k, void* cuda_stream) {
-  return topk_dev_locked(c, d_queries_f16, b, k, cuda_stream);
+int cache_topk_dev_locked(sr_cache* c, const void* d_queries_f16, const float* d_queries_f32, int b, int k,
+                          void* cuda_stream) {
+  return topk_dev_locked(c, d_queries_f16, d_queries_f32, b, k, cuda_stream);
+}
+int cache_exact_stats(sr_cache* c, int b, int32_t* path, int32_t* band, double* eps, int* candidates, int* fallback) {
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (!c->exact || c->last_b <= 0 || b != c->last_b) return -1;
+  cudaSetDevice(c->device);
+  if (cudaMemcpy(path, c->d_path, static_cast<size_t>(b) * 4, cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(band, c->d_band, static_cast<size_t>(b) * 4, cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(eps, c->d_eps, static_cast<size_t>(b) * 8, cudaMemcpyDeviceToHost) != cudaSuccess)
+    return -1;
+  if (candidates) *candidates = c->last_kc;
+  if (fallback) *fallback = c->last_fallback;
+  return 0;
 }
 }  // namespace srb
 
 extern "C" {
 
-int sr_cache_create(int device, int capacity, int dim, int id_offset, sr_cache** out) {
+static int cache_create(int device, int capacity, int dim, int id_offset, bool exact, int sum_rule, sr_cache** out) {
   if (!out || capacity <= 0 || dim <= 0 || dim % 8 != 0) return cfail("sr_cache_create: bad arguments (dim % 8 == 0)");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return cfail("sr_cache_create: no such CUDA device");
   cudaSetDevice(device);
   sr_cache* c = new sr_cache();
   c->device = device; c->capacity = capacity; c->dim = dim; c->id_offset = id_offset;
+  c->exact = exact; c->sum_rule = sum_rule;
   c->cap_pad = (capacity + 255) / 256 * 256;  // GEMM N tiles may read (never report) the padding rows
   if (cudaMalloc(reinterpret_cast<void**>(&c->rows), static_cast<size_t>(c->cap_pad) * dim * 2) != cudaSuccess ||
       cudaMalloc(reinterpret_cast<void**>(&c->valid), c->cap_pad) != cudaSuccess ||
+      (exact && cudaMalloc(reinterpret_cast<void**>(&c->rows32), static_cast<size_t>(capacity) * dim * 4) != cudaSuccess) ||
       cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) {
     sr_cache_free(c);
     return cfail("sr_cache_create: allocation failed");
@@ -101,11 +165,20 @@ int sr_cache_create(int device, int capacity, int dim, int id_offset, sr_cache**
   return 0;
 }
 
+int sr_cache_create(int device, int capacity, int dim, int id_offset, sr_cache** out) {
+  return cache_create(device, capacity, dim, id_offset, false, 0, out);
+}
+
+int sr_cache_create_exact(int device, int capacity, int dim, int id_offset, int sum_rule, sr_cache** out) {
+  if (sum_rule != 0 && sum_rule != 1) return cfail("sr_cache_create_exact: sum_rule must be 0 (unfused) or 1 (fused)");
+  return cache_create(device, capacity, dim, id_offset, true, sum_rule, out);
+}
+
 void sr_cache_free(sr_cache* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   if (c->stream) { cudaStreamSynchronize(c->stream); cudaStreamDestroy(c->stream); }
-  void* ptrs[] = {c->rows, c->valid, c->ws, c->d_q, c->d_q32, c->d_idx, c->d_score};
+  void* ptrs[] = {c->rows, c->valid, c->ws, c->d_q, c->d_q32, c->d_idx, c->d_score, c->rows32, c->d_path, c->d_band, c->d_eps};
   for (void* p : ptrs) if (p) cudaFree(p);
   delete c;
 }
@@ -115,6 +188,22 @@ int sr_cache_add(sr_cache* c, const float* rows, int n) {
   std::lock_guard<std::mutex> lk(c->mu);
   if (c->size + n > c->capacity) return cfail("sr_cache_add: capacity exceeded");
   cudaSetDevice(c->device);
+  if (c->exact) {
+    // the fp32 rows go up as they are and the fp16 copy is rounded from them on the device
+    const double norm = checked_max_norm(rows, static_cast<size_t>(n), c->dim);
+    if (norm < 0) return cfail("sr_cache_add: an exact cache takes finite components of magnitude <= 65504 only");
+    const size_t ne = static_cast<size_t>(n) * c->dim;
+    float* dst = c->rows32 + static_cast<size_t>(c->size) * c->dim;
+    bool ok = cudaMemcpyAsync(dst, rows, ne * 4, cudaMemcpyHostToDevice, c->stream) == cudaSuccess &&
+              srb::cast_rows_f16(c->stream, dst, ne, c->rows + static_cast<size_t>(c->size) * c->dim) == 0 &&
+              cudaMemsetAsync(c->valid + c->size, 1, n, c->stream) == cudaSuccess;
+    ok = cudaStreamSynchronize(c->stream) == cudaSuccess && ok;
+    if (!ok) return cfail("sr_cache_add: H2D failed");
+    c->rmax = std::max(c->rmax, norm);
+    const int first = c->size;
+    c->size += n;
+    return first;
+  }
   // fp32 up in pieces of <= 64 MiB, rounded to fp16 (rn) on the device straight into the store
   const size_t piece_rows = std::max<size_t>(1, (64u << 20) / (static_cast<size_t>(c->dim) * 4));
   float* stage = nullptr;
@@ -166,6 +255,9 @@ int sr_cache_move(sr_cache* c, int dst_row, int src_row) {
   bool ok = cudaMemcpyAsync(c->rows + static_cast<size_t>(dst_row) * c->dim, c->rows + static_cast<size_t>(src_row) * c->dim, rb,
                             cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
   ok = ok && cudaMemcpyAsync(c->valid + dst_row, c->valid + src_row, 1, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+  if (c->exact)
+    ok = ok && cudaMemcpyAsync(c->rows32 + static_cast<size_t>(dst_row) * c->dim, c->rows32 + static_cast<size_t>(src_row) * c->dim,
+                               rb * 2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
   return (cudaStreamSynchronize(c->stream) == cudaSuccess && ok) ? 0 : -1;
 }
 
@@ -192,9 +284,10 @@ int sr_cache_compact(sr_cache* c, const uint8_t* keep, int n) {
   std::vector<uint8_t> valid(static_cast<size_t>(n));
   if (cudaMemcpy(valid.data(), c->valid, n, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
   const size_t rb = static_cast<size_t>(c->dim) * 2;
-  const int scratch_rows = static_cast<int>(std::min<size_t>(static_cast<size_t>(n), std::max<size_t>(1, (64u << 20) / rb)));
-  __half* scratch = nullptr;
-  if (cudaMalloc(reinterpret_cast<void**>(&scratch), static_cast<size_t>(scratch_rows) * rb) != cudaSuccess)
+  const size_t unit = c->exact ? 2 * rb : rb;   // an exact cache moves its fp32 rows through the same scratch
+  const int scratch_rows = static_cast<int>(std::min<size_t>(static_cast<size_t>(n), std::max<size_t>(1, (64u << 20) / unit)));
+  void* scratch = nullptr;
+  if (cudaMalloc(&scratch, static_cast<size_t>(scratch_rows) * unit) != cudaSuccess)
     return cfail("sr_cache_compact: allocation failed");
   bool ok = true;
   int w = first_drop;
@@ -205,6 +298,10 @@ int sr_cache_compact(sr_cache* c, const uint8_t* keep, int n) {
     const size_t bytes = static_cast<size_t>(e - r) * rb;
     ok = cudaMemcpyAsync(scratch, c->rows + static_cast<size_t>(r) * c->dim, bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess &&
          cudaMemcpyAsync(c->rows + static_cast<size_t>(w) * c->dim, scratch, bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+    if (c->exact)
+      ok = ok &&
+           cudaMemcpyAsync(scratch, c->rows32 + static_cast<size_t>(r) * c->dim, 2 * bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess &&
+           cudaMemcpyAsync(c->rows32 + static_cast<size_t>(w) * c->dim, scratch, 2 * bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
     for (int i = r; i < e; ++i) valid[w + (i - r)] = valid[i];
     w += e - r;
     r = e;
@@ -230,12 +327,14 @@ int sr_cache_topk_dev(sr_cache* c, const void* d_queries_f16, int b, int k, void
   // the lock covers growing the scratch and queueing the scan; the result buffers belong to the cache, so callers of
   // this asynchronous entry serialise their use of one cache themselves (sr_b200.h)
   std::lock_guard<std::mutex> lk(c->mu);
-  return topk_dev_locked(c, d_queries_f16, b, k, cuda_stream);
+  return topk_dev_locked(c, d_queries_f16, nullptr, b, k, cuda_stream);
 }
 
 int sr_cache_topk(sr_cache* c, const float* queries, int b, int k, int32_t* out_idx, float* out_score) {
   if (!c || !queries || b <= 0 || k <= 0 || !out_idx || !out_score) return -1;
   std::lock_guard<std::mutex> lk(c->mu);
+  if (c->exact && checked_max_norm(queries, static_cast<size_t>(b), c->dim) < 0)
+    return cfail("sr_cache_topk: an exact cache takes finite query components of magnitude <= 65504 only");
   cudaSetDevice(c->device);
   if (ensure(c, b, k)) return cfail("sr_cache_topk: allocation failed");
   // fp32 up, rounded to fp16 (rn) on the device: a host conversion loop over b*dim values costs more than the scan at
@@ -243,9 +342,7 @@ int sr_cache_topk(sr_cache* c, const float* queries, int b, int k, int32_t* out_
   const size_t nq = static_cast<size_t>(b) * c->dim;
   if (cudaMemcpyAsync(c->d_q32, queries, nq * 4, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) return -1;
   if (srb::cast_rows_f16(c->stream, c->d_q32, nq, c->d_q)) return -1;
-  if (cache_topk(c->stream, c->d_q, b, c->rows, c->valid, c->size, c->dim, k, c->id_offset, c->d_idx, c->d_score, c->ws,
-                 c->ws_bytes))
-    return -1;
+  if (topk_dev_locked(c, c->d_q, c->d_q32, b, k, nullptr)) return -1;
   cudaMemcpyAsync(out_idx, c->d_idx, static_cast<size_t>(b) * k * 4, cudaMemcpyDeviceToHost, c->stream);
   cudaMemcpyAsync(out_score, c->d_score, static_cast<size_t>(b) * k * 4, cudaMemcpyDeviceToHost, c->stream);
   const cudaError_t e = cudaStreamSynchronize(c->stream);
@@ -256,7 +353,7 @@ int sr_cache_topk(sr_cache* c, const float* queries, int b, int k, int32_t* out_
 int sr_cache_topk_packed_dev(sr_cache* c, const void* d_queries_f16, int b, int k, void* d_pairs_out, void* cuda_stream) {
   if (!c || b <= 0 || k <= 0 || !d_pairs_out) return -1;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (topk_dev_locked(c, d_queries_f16, b, k, cuda_stream)) return -1;
+  if (topk_dev_locked(c, d_queries_f16, nullptr, b, k, cuda_stream)) return -1;
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : c->stream;
   return cache_pack_pairs(s, c->d_idx, c->d_score, b * k, d_pairs_out);
 }

@@ -13,6 +13,9 @@
 //   stage 2: one CTA per query: same selection over the segment winners.
 #include "kernels.h"
 
+#include <algorithm>
+#include <initializer_list>
+
 #include "common.cuh"
 #include "gemm.h"
 
@@ -292,6 +295,20 @@ constexpr int kFusedLists = 320;  // upper bound of the lists per query (= 2 x C
 constexpr int kMaxK = 64;         // stage 1 keeps 64 entries per warp (wv / wi)
 constexpr size_t kStage2SmemMax = 200 * 1024;   // stage 2 holds every candidate of its query in shared memory
 
+// The two-stage part of a plan (score chunks, segments, stage-2 candidates, workspace); false, with the route left
+// refused, where stage 2 would hold more than kStage2SmemMax of candidates per query.
+static bool plan_two_stage(CachePlan& p, int B, int N, int k) {
+  p.chunk_rows = chunk_rows(B, N);
+  p.chunks = (N + p.chunk_rows - 1) / p.chunk_rows;
+  p.segments = (N + kSegment - 1) / kSegment;
+  p.candidates = p.segments * k;
+  p.stage2_smem = static_cast<size_t>(p.candidates) * 8;
+  if (p.stage2_smem > kStage2SmemMax) return false;
+  p.workspace_bytes = align_up(static_cast<size_t>(B) * p.chunk_rows * 4, 256) +
+                      2 * align_up(static_cast<size_t>(B) * p.candidates * 4, 256);
+  return true;
+}
+
 CachePlan cache_topk_plan(int B, int N, int D, int k) {
   CachePlan p;
   if (B <= 0 || k <= 0 || k > kMaxK || N < 0) return p;
@@ -305,15 +322,8 @@ CachePlan cache_topk_plan(int B, int N, int D, int k) {
     p.workspace_bytes = 2 * align_up(static_cast<size_t>(B) * kFusedLists * kFusedK * 4, 256);
     return p;
   }
-  p.chunk_rows = chunk_rows(B, N);
-  p.chunks = (N + p.chunk_rows - 1) / p.chunk_rows;
-  p.segments = (N + kSegment - 1) / kSegment;
-  p.candidates = p.segments * k;
-  p.stage2_smem = static_cast<size_t>(p.candidates) * 8;
-  if (p.stage2_smem > kStage2SmemMax) return p;
+  if (!plan_two_stage(p, B, N, k)) return p;
   p.route = (B <= 4 && D % 8 == 0 && static_cast<size_t>(B) * D * 4 <= 48 * 1024) ? CACHE_GEMV : CACHE_GEMM;
-  p.workspace_bytes = align_up(static_cast<size_t>(B) * p.chunk_rows * 4, 256) +
-                      2 * align_up(static_cast<size_t>(B) * p.candidates * 4, 256);
   return p;
 }
 
@@ -420,6 +430,301 @@ int cache_merge_packed(cudaStream_t stream, const void* pairs, int G, int B, int
   if (smem + kSelStaticSmem > kDefaultSmem)
     SRB_CUDA_CHECK(cudaFuncSetAttribute(merge_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   merge_packed_kernel<<<B, kSelThreads, smem, stream>>>(static_cast<const int2*>(pairs), G, B, k, out_idx, out_score);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
+  return 0;
+}
+
+// ---- exact caches (sr_cache_create_exact): the scores of the reference's embeddingDotProduct on the fp32 rows and query
+// (pkg/cache/inmemory_cache_search.go:14-20: dot = 0; dot += q[i] * c[i] in index order), bit for bit.
+//
+// The fp16 scan above stays the filter.  It returns k' >= k candidates per query by their fp16-operand score s16.  With
+// eps >= |s16 - s_go| for every row (s_go the Go score), any row with s16 < s16_(k) - 2 eps has s_go < s16_(k) - eps <=
+// s_go(t) for each of the k rows t of the fp16 top-k, so it is not in the exact top-k.  The band {s16 >= s16_(k) - 2 eps}
+// therefore holds the exact top-k, and the candidate list holds the whole band when it holds every valid row (it ends in
+// -1) or when its last score is strictly below s16_(k) - 2 eps.  Such a query is certified: its band is rescored in Go
+// order and ordered by (score descending, index ascending).  Every other query falls back to an exhaustive exact scan.
+//
+// eps, for a query q and any stored row r, with Q = |q|_2, R >= |r|_2 for every row (the cache keeps the maximum of its
+// rows), S = sqrt(D), and u = 2^-24 the unit roundoff of fp32:
+//  1. fp16 operands.  fp16(x) = x + a with |a| <= d |x| + h, d = 2^-11 (normal range) and h = 2^-25 (half the subnormal
+//     spacing), for |x| <= 65504 (larger or non-finite components are refused at the door).  Then
+//     |q~ r~ - q r| <= |q| |b| + |r| |a| + |a| |b| <= (2d + d^2) |q r| + h (1 + d) (|q| + |r|) + h^2 per component, and by
+//     Cauchy-Schwarz the sum is at most E1 = (2d + d^2) Q R + h (1 + d) S (Q + R) + D h^2.
+//  2. The scan's fp32 sum of the exact products q~_i r~_i (11 x 11 significant bits fit in fp32, and the smallest product
+//     2^-48 is a normal fp32 number).  Whatever the order -- wgmma's accumulation, the GEMV's fmaf chains and shuffle tree --
+//     each partial sum is one of at most D additions, so with a rounding error per addition of at most u' = 8 u relative
+//     (round-to-nearest gives u; 8 u leaves room for truncation and the tensor cores' alignment of their addends) the error
+//     is at most E2 = g'_D sum |q~_i r~_i| <= g'_D ((1 + d)^2 Q R + h (1 + d) S (Q + R) + D h^2), g'_D = D u' / (1 - D u').
+//  3. Go's own sum: D roundings of either rule (a product and an addition each, or one fma each) give
+//     E3 = g_D sum |q_i r_i| <= g_D Q R, g_D = D u / (1 - D u).
+//  4. Underflow: every rounding may also lose up to 2^-150 absolute; 2 D of them at 2^-149 each give E4 = 2 D 2^-149.
+// eps = (E1 + E2 + E3 + E4) (1 + 2^-20), the last factor covering the float64 evaluation of eps and of Q.
+// (oracle/cache_exact_oracle.py exact_eps restates it; tests/test_cache_exact_oracle.py checks it on adversarial rows.)
+__host__ __device__ inline double exact_eps(double Q, double R, int D) {
+  const double d = 1.0 / 2048, h = 1.0 / 33554432.0, u = 1.0 / 16777216.0, S = sqrt(static_cast<double>(D));
+  const double g = D * u / (1 - D * u), g8 = D * 8 * u / (1 - D * 8 * u);
+  const double cross = h * (1 + d) * S * (Q + R) + D * h * h;
+  const double e1 = (2 * d + d * d) * Q * R + cross;
+  const double e2 = g8 * ((1 + d) * (1 + d) * Q * R + cross);
+  const double e3 = g * Q * R;
+  const double e4 = 2.0 * D * 0x1p-149;
+  return (e1 + e2 + e3 + e4) * (1 + 0x1p-20);
+}
+
+namespace {
+
+constexpr int kExactCand = 64;   // the most candidates a query's band may hold (one thread each in exact_band_kernel)
+
+// one Go-order term: rule 0 rounds the product, then the sum (Go amd64 v1); rule 1 is one fused multiply-add (Go arm64,
+// amd64 v3).  Explicit intrinsics: nvcc would contract `acc + a * b` into an fma and turn rule 0 into rule 1.
+template <int kRule>
+__device__ __forceinline__ float go_term(float acc, float a, float b) {
+  return kRule == 0 ? __fadd_rn(acc, __fmul_rn(a, b)) : __fmaf_rn(a, b, acc);
+}
+
+// One CTA per query, one thread per candidate.  Certifies the band (see above); a certified query's band members are
+// rescored in Go order from the fp32 row and fp32 query, ranked, and its k results written; any other query is appended
+// to the fallback list and left to exact_scores_kernel.  path / band / eps: the test hook's record of the query.
+template <int kRule>
+__global__ void __launch_bounds__(kExactCand)
+exact_band_kernel(const float* __restrict__ queries, const float* __restrict__ rows32, int D, double rmax,
+                  const int* __restrict__ cand_idx, const float* __restrict__ cand_score, int kc, int k, int id_offset,
+                  int* __restrict__ out_idx, float* __restrict__ out_score, int* __restrict__ fb_list,
+                  int* __restrict__ fb_count, int* __restrict__ path, int* __restrict__ band, double* __restrict__ eps) {
+  extern __shared__ float qs[];   // [D]
+  __shared__ double red[kExactCand / 32];
+  __shared__ float sv[kExactCand];
+  __shared__ int si[kExactCand];
+  __shared__ int order[kExactCand];
+  const int q = blockIdx.x, t = threadIdx.x;
+  double ss = 0;
+  for (int i = t; i < D; i += kExactCand) {
+    const float x = queries[static_cast<size_t>(q) * D + i];
+    qs[i] = x;
+    ss += static_cast<double>(x) * x;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  if (lane_id() == 0) red[t >> 5] = ss;
+  order[t] = -1;
+  __syncthreads();
+  const double e = exact_eps(sqrt(red[0] + red[1]), rmax, D);
+  const int* ci = cand_idx + static_cast<size_t>(q) * kc;
+  const float* cs = cand_score + static_cast<size_t>(q) * kc;
+  const bool all_rows = ci[k - 1] < 0 || ci[kc - 1] < 0;          // fewer than k' valid rows: every one is listed
+  const double thr = ci[k - 1] < 0 ? -INFINITY : static_cast<double>(cs[k - 1]) - 2 * e;
+  const bool certified = all_rows || static_cast<double>(cs[kc - 1]) < thr;
+  const int mine = t < kc && ci[t] >= 0 && static_cast<double>(cs[t]) >= thr ? ci[t] : -1;
+  const int members = __syncthreads_count(mine >= 0);
+  if (t == 0) { path[q] = certified ? 0 : 1; band[q] = members; eps[q] = e; }
+  if (!certified) {
+    if (t == 0) fb_list[atomicAdd(fb_count, 1)] = q;
+    return;
+  }
+  float s = -INFINITY;
+  if (mine >= 0) {
+    const float4* r4 = reinterpret_cast<const float4*>(rows32 + static_cast<size_t>(mine) * D);
+    s = 0.f;
+    for (int c = 0; c < D / 4; ++c) {
+      const float4 r = __ldg(r4 + c);
+      s = go_term<kRule>(s, qs[4 * c], r.x);
+      s = go_term<kRule>(s, qs[4 * c + 1], r.y);
+      s = go_term<kRule>(s, qs[4 * c + 2], r.z);
+      s = go_term<kRule>(s, qs[4 * c + 3], r.w);
+    }
+  }
+  sv[t] = s;
+  si[t] = mine;
+  __syncthreads();
+  if (mine >= 0) {
+    int rank = 0;
+    for (int j = 0; j < kExactCand; ++j) rank += better(sv[j], si[j], s, mine) ? 1 : 0;
+    if (rank < k) order[rank] = t;
+  }
+  __syncthreads();
+  if (t < k) {
+    const int w = order[t];
+    out_idx[static_cast<size_t>(q) * k + t] = w >= 0 ? si[w] + id_offset : -1;
+    out_score[static_cast<size_t>(q) * k + t] = w >= 0 ? sv[w] : -INFINITY;
+  }
+}
+
+// Exhaustive Go-order scores of the fallback queries: scores[j, row] for the nq queries listed in fb_list (rows of
+// `queries`) against rows [0, n) of rows32.  A register-tiled SIMT product, 32 queries x 128 rows per CTA, 4 x 4 per
+// thread; every accumulator takes its D terms one at a time in index order (the K loop is never split), which is the
+// Go sum.
+constexpr int kXq = 32, kXr = 128, kXk = 8;
+template <int kRule>
+__global__ void __launch_bounds__(256)
+exact_scores_kernel(const float* __restrict__ queries, const int* __restrict__ fb_list, const int* __restrict__ fb_count,
+                    const float* __restrict__ rows32, int n, int D, int ld, float* __restrict__ scores) {
+  __shared__ float qs[kXk][kXq];
+  __shared__ float rs[kXk][kXr + 4];
+  const int nq = *fb_count;
+  const int q0 = blockIdx.y * kXq, r0 = blockIdx.x * kXr;
+  if (q0 >= nq) return;
+  const int tq = threadIdx.x >> 5, tr = threadIdx.x & 31;    // queries q0 + tq * 4 + i, rows r0 + tr + 32 j
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+  // loaders: thread -> (query, two k), and (row, k half)
+  const int lq = threadIdx.x >> 3, lk = threadIdx.x & 7;
+  const float* qrow = (q0 + lq < nq) ? queries + static_cast<size_t>(fb_list[q0 + lq]) * D : nullptr;
+  const int lr = threadIdx.x >> 1, lh = (threadIdx.x & 1) * 4;
+  const float* rrow = (r0 + lr < n) ? rows32 + static_cast<size_t>(r0 + lr) * D : nullptr;
+  for (int k0 = 0; k0 < D; k0 += kXk) {
+    qs[lk][lq] = qrow ? qrow[k0 + lk] : 0.f;
+    const float4 r = rrow ? __ldg(reinterpret_cast<const float4*>(rrow + k0 + lh)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    rs[lh][lr] = r.x; rs[lh + 1][lr] = r.y; rs[lh + 2][lr] = r.z; rs[lh + 3][lr] = r.w;
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < kXk; ++kk) {
+      float a[4], b[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = qs[kk][tq * 4 + i];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) b[j] = rs[kk][tr + 32 * j];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = go_term<kRule>(acc[i][j], a[i], b[j]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int qq = q0 + tq * 4 + i;
+    if (qq >= nq) continue;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int rr = r0 + tr + 32 * j;
+      if (rr < n) scores[static_cast<size_t>(qq) * ld + rr] = acc[i][j];
+    }
+  }
+}
+
+// results of the compacted fallback queries back to their rows
+__global__ void exact_scatter_kernel(const int* __restrict__ fb_list, const int* __restrict__ fb_count, int k,
+                                     const int* __restrict__ idx, const float* __restrict__ score, int* __restrict__ out_idx,
+                                     float* __restrict__ out_score) {
+  const int j = blockIdx.x;
+  if (j >= *fb_count) return;
+  const int q = fb_list[j];
+  for (int r = threadIdx.x; r < k; r += blockDim.x) {
+    out_idx[static_cast<size_t>(q) * k + r] = idx[static_cast<size_t>(j) * k + r];
+    out_score[static_cast<size_t>(q) * k + r] = score[static_cast<size_t>(j) * k + r];
+  }
+}
+
+// Workspace of cache_topk_exact: the candidate scan's (reused by the fallback's score chunks and selection), then the
+// candidates, the fallback list and the fallback results.
+struct ExactLayout {
+  int kc = 0;               // candidates per query
+  CachePlan scan, fallback;
+  size_t cand_idx = 0, cand_score = 0, fb_list = 0, fb_idx = 0, fb_score = 0, total = 0;
+};
+ExactLayout exact_layout(int B, int N, int D, int k) {
+  ExactLayout L;
+  if (B <= 0 || k <= 0 || k > kMaxK || N < 0 || D % 8 != 0) return L;
+  if (N > 0 && !plan_two_stage(L.fallback, B, N, k)) return L;
+  // k' = 32 for k <= 32 and 64 above, where the two-stage plan takes it, else fewer; k' = k always fits when the
+  // fallback's selection does.  Not the fused route: its 8 per list are too few to certify a band at k = 8.  Not 64 for
+  // small k: stage 1 has no lane-maximum bound above k = 32 and makes 64 passes over every warp's scores, which made the
+  // candidate scan of BASELINE cfg 4 at b 1024 take 128 ms against 3.7 ms for the default cache's fused route (H100 80GB
+  // HBM3, 700 W).
+  for (int kc : {k <= 32 ? 32 : kExactCand, 16, k}) {
+    if (kc < k) continue;
+    L.scan = cache_topk_plan(B, N, D, kc);
+    if (L.scan.route != CACHE_REFUSED) { L.kc = kc; break; }
+  }
+  if (L.kc == 0) return L;
+  size_t off = std::max(L.scan.workspace_bytes, N > 0 ? L.fallback.workspace_bytes : 0);
+  auto take = [&](size_t bytes) { const size_t at = off; off = align_up(off + bytes, 256); return at; };
+  off = align_up(off, 256);
+  L.cand_idx = take(static_cast<size_t>(B) * L.kc * 4);
+  L.cand_score = take(static_cast<size_t>(B) * L.kc * 4);
+  L.fb_list = take(static_cast<size_t>(B + 1) * 4);   // [0] count, then the queries
+  L.fb_idx = take(static_cast<size_t>(B) * k * 4);
+  L.fb_score = take(static_cast<size_t>(B) * k * 4);
+  L.total = off;
+  return L;
+}
+
+}  // namespace
+
+int cache_exact_candidates(int B, int N, int D, int k) { return exact_layout(B, N, D, k).kc; }
+size_t cache_topk_exact_workspace_bytes(int B, int N, int D, int k) { return exact_layout(B, N, D, k).total; }
+
+int cache_topk_exact(cudaStream_t stream, const float* queries32, const __half* queries16, int B, const __half* cache,
+                     const float* cache32, const uint8_t* valid, int N, int D, double rmax, int k, int sum_rule,
+                     int id_offset, int* out_idx, float* out_score, void* workspace, size_t workspace_bytes, int* path,
+                     int* band, double* eps, int* n_fallback) {
+  if (B <= 0 || k <= 0) return 0;
+  const ExactLayout L = exact_layout(B, N, D, k);
+  if (L.kc == 0 || (sum_rule != 0 && sum_rule != 1)) {
+    fprintf(stderr, "[srb200] cache_topk_exact: k=%d over %d rows unsupported (k <= %d, ceil(rows / %d) * k <= %d)\n", k,
+            N, kMaxK, kSegment, static_cast<int>(kStage2SmemMax / 8));
+    return -1;
+  }
+  if (workspace_bytes < L.total) {
+    fprintf(stderr, "[srb200] cache_topk_exact: workspace too small\n");
+    return -1;
+  }
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  int* cand_idx = reinterpret_cast<int*>(ws + L.cand_idx);
+  float* cand_score = reinterpret_cast<float*>(ws + L.cand_score);
+  int* fb_count = reinterpret_cast<int*>(ws + L.fb_list);
+  int* fb_list = fb_count + 1;
+  if (cache_topk(stream, queries16, B, cache, valid, N, D, L.kc, 0, cand_idx, cand_score, ws, L.scan.workspace_bytes))
+    return -1;
+  SRB_CUDA_CHECK(cudaMemsetAsync(fb_count, 0, 4, stream));
+  const size_t qsmem = static_cast<size_t>(D) * 4;
+  auto band_kernel = sum_rule == 0 ? exact_band_kernel<0> : exact_band_kernel<1>;
+  if (qsmem > kDefaultSmem - 2048)
+    SRB_CUDA_CHECK(cudaFuncSetAttribute(band_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(qsmem)));
+  band_kernel<<<B, kExactCand, qsmem, stream>>>(queries32, cache32, D, rmax, cand_idx, cand_score, L.kc, k, id_offset,
+                                                out_idx, out_score, fb_list, fb_count, path, band, eps);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
+  int nf = 0;
+  SRB_CUDA_CHECK(cudaMemcpyAsync(&nf, fb_count, 4, cudaMemcpyDeviceToHost, stream));
+  SRB_CUDA_CHECK(cudaStreamSynchronize(stream));
+  if (n_fallback) *n_fallback = nf;
+  if (nf == 0) return 0;
+  // Exhaustive exact scan of the fallback queries only: Go-order scores in chunks, then the two-stage selection of
+  // cache_topk over them, then the results back to their query rows.
+  const CachePlan& P = L.fallback;
+  const int chunk = P.chunk_rows;
+  float* scores = reinterpret_cast<float*>(ws);
+  int* sel_idx = reinterpret_cast<int*>(ws + align_up(static_cast<size_t>(B) * chunk * 4, 256));
+  float* sel_score = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sel_idx) +
+                                              align_up(static_cast<size_t>(B) * P.candidates * 4, 256));
+  int* fb_idx = reinterpret_cast<int*>(ws + L.fb_idx);
+  float* fb_score = reinterpret_cast<float*>(ws + L.fb_score);
+  auto scores_kernel = sum_rule == 0 ? exact_scores_kernel<0> : exact_scores_kernel<1>;
+  for (int row0 = 0; row0 < N; row0 += chunk) {
+    const int n = (N - row0) < chunk ? (N - row0) : chunk;
+    const dim3 grid((n + kXr - 1) / kXr, (nf + kXq - 1) / kXq);
+    scores_kernel<<<grid, 256, 0, stream>>>(queries32, fb_list, fb_count, cache32 + static_cast<size_t>(row0) * D, n, D,
+                                            chunk, scores);
+    SRB_CUDA_CHECK(cudaGetLastError());
+    note_launch();
+    const dim3 sgrid((n + kSegment - 1) / kSegment, nf);
+    select_stage1<<<sgrid, kSelThreads, 0, stream>>>(scores, chunk, n, row0, valid, k, row0 / kSegment, P.segments,
+                                                     sel_idx, sel_score);
+    SRB_CUDA_CHECK(cudaGetLastError());
+    note_launch();
+  }
+  const size_t smem = P.stage2_smem;
+  if (smem + kSelStaticSmem > kDefaultSmem)
+    SRB_CUDA_CHECK(cudaFuncSetAttribute(select_stage2, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  select_stage2<<<nf, kSelThreads, smem, stream>>>(sel_idx, sel_score, P.candidates, k, id_offset, fb_idx, fb_score);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
+  exact_scatter_kernel<<<nf, 64, 0, stream>>>(fb_list, fb_count, k, fb_idx, fb_score, out_idx, out_score);
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   return 0;
