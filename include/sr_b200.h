@@ -165,10 +165,12 @@ SR_API int sr_cache_create(int device, int capacity, int dim, int id_offset, sr_
  * k <= 32 and 64 above, where the two-stage selection takes that many, else 16 or k), a certified band of them is rescored in Go order, and a query
  * whose band does not fit in k' is scanned exhaustively in Go order on the CUDA cores.  Limits: 1 <= k <= 64 and
  * ceil(size / 8192) * k <= 25600 for every b (the fallback selects through the two-stage selection; there is no fused
- * route), and the scan synchronises once in the middle.  Refused (-1, outputs untouched): rows (sr_cache_add) or queries
- * (sr_cache_topk) with a non-finite component or one of magnitude above 65504; sr_cache_topk_dev and
- * sr_cache_topk_packed_dev, which see only fp16 queries -- scan each shard with sr_cache_topk and merge the lists with
- * sr_cache_merge_topk, which is exact on exact scores.  Lifecycle calls keep both stores in step. */
+ * route).  No scan waits on the host: how many queries fell back stays on the device.  Refused (-1, outputs untouched):
+ * rows (sr_cache_add) or queries (sr_cache_topk) with a non-finite component or one of magnitude above 65504;
+ * sr_cache_topk_dev and sr_cache_topk_packed_dev, which see only fp16 queries -- device-resident queries of an exact cache
+ * go through sr_cache_topk_f32_dev and sr_cache_topk_packed_f32_dev, and a sharded exact cache merges its shards' lists
+ * with sr_cache_merge_packed_dev or sr_cache_merge_topk, which are exact on exact scores.  Lifecycle calls keep both
+ * stores in step. */
 SR_API int sr_cache_create_exact(int device, int capacity, int dim, int id_offset, int sum_rule, sr_cache** out);
 SR_API void sr_cache_free(sr_cache* c);
 /* Append n rows (float32 host, rounded to fp16 on upload); returns first local row index or -1. */
@@ -195,8 +197,20 @@ SR_API int sr_cache_topk(sr_cache* c, const float* queries, int b, int k, int32_
 /* device-resident variant: d_queries fp16 [b, dim]; results in device buffers owned by the cache, valid until the next
  * scan of this cache.  Asynchronous on `cuda_stream`: growing the scratch and queueing the scan are locked, but callers
  * that share one cache through this entry serialise "scan, then read the results" themselves (sr_cache_topk and
- * sr_cache_lookup_ids do it under the cache's lock). */
+ * sr_cache_lookup_ids do it under the cache's lock).  Refused (-1) for exact caches: use sr_cache_topk_f32_dev. */
 SR_API int sr_cache_topk_dev(sr_cache* c, const void* d_queries_f16, int b, int k, void* cuda_stream);
+/* device-resident variant for fp32 queries, and the one for exact caches: d_queries_f32 device [b, dim] fp32, rounded to
+ * fp16 into the cache's own query buffer for the candidate scan; results where sr_cache_topk_dev puts them, with its
+ * limits and its rule that callers of one cache serialise "scan, then read".  Default cache: bitwise sr_cache_topk on the
+ * same queries.  Exact cache: bitwise sr_cache_topk on the same queries under the cache's sum rule; a query with a
+ * non-finite component or one above 65504 in magnitude, which sr_cache_topk refuses on the host, is refused here on the
+ * device: its k results are (-1, -inf) and the batch's other queries are unaffected.  Asynchronous: nothing waits on the
+ * host between the call and the stream reaching its results, except the scratch growth of the first call at a larger
+ * (b, k) or after the store grew (it synchronises the device).  So the scan can be captured into a CUDA graph after one
+ * eager call at the same (b, k).  A captured scan stays valid across sr_cache_set_valid / sr_cache_invalidate /
+ * sr_cache_move; after sr_cache_add, sr_cache_truncate or sr_cache_compact capture again: the row count, the largest row
+ * norm and the scratch are arguments of the captured launches. */
+SR_API int sr_cache_topk_f32_dev(sr_cache* c, const float* d_queries_f32, int b, int k, void* cuda_stream);
 SR_API const int32_t* sr_cache_dev_idx(const sr_cache* c);
 /* Sharded cache (SURVEY 8e): every rank scans its row shard for the whole query batch, the per-rank [b,k] lists travel
  * as 8-byte entries {float score, int32 GLOBAL id} (b * k * 8 bytes per rank through ONE all-gather over NVLink), and
@@ -206,6 +220,12 @@ SR_API const int32_t* sr_cache_dev_idx(const sr_cache* c);
  * of the collective).  sr_cache_merge_packed_dev: d_pairs_parts [g][b,k] entries -> d_out_idx / d_out_score [b,k];
  * g * k <= 6144 (every entry of a query in 48 KB of shared memory), -1 with the outputs untouched beyond that. */
 SR_API int sr_cache_topk_packed_dev(sr_cache* c, const void* d_queries_f16, int b, int k, void* d_pairs_out, void* cuda_stream);
+/* sr_cache_topk_f32_dev + pack into d_pairs_out [b,k]: the sharded scan of exact caches (and of default caches fed fp32
+ * queries).  Each exact shard's list holds the exact scores of its own rows, so sr_cache_merge_packed_dev of the shards'
+ * lists is the unsharded exact cache's result; a query refused on the device is (-1, -inf) in every shard and merges to
+ * (-1, -inf).  sr_cache_topk_packed_dev refuses exact caches. */
+SR_API int sr_cache_topk_packed_f32_dev(sr_cache* c, const float* d_queries_f32, int b, int k, void* d_pairs_out,
+                                        void* cuda_stream);
 SR_API int sr_cache_merge_packed_dev(int device, const void* d_pairs_parts, int g, int b, int k, int32_t* d_out_idx,
                                      float* d_out_score, void* cuda_stream);
 SR_API const float* sr_cache_dev_score(const sr_cache* c);

@@ -80,10 +80,12 @@ SR_API int sr_test_gemm_desc(const sr_gemm_desc* d, int* topk_lists);
  * query (fused: the upper bound).  Returns -1 (route -1) wherever sr_cache_topk refuses the shape. */
 SR_API int sr_test_cache_plan(int b, int n, int dim, int k, int* route, int* chunks, int* candidates);
 /* The last scan of an exact cache (sr_cache_create_exact) over b queries, per query: path 0 when its band of possible
- * winners was certified inside the candidates of the fp16 scan, 1 when it fell back to the exhaustive exact scan; band = the
- * candidates at or above s16_(k) - 2 eps (for a fallback query: all of them); eps = the bound on |fp16-operand score - Go
- * score| (csrc/cache_scan.cu exact_eps).  candidates = k' of that scan, fallback = its fallback queries (either may be
- * null).  -1 for a cache that is not exact or whose last scan had another b. */
+ * winners was certified inside the candidates of the fp16 scan, 1 when it fell back to the exhaustive exact scan, 2 when
+ * the device refused it (a component out of range; band and eps 0); band = the candidates at or above s16_(k) - 2 eps (for
+ * a fallback query: all of them); eps = the bound on |fp16-operand score - Go score| (csrc/cache_scan.cu exact_eps).
+ * candidates = k' of that scan, fallback = its fallback queries, read from the device at this call (either may be null).
+ * After a device-resident scan, call it once the scan's stream has reached its results.  -1 for a cache that is not exact
+ * or whose last scan had another b. */
 SR_API int sr_test_cache_exact_stats(sr_cache* c, int b, int32_t* path, int32_t* band, double* eps, int* candidates,
                                      int* fallback);
 SR_API int sr_test_hl_to_f32(const void* hi_f16, const void* lo_f16, const float* pivot, int t, int hdim, float* x);

@@ -87,6 +87,8 @@ def load_library(path: Optional[str] = None):
     L.sr_cache_dev_score.restype = vp
     L.sr_cache_merge_topk.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp]
     L.sr_cache_topk_packed_dev.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp]
+    L.sr_cache_topk_f32_dev.argtypes = [vp, vp, C.c_int, C.c_int, vp]
+    L.sr_cache_topk_packed_f32_dev.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp]
     L.sr_cache_merge_packed_dev.argtypes = [C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     _attach_hooks(L)
     _lib = L

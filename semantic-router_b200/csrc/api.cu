@@ -344,7 +344,7 @@ int sr_cache_lookup_ids(sr_model* h, sr_cache* c, const int32_t* ids, const int3
     h->q16_elems = n;
   }
   if (cast_rows_f16(m.stream, w.emb, n, h->q16)) return fail("cast failed");
-  // an exact cache scores the fp32 embedding itself; the fp16 copy only feeds its candidate scan
+  // an exact cache scores the fp32 embedding itself (and rounds its own fp16 copy for its candidate scan)
   if (cache_topk_dev_locked(c, h->q16, w.emb, batch, k, m.stream)) return fail("cache scan failed");
   cudaMemcpyAsync(out_idx, sr_cache_dev_idx(c), static_cast<size_t>(batch) * k * 4, cudaMemcpyDeviceToHost, m.stream);
   cudaMemcpyAsync(out_score, sr_cache_dev_score(c), static_cast<size_t>(batch) * k * 4, cudaMemcpyDeviceToHost, m.stream);

@@ -29,7 +29,7 @@ struct sr_cache {
   std::mutex mu;
   // exact caches (sr_cache_create_exact): the rows as passed to sr_cache_add, bit for bit, beside the fp16 copy the scan
   // reads; the largest L2 norm any row ever added had (removing rows leaves it an upper bound); the record of the last
-  // scan per query (sr_test_cache_exact_stats)
+  // scan per query (sr_test_cache_exact_stats), its fallback count left on the device where the scan keeps it
   bool exact = false;
   int sum_rule = 0;
   float* rows32 = nullptr;
@@ -37,7 +37,8 @@ struct sr_cache {
   int* d_path = nullptr;
   int* d_band = nullptr;
   double* d_eps = nullptr;
-  int last_b = 0, last_kc = 0, last_fallback = 0;
+  int last_b = 0, last_kc = 0;
+  const int* last_fallback = nullptr;
 };
 
 namespace {
@@ -99,24 +100,33 @@ int ensure(sr_cache* c, int b, int k) {
   }
   return 0;
 }
-// d_queries_f32: the queries before their fp16 rounding, which an exact cache scores with (null: refused there)
+// d_queries_f32: the queries before their fp16 rounding, which an exact cache scores with (null: refused there); an exact
+// cache rounds them to fp16 into its own query buffer itself and does not read d_queries_f16
 int topk_dev_locked(sr_cache* c, const void* d_queries_f16, const float* d_queries_f32, int b, int k, void* cuda_stream) {
-  if (c->exact && !d_queries_f32) return cfail("sr_cache_topk: an exact cache needs the fp32 queries (sr_cache_topk)");
+  if (c->exact && !d_queries_f32)
+    return cfail("sr_cache_topk: an exact cache needs the fp32 queries (sr_cache_topk, sr_cache_topk_f32_dev)");
   cudaSetDevice(c->device);
   if (ensure(c, b, k)) return cfail("sr_cache_topk: allocation failed");
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : c->stream;
-  const __half* q16 = static_cast<const __half*>(d_queries_f16);
   if (!c->exact)
-    return cache_topk(s, q16, b, c->rows, c->valid, c->size, c->dim, k, c->id_offset, c->d_idx, c->d_score, c->ws,
-                      c->ws_bytes);
-  int fallback = 0;
-  if (cache_topk_exact(s, d_queries_f32, q16, b, c->rows, c->rows32, c->valid, c->size, c->dim, c->rmax, k, c->sum_rule,
-                       c->id_offset, c->d_idx, c->d_score, c->ws, c->ws_bytes, c->d_path, c->d_band, c->d_eps, &fallback))
+    return cache_topk(s, static_cast<const __half*>(d_queries_f16), b, c->rows, c->valid, c->size, c->dim, k, c->id_offset,
+                      c->d_idx, c->d_score, c->ws, c->ws_bytes);
+  if (cache_topk_exact(s, d_queries_f32, c->d_q, b, c->rows, c->rows32, c->valid, c->size, c->dim, c->rmax, k, c->sum_rule,
+                       c->id_offset, c->d_idx, c->d_score, c->ws, c->ws_bytes, c->d_path, c->d_band, c->d_eps))
     return -1;
   c->last_b = b;
   c->last_kc = cache_exact_candidates(b, c->size, c->dim, k);
-  c->last_fallback = fallback;
+  c->last_fallback = cache_exact_fallback_count(c->ws, b, c->size, c->dim, k);
   return 0;
+}
+// fp32 queries on the device [b, dim]: a default cache rounds them to fp16 into its own query buffer (as sr_cache_topk
+// always has) and scans that; an exact cache scores them as they are
+int topk_f32_locked(sr_cache* c, const float* d_queries_f32, int b, int k, void* cuda_stream) {
+  cudaSetDevice(c->device);
+  if (ensure(c, b, k)) return cfail("sr_cache_topk: allocation failed");
+  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : c->stream;
+  if (!c->exact && srb::cast_rows_f16(s, d_queries_f32, static_cast<size_t>(b) * c->dim, c->d_q)) return -1;
+  return topk_dev_locked(c, c->d_q, d_queries_f32, b, k, cuda_stream);
 }
 }  // namespace
 
@@ -136,7 +146,10 @@ int cache_exact_stats(sr_cache* c, int b, int32_t* path, int32_t* band, double* 
       cudaMemcpy(eps, c->d_eps, static_cast<size_t>(b) * 8, cudaMemcpyDeviceToHost) != cudaSuccess)
     return -1;
   if (candidates) *candidates = c->last_kc;
-  if (fallback) *fallback = c->last_fallback;
+  if (fallback) {
+    *fallback = 0;
+    if (c->last_fallback && cudaMemcpy(fallback, c->last_fallback, 4, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+  }
   return 0;
 }
 }  // namespace srb
@@ -341,8 +354,7 @@ int sr_cache_topk(sr_cache* c, const float* queries, int b, int k, int32_t* out_
   // large b
   const size_t nq = static_cast<size_t>(b) * c->dim;
   if (cudaMemcpyAsync(c->d_q32, queries, nq * 4, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) return -1;
-  if (srb::cast_rows_f16(c->stream, c->d_q32, nq, c->d_q)) return -1;
-  if (topk_dev_locked(c, c->d_q, c->d_q32, b, k, nullptr)) return -1;
+  if (topk_f32_locked(c, c->d_q32, b, k, nullptr)) return -1;
   cudaMemcpyAsync(out_idx, c->d_idx, static_cast<size_t>(b) * k * 4, cudaMemcpyDeviceToHost, c->stream);
   cudaMemcpyAsync(out_score, c->d_score, static_cast<size_t>(b) * k * 4, cudaMemcpyDeviceToHost, c->stream);
   const cudaError_t e = cudaStreamSynchronize(c->stream);
@@ -354,6 +366,20 @@ int sr_cache_topk_packed_dev(sr_cache* c, const void* d_queries_f16, int b, int 
   if (!c || b <= 0 || k <= 0 || !d_pairs_out) return -1;
   std::lock_guard<std::mutex> lk(c->mu);
   if (topk_dev_locked(c, d_queries_f16, nullptr, b, k, cuda_stream)) return -1;
+  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : c->stream;
+  return cache_pack_pairs(s, c->d_idx, c->d_score, b * k, d_pairs_out);
+}
+
+int sr_cache_topk_f32_dev(sr_cache* c, const float* d_queries_f32, int b, int k, void* cuda_stream) {
+  if (!c || !d_queries_f32 || b <= 0 || k <= 0) return -1;
+  std::lock_guard<std::mutex> lk(c->mu);
+  return topk_f32_locked(c, d_queries_f32, b, k, cuda_stream);
+}
+
+int sr_cache_topk_packed_f32_dev(sr_cache* c, const float* d_queries_f32, int b, int k, void* d_pairs_out, void* cuda_stream) {
+  if (!c || !d_queries_f32 || b <= 0 || k <= 0 || !d_pairs_out) return -1;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (topk_f32_locked(c, d_queries_f32, b, k, cuda_stream)) return -1;
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : c->stream;
   return cache_pack_pairs(s, c->d_idx, c->d_score, b * k, d_pairs_out);
 }

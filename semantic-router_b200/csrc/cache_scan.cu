@@ -78,15 +78,15 @@ __device__ __forceinline__ Cand warp_argmax(Cand c) {   // every lane ends up wi
 // of the score GEMM it follows.)
 constexpr int kListCap = 128;   // candidates per warp
 
-__global__ void __launch_bounds__(kSelThreads)
-select_stage1(const float* __restrict__ scores, int ld, int n, int row0, const uint8_t* __restrict__ valid,
-              int k, int seg0, int total_segments, int* __restrict__ cand_idx, float* __restrict__ cand_score) {
+// stage 1 of one (query, segment)
+__device__ __forceinline__ void stage1_item(const float* __restrict__ scores, int ld, int n, int row0,
+                                            const uint8_t* __restrict__ valid, int k, int seg0, int total_segments,
+                                            int* __restrict__ cand_idx, float* __restrict__ cand_score, int q, int seg) {
   constexpr int kWarps = kSelThreads / 32;
   __shared__ float lv[kWarps][kListCap];
   __shared__ int li[kWarps][kListCap];
   __shared__ float wv[kWarps * 64];
   __shared__ int wi[kWarps * 64];
-  const int q = blockIdx.y, seg = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = lane_id();
   const int base = seg * kSegment + warp * (kSegment / kWarps);   // first local row of this warp's 1024 scores
   const float* s = scores + static_cast<size_t>(q) * ld + base;
@@ -150,21 +150,42 @@ select_stage1(const float* __restrict__ scores, int ld, int n, int row0, const u
     }
   }
   __syncthreads();
-  if (warp != 0) return;
-  int* oi = cand_idx + (static_cast<size_t>(q) * total_segments + seg0 + seg) * k;
-  float* os = cand_score + (static_cast<size_t>(q) * total_segments + seg0 + seg) * k;
-  for (int r = 0; r < k; ++r) {
-    Cand c{-INFINITY, -1};
-    int where = -1;
-    for (int w = 0; w < kWarps; ++w)
-      for (int t = lane; t < k; t += 32) {
-        const int at = w * 64 + t;
-        if (better(wv[at], wi[at], c.v, c.i)) { c.v = wv[at]; c.i = wi[at]; where = at; }
-      }
-    const Cand b = warp_argmax(c);
-    if (where >= 0 && b.i >= 0 && c.i == b.i) wi[where] = -1;
-    __syncwarp();
-    if (lane == 0) { oi[r] = b.i; os[r] = b.i >= 0 ? b.v : -INFINITY; }
+  if (warp == 0) {
+    int* oi = cand_idx + (static_cast<size_t>(q) * total_segments + seg0 + seg) * k;
+    float* os = cand_score + (static_cast<size_t>(q) * total_segments + seg0 + seg) * k;
+    for (int r = 0; r < k; ++r) {
+      Cand c{-INFINITY, -1};
+      int where = -1;
+      for (int w = 0; w < kWarps; ++w)
+        for (int t = lane; t < k; t += 32) {
+          const int at = w * 64 + t;
+          if (better(wv[at], wi[at], c.v, c.i)) { c.v = wv[at]; c.i = wi[at]; where = at; }
+        }
+      const Cand b = warp_argmax(c);
+      if (where >= 0 && b.i >= 0 && c.i == b.i) wi[where] = -1;
+      __syncwarp();
+      if (lane == 0) { oi[r] = b.i; os[r] = b.i >= 0 ? b.v : -INFINITY; }
+    }
+  }
+}
+
+// one CTA per (query, segment): grid (segments of the chunk, B)
+__global__ void __launch_bounds__(kSelThreads)
+select_stage1(const float* __restrict__ scores, int ld, int n, int row0, const uint8_t* __restrict__ valid,
+              int k, int seg0, int total_segments, int* __restrict__ cand_idx, float* __restrict__ cand_score) {
+  stage1_item(scores, ld, n, row0, valid, k, seg0, total_segments, cand_idx, cand_score, blockIdx.y, blockIdx.x);
+}
+
+// The same over *nq queries, a number read on the device: the CTAs of a fixed grid stride over its (query, segment)
+// pairs.  The exact scan's fallback, whose query count the host never learns.
+__global__ void __launch_bounds__(kSelThreads)
+select_stage1_counted(const float* __restrict__ scores, int ld, int n, int row0, const uint8_t* __restrict__ valid,
+                      int k, int seg0, int total_segments, int* __restrict__ cand_idx, float* __restrict__ cand_score,
+                      const int* __restrict__ nq) {
+  const int nseg = (n + kSegment - 1) / kSegment, items = *nq * nseg;
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    stage1_item(scores, ld, n, row0, valid, k, seg0, total_segments, cand_idx, cand_score, item / nseg, item % nseg);
+    __syncthreads();   // warp 0 has read wv / wi before the next item rewrites them
   }
 }
 
@@ -212,20 +233,19 @@ scores_small_kernel(const __half* __restrict__ queries, const __half* __restrict
 }
 
 // per query: top-k over `ncand` candidates; writes global ids (local + id_offset)
-__global__ void __launch_bounds__(kSelThreads)
-select_stage2(const int* __restrict__ cand_idx, const float* __restrict__ cand_score, int ncand, int k, int id_offset,
-              int* __restrict__ out_idx, float* __restrict__ out_score) {
+__device__ __forceinline__ void stage2_item(const int* __restrict__ cand_idx, const float* __restrict__ cand_score,
+                                            int ncand, int k, int id_offset, int* __restrict__ out_idx,
+                                            float* __restrict__ out_score, int q) {
   __shared__ Cand red[kSelThreads / 32];
   extern __shared__ uint8_t dyn[];
   float* sv = reinterpret_cast<float*>(dyn);
   int* si = reinterpret_cast<int*>(sv + ncand);
-  const int q = blockIdx.x;
   for (int c = threadIdx.x; c < ncand; c += kSelThreads) {
     sv[c] = cand_score[static_cast<size_t>(q) * ncand + c];
     si[c] = cand_idx[static_cast<size_t>(q) * ncand + c];
   }
   __syncthreads();
-  for (int r = 0; r < k; ++r) {
+  for (int r = 0; r < k; ++r) {   // each round ends on a barrier
     Cand c{-INFINITY, -1};
     int where = -1;
     for (int j = threadIdx.x; j < ncand; j += kSelThreads)
@@ -238,6 +258,23 @@ select_stage2(const int* __restrict__ cand_idx, const float* __restrict__ cand_s
     }
     __syncthreads();
   }
+}
+
+// one CTA per query
+__global__ void __launch_bounds__(kSelThreads)
+select_stage2(const int* __restrict__ cand_idx, const float* __restrict__ cand_score, int ncand, int k, int id_offset,
+              int* __restrict__ out_idx, float* __restrict__ out_score) {
+  stage2_item(cand_idx, cand_score, ncand, k, id_offset, out_idx, out_score, blockIdx.x);
+}
+
+// over *nq queries, read on the device, by a fixed grid (the exact scan's fallback, as select_stage1_counted); the last
+// round's barrier of one query lets the next one's loads overwrite sv / si
+__global__ void __launch_bounds__(kSelThreads)
+select_stage2_counted(const int* __restrict__ cand_idx, const float* __restrict__ cand_score, int ncand, int k,
+                      int id_offset, int* __restrict__ out_idx, float* __restrict__ out_score, const int* __restrict__ nq) {
+  const int queries = *nq;
+  for (int q = blockIdx.x; q < queries; q += gridDim.x)
+    stage2_item(cand_idx, cand_score, ncand, k, id_offset, out_idx, out_score, q);
 }
 
 // Exchange format of a sharded cache (SURVEY 8e): one 8-byte entry per (query, rank) = {fp32 score, int32 GLOBAL id}.
@@ -279,6 +316,15 @@ merge_packed_kernel(const int2* __restrict__ pairs, int G, int B, int k, int* __
 }
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+int sm_count() {   // of the current device; the devices of one process are taken to be alike
+  static int num_sms = 0;
+  if (!num_sms) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+      return 1;
+  }
+  return num_sms;
+}
 inline int chunk_rows(int B, int N) {
   // keep the score buffer <= 1 GiB; multiple of the stage-1 segment
   size_t rows = (static_cast<size_t>(1) << 30) / (static_cast<size_t>(B > 0 ? B : 1) * 4);
@@ -377,13 +423,7 @@ int cache_topk(cudaStream_t stream, const __half* queries, int B, const __half* 
     const int n = (N - row0) < chunk ? (N - row0) : chunk;
     const int n_pad = static_cast<int>(align_up(n, 64));  // cache allocation is padded to 256 rows
     if (plan.route == CACHE_GEMV) {
-      static int num_sms = 0;
-      if (!num_sms) {
-        int dev = 0;
-        SRB_CUDA_CHECK(cudaGetDevice(&dev));
-        SRB_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-      }
-      const int grid = num_sms * 8;   // 8 CTAs x 8 warps per SM: enough loads in flight to cover the HBM latency
+      const int grid = sm_count() * 8;   // 8 CTAs x 8 warps per SM: enough loads in flight to cover the HBM latency
       const size_t smem = static_cast<size_t>(B) * D * 4;
       const __half* cw = cache + static_cast<size_t>(row0) * D;
       switch (B) {
@@ -483,9 +523,28 @@ __device__ __forceinline__ float go_term(float acc, float a, float b) {
   return kRule == 0 ? __fadd_rn(acc, __fmul_rn(a, b)) : __fmaf_rn(a, b, acc);
 }
 
+// What the bound eps covers (and sr_cache_topk checks on the host): a finite component of magnitude <= 65504, which
+// rounds to a finite fp16 value.  NaN fails the comparison too.
+__device__ __forceinline__ bool exact_in_range(float x) { return fabsf(x) <= 65504.f; }
+
+// The fp16 copy of the queries that feeds the candidate scan, one CTA per query: round to nearest, as cast_rows_f16; a
+// query with a component out of range is written as zeros instead, so that no NaN reaches the candidate selection
+// (exact_band_kernel refuses that query).
+__global__ void __launch_bounds__(256)
+exact_query_f16_kernel(const float* __restrict__ queries, int D, __half* __restrict__ out) {
+  const float* x = queries + static_cast<size_t>(blockIdx.x) * D;
+  __half* y = out + static_cast<size_t>(blockIdx.x) * D;
+  bool bad = false;
+  for (int i = threadIdx.x; i < D; i += blockDim.x) bad |= !exact_in_range(x[i]);
+  bad = __syncthreads_or(bad);
+  for (int i = threadIdx.x; i < D; i += blockDim.x) y[i] = __float2half_rn(bad ? 0.f : x[i]);
+}
+
 // One CTA per query, one thread per candidate.  Certifies the band (see above); a certified query's band members are
 // rescored in Go order from the fp32 row and fp32 query, ranked, and its k results written; any other query is appended
-// to the fallback list and left to exact_scores_kernel.  path / band / eps: the test hook's record of the query.
+// to the fallback list and left to exact_scores_kernel.  A query with a component out of range is refused: its k results
+// are (-1, -inf) and it never reaches the fallback.  path / band / eps: the test hook's record of the query (path 0
+// certified, 1 fallback, 2 refused with band and eps 0).
 template <int kRule>
 __global__ void __launch_bounds__(kExactCand)
 exact_band_kernel(const float* __restrict__ queries, const float* __restrict__ rows32, int D, double rmax,
@@ -499,16 +558,25 @@ exact_band_kernel(const float* __restrict__ queries, const float* __restrict__ r
   __shared__ int order[kExactCand];
   const int q = blockIdx.x, t = threadIdx.x;
   double ss = 0;
+  bool bad = false;
   for (int i = t; i < D; i += kExactCand) {
     const float x = queries[static_cast<size_t>(q) * D + i];
     qs[i] = x;
     ss += static_cast<double>(x) * x;
+    bad |= !exact_in_range(x);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
   if (lane_id() == 0) red[t >> 5] = ss;
   order[t] = -1;
-  __syncthreads();
+  if (__syncthreads_or(bad)) {
+    if (t == 0) { path[q] = 2; band[q] = 0; eps[q] = 0; }
+    if (t < k) {
+      out_idx[static_cast<size_t>(q) * k + t] = -1;
+      out_score[static_cast<size_t>(q) * k + t] = -INFINITY;
+    }
+    return;
+  }
   const double e = exact_eps(sqrt(red[0] + red[1]), rmax, D);
   const int* ci = cand_idx + static_cast<size_t>(q) * kc;
   const float* cs = cand_score + static_cast<size_t>(q) * kc;
@@ -550,10 +618,11 @@ exact_band_kernel(const float* __restrict__ queries, const float* __restrict__ r
   }
 }
 
-// Exhaustive Go-order scores of the fallback queries: scores[j, row] for the nq queries listed in fb_list (rows of
-// `queries`) against rows [0, n) of rows32.  A register-tiled SIMT product, 32 queries x 128 rows per CTA, 4 x 4 per
+// Exhaustive Go-order scores of the fallback queries: scores[j, row] for the *fb_count queries listed in fb_list (rows of
+// `queries`) against rows [0, n) of rows32.  A register-tiled SIMT product, 32 queries x 128 rows per tile, 4 x 4 per
 // thread; every accumulator takes its D terms one at a time in index order (the K loop is never split), which is the
-// Go sum.
+// Go sum.  The count stays on the device: a fixed grid strides over the tiles it implies, so with no fallback every CTA
+// reads the count and exits.
 constexpr int kXq = 32, kXr = 128, kXk = 8;
 template <int kRule>
 __global__ void __launch_bounds__(256)
@@ -562,61 +631,71 @@ exact_scores_kernel(const float* __restrict__ queries, const int* __restrict__ f
   __shared__ float qs[kXk][kXq];
   __shared__ float rs[kXk][kXr + 4];
   const int nq = *fb_count;
-  const int q0 = blockIdx.y * kXq, r0 = blockIdx.x * kXr;
-  if (q0 >= nq) return;
+  const int rtiles = (n + kXr - 1) / kXr, tiles = (nq + kXq - 1) / kXq * rtiles;
   const int tq = threadIdx.x >> 5, tr = threadIdx.x & 31;    // queries q0 + tq * 4 + i, rows r0 + tr + 32 j
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  // loaders: thread -> (query, two k), and (row, k half)
-  const int lq = threadIdx.x >> 3, lk = threadIdx.x & 7;
-  const float* qrow = (q0 + lq < nq) ? queries + static_cast<size_t>(fb_list[q0 + lq]) * D : nullptr;
+  const int lq = threadIdx.x >> 3, lk = threadIdx.x & 7;     // loaders: thread -> (query, k), and (row, k half)
   const int lr = threadIdx.x >> 1, lh = (threadIdx.x & 1) * 4;
-  const float* rrow = (r0 + lr < n) ? rows32 + static_cast<size_t>(r0 + lr) * D : nullptr;
-  for (int k0 = 0; k0 < D; k0 += kXk) {
-    qs[lk][lq] = qrow ? qrow[k0 + lk] : 0.f;
-    const float4 r = rrow ? __ldg(reinterpret_cast<const float4*>(rrow + k0 + lh)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    rs[lh][lr] = r.x; rs[lh + 1][lr] = r.y; rs[lh + 2][lr] = r.z; rs[lh + 3][lr] = r.w;
-    __syncthreads();
+  for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int q0 = tile / rtiles * kXq, r0 = tile % rtiles * kXr;
+    float acc[4][4];
 #pragma unroll
-    for (int kk = 0; kk < kXk; ++kk) {
-      float a[4], b[4];
+    for (int i = 0; i < 4; ++i)
 #pragma unroll
-      for (int i = 0; i < 4; ++i) a[i] = qs[kk][tq * 4 + i];
+      for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    const float* qrow = (q0 + lq < nq) ? queries + static_cast<size_t>(fb_list[q0 + lq]) * D : nullptr;
+    const float* rrow = (r0 + lr < n) ? rows32 + static_cast<size_t>(r0 + lr) * D : nullptr;
+    for (int k0 = 0; k0 < D; k0 += kXk) {   // ends on a barrier: the next tile's loads find qs / rs read
+      qs[lk][lq] = qrow ? qrow[k0 + lk] : 0.f;
+      const float4 r = rrow ? __ldg(reinterpret_cast<const float4*>(rrow + k0 + lh)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      rs[lh][lr] = r.x; rs[lh + 1][lr] = r.y; rs[lh + 2][lr] = r.z; rs[lh + 3][lr] = r.w;
+      __syncthreads();
 #pragma unroll
-      for (int j = 0; j < 4; ++j) b[j] = rs[kk][tr + 32 * j];
+      for (int kk = 0; kk < kXk; ++kk) {
+        float a[4], b[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 4; ++i) a[i] = qs[kk][tq * 4 + i];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = go_term<kRule>(acc[i][j], a[i], b[j]);
+        for (int j = 0; j < 4; ++j) b[j] = rs[kk][tr + 32 * j];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) acc[i][j] = go_term<kRule>(acc[i][j], a[i], b[j]);
+      }
+      __syncthreads();
     }
-    __syncthreads();
-  }
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int qq = q0 + tq * 4 + i;
-    if (qq >= nq) continue;
+    for (int i = 0; i < 4; ++i) {
+      const int qq = q0 + tq * 4 + i;
+      if (qq >= nq) continue;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int rr = r0 + tr + 32 * j;
-      if (rr < n) scores[static_cast<size_t>(qq) * ld + rr] = acc[i][j];
+      for (int j = 0; j < 4; ++j) {
+        const int rr = r0 + tr + 32 * j;
+        if (rr < n) scores[static_cast<size_t>(qq) * ld + rr] = acc[i][j];
+      }
     }
   }
 }
 
-// results of the compacted fallback queries back to their rows
+// results of the compacted fallback queries back to their rows (a fixed grid striding over the device's count)
 __global__ void exact_scatter_kernel(const int* __restrict__ fb_list, const int* __restrict__ fb_count, int k,
                                      const int* __restrict__ idx, const float* __restrict__ score, int* __restrict__ out_idx,
                                      float* __restrict__ out_score) {
-  const int j = blockIdx.x;
-  if (j >= *fb_count) return;
-  const int q = fb_list[j];
-  for (int r = threadIdx.x; r < k; r += blockDim.x) {
-    out_idx[static_cast<size_t>(q) * k + r] = idx[static_cast<size_t>(j) * k + r];
-    out_score[static_cast<size_t>(q) * k + r] = score[static_cast<size_t>(j) * k + r];
+  const int nq = *fb_count;
+  for (int j = blockIdx.x; j < nq; j += gridDim.x) {
+    const int q = fb_list[j];
+    for (int r = threadIdx.x; r < k; r += blockDim.x) {
+      out_idx[static_cast<size_t>(q) * k + r] = idx[static_cast<size_t>(j) * k + r];
+      out_score[static_cast<size_t>(q) * k + r] = score[static_cast<size_t>(j) * k + r];
+    }
   }
+}
+
+// CTAs of `kernel` that fit on the device at once (no dynamic shared memory): the fixed grid of the fallback's launches
+template <typename Kernel>
+int one_wave(Kernel kernel, int threads) {
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
+  return per_sm * sm_count();
 }
 
 // Workspace of cache_topk_exact: the candidate scan's (reused by the fallback's score chunks and selection), then the
@@ -657,11 +736,15 @@ ExactLayout exact_layout(int B, int N, int D, int k) {
 
 int cache_exact_candidates(int B, int N, int D, int k) { return exact_layout(B, N, D, k).kc; }
 size_t cache_topk_exact_workspace_bytes(int B, int N, int D, int k) { return exact_layout(B, N, D, k).total; }
+const int* cache_exact_fallback_count(const void* workspace, int B, int N, int D, int k) {
+  const ExactLayout L = exact_layout(B, N, D, k);
+  return L.kc ? reinterpret_cast<const int*>(static_cast<const uint8_t*>(workspace) + L.fb_list) : nullptr;
+}
 
-int cache_topk_exact(cudaStream_t stream, const float* queries32, const __half* queries16, int B, const __half* cache,
+int cache_topk_exact(cudaStream_t stream, const float* queries32, __half* queries16, int B, const __half* cache,
                      const float* cache32, const uint8_t* valid, int N, int D, double rmax, int k, int sum_rule,
                      int id_offset, int* out_idx, float* out_score, void* workspace, size_t workspace_bytes, int* path,
-                     int* band, double* eps, int* n_fallback) {
+                     int* band, double* eps) {
   if (B <= 0 || k <= 0) return 0;
   const ExactLayout L = exact_layout(B, N, D, k);
   if (L.kc == 0 || (sum_rule != 0 && sum_rule != 1)) {
@@ -678,6 +761,9 @@ int cache_topk_exact(cudaStream_t stream, const float* queries32, const __half* 
   float* cand_score = reinterpret_cast<float*>(ws + L.cand_score);
   int* fb_count = reinterpret_cast<int*>(ws + L.fb_list);
   int* fb_list = fb_count + 1;
+  exact_query_f16_kernel<<<B, 256, 0, stream>>>(queries32, D, queries16);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
   if (cache_topk(stream, queries16, B, cache, valid, N, D, L.kc, 0, cand_idx, cand_score, ws, L.scan.workspace_bytes))
     return -1;
   SRB_CUDA_CHECK(cudaMemsetAsync(fb_count, 0, 4, stream));
@@ -689,13 +775,14 @@ int cache_topk_exact(cudaStream_t stream, const float* queries32, const __half* 
                                                 out_idx, out_score, fb_list, fb_count, path, band, eps);
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
-  int nf = 0;
-  SRB_CUDA_CHECK(cudaMemcpyAsync(&nf, fb_count, 4, cudaMemcpyDeviceToHost, stream));
-  SRB_CUDA_CHECK(cudaStreamSynchronize(stream));
-  if (n_fallback) *n_fallback = nf;
-  if (nf == 0) return 0;
+  if (N == 0) return 0;   // every query of an empty store is certified
   // Exhaustive exact scan of the fallback queries only: Go-order scores in chunks, then the two-stage selection of
-  // cache_topk over them, then the results back to their query rows.
+  // cache_topk over them, then the results back to their query rows.  The number of fallback queries stays on the device
+  // (nothing waits for it on the host, so the scan can be captured into a CUDA graph): every launch below has a fixed grid
+  // of about one wave whose CTAs stride over the work that number implies, and with no fallback each is one short wave
+  // of early exits.
+  static const int scores_grid[2] = {one_wave(exact_scores_kernel<0>, 256), one_wave(exact_scores_kernel<1>, 256)};
+  static const int stage1_grid = one_wave(select_stage1_counted, kSelThreads);
   const CachePlan& P = L.fallback;
   const int chunk = P.chunk_rows;
   float* scores = reinterpret_cast<float*>(ws);
@@ -707,24 +794,24 @@ int cache_topk_exact(cudaStream_t stream, const float* queries32, const __half* 
   auto scores_kernel = sum_rule == 0 ? exact_scores_kernel<0> : exact_scores_kernel<1>;
   for (int row0 = 0; row0 < N; row0 += chunk) {
     const int n = (N - row0) < chunk ? (N - row0) : chunk;
-    const dim3 grid((n + kXr - 1) / kXr, (nf + kXq - 1) / kXq);
-    scores_kernel<<<grid, 256, 0, stream>>>(queries32, fb_list, fb_count, cache32 + static_cast<size_t>(row0) * D, n, D,
-                                            chunk, scores);
+    scores_kernel<<<scores_grid[sum_rule], 256, 0, stream>>>(queries32, fb_list, fb_count,
+                                                             cache32 + static_cast<size_t>(row0) * D, n, D, chunk, scores);
     SRB_CUDA_CHECK(cudaGetLastError());
     note_launch();
-    const dim3 sgrid((n + kSegment - 1) / kSegment, nf);
-    select_stage1<<<sgrid, kSelThreads, 0, stream>>>(scores, chunk, n, row0, valid, k, row0 / kSegment, P.segments,
-                                                     sel_idx, sel_score);
+    select_stage1_counted<<<stage1_grid, kSelThreads, 0, stream>>>(scores, chunk, n, row0, valid, k, row0 / kSegment,
+                                                                   P.segments, sel_idx, sel_score, fb_count);
     SRB_CUDA_CHECK(cudaGetLastError());
     note_launch();
   }
   const size_t smem = P.stage2_smem;
   if (smem + kSelStaticSmem > kDefaultSmem)
-    SRB_CUDA_CHECK(cudaFuncSetAttribute(select_stage2, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  select_stage2<<<nf, kSelThreads, smem, stream>>>(sel_idx, sel_score, P.candidates, k, id_offset, fb_idx, fb_score);
+    SRB_CUDA_CHECK(cudaFuncSetAttribute(select_stage2_counted, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        static_cast<int>(smem)));
+  select_stage2_counted<<<sm_count(), kSelThreads, smem, stream>>>(sel_idx, sel_score, P.candidates, k, id_offset, fb_idx,
+                                                                   fb_score, fb_count);
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
-  exact_scatter_kernel<<<nf, 64, 0, stream>>>(fb_list, fb_count, k, fb_idx, fb_score, out_idx, out_score);
+  exact_scatter_kernel<<<sm_count(), 64, 0, stream>>>(fb_list, fb_count, k, fb_idx, fb_score, out_idx, out_score);
   SRB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   return 0;

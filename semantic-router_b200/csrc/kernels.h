@@ -123,17 +123,20 @@ size_t cache_topk_workspace_bytes(int B, int N, int D, int k);
 
 // Exact caches: the same top-k with scores bitwise the reference's sequential fp32 dot product of the fp32 query
 // (queries32 [B,D]) and the fp32 rows (cache32 [N,D]), sum_rule 0 (product rounded, then added) or 1 (one fma per term).
-// The fp16 scan (queries16, cache) picks k' candidates per query; queries whose band of possible winners is not
-// certified within them are scanned exhaustively in Go order.  rmax >= every stored row's L2 norm.  path / band / eps
-// [B]: per query 0 certified or 1 fallback, the candidates in its band, its bound eps.  Synchronises `stream` once
-// (*n_fallback, the fallback queries, decides the exhaustive launches).  Refused (-1) where the two-stage selection at k
-// is (ceil(N / 8192) * k > 25600) and for D % 8 != 0.
+// The scan rounds the queries to fp16 into queries16 [B,D] (its own scratch) and the fp16 scan (queries16, cache) picks
+// k' candidates per query; queries whose band of possible winners is not certified within them are scanned exhaustively
+// in Go order.  A query with a non-finite component or one above 65504 in magnitude is refused on the device: its k
+// results are (-1, -inf).  rmax >= every stored row's L2 norm.  path / band / eps [B]: per query 0 certified, 1 fallback
+// or 2 refused, the candidates in its band, its bound eps.  Nothing waits on the host: the number of fallback queries
+// stays on the device (cache_exact_fallback_count points at it).  Refused (-1) where the two-stage selection at k is
+// (ceil(N / 8192) * k > 25600) and for D % 8 != 0.
 int cache_exact_candidates(int B, int N, int D, int k);   // k'; 0 where refused
 size_t cache_topk_exact_workspace_bytes(int B, int N, int D, int k);
-int cache_topk_exact(cudaStream_t stream, const float* queries32, const __half* queries16, int B, const __half* cache,
+const int* cache_exact_fallback_count(const void* workspace, int B, int N, int D, int k);   // device int; null where refused
+int cache_topk_exact(cudaStream_t stream, const float* queries32, __half* queries16, int B, const __half* cache,
                      const float* cache32, const uint8_t* valid, int N, int D, double rmax, int k, int sum_rule,
                      int id_offset, int* out_idx, float* out_score, void* workspace, size_t workspace_bytes, int* path,
-                     int* band, double* eps, int* n_fallback);
+                     int* band, double* eps);
 
 // sharded-cache exchange format: 8-byte entries {fp32 score, int32 global id}
 int cache_pack_pairs(cudaStream_t stream, const int* idx, const float* score, int n, void* pairs_out);

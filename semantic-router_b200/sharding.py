@@ -5,7 +5,8 @@
 * partitioned semantic cache: rank r owns rows [r*N/G, (r+1)*N/G); every rank scans its shard for the whole query
   batch (queries are replicated at enqueue), the per-shard [B,k] (score, GLOBAL id) lists are exchanged with ONE
   all-gather (B*k*8 bytes per rank: {fp32 score, int32 global id} entries; NCCL over NVLink on GPUs, gloo in the CPU tests) and merged with the reference
-  tie rule (descending score, lower global index first).
+  tie rule (descending score, lower global index first).  Exact caches take the same exchange with fp32 queries: each
+  shard's list holds the exact scores of its own rows, so the merge is the unsharded exact result.
 """
 from __future__ import annotations
 
@@ -62,21 +63,25 @@ def allgather_topk(idx, score, group=None):
     return merge_topk([gi[r].numpy() for r in range(world)], [gs[r].numpy() for r in range(world)])
 
 
-def sharded_topk_dev(cache, d_queries_f16, k: int, group=None):
+def sharded_topk_dev(cache, d_queries, k: int, group=None):
     """The whole sharded lookup on the device (cfg 4): scan this rank's shard for the (replicated) query batch, pack,
     all-gather 8-byte entries over NCCL, merge.  `cache`: binding.Cache holding this rank's rows with id_offset = first
-    global row; d_queries_f16: torch fp16 CUDA tensor [B, D].  Returns (idx int32 [B,k], score fp32 [B,k]) CUDA tensors,
-    identical on every rank.  Everything is queued on torch's current stream."""
+    global row; d_queries: torch CUDA tensor [B, D], fp16 (sr_cache_topk_packed_dev) or fp32
+    (sr_cache_topk_packed_f32_dev: the route of exact caches, whose merged lists are the unsharded exact result).
+    Returns (idx int32 [B,k], score fp32 [B,k]) CUDA tensors, identical on every rank.  Everything is queued on torch's
+    current stream."""
     import ctypes as C
     import torch
     from .binding import lib
-    b = d_queries_f16.shape[0]
-    dev = d_queries_f16.device
-    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    b = d_queries.shape[0]
+    dev = d_queries.device
+    # torch's default stream is the legacy stream, handle 0, which the C ABI reads as "the cache's own stream": name it
+    # cudaStreamLegacy (1) so that the scan is ordered before the all-gather
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream or 1)
     pairs = torch.empty((b, k, 2), dtype=torch.int32, device=dev)
-    if lib().sr_cache_topk_packed_dev(cache.handle, C.c_void_p(d_queries_f16.data_ptr()), b, k,
-                                      C.c_void_p(pairs.data_ptr()), stream) != 0:
-        raise RuntimeError("sr_cache_topk_packed_dev failed")
+    scan = lib().sr_cache_topk_packed_f32_dev if d_queries.dtype == torch.float32 else lib().sr_cache_topk_packed_dev
+    if scan(cache.handle, C.c_void_p(d_queries.data_ptr()), b, k, C.c_void_p(pairs.data_ptr()), stream) != 0:
+        raise RuntimeError(f"{scan.__name__} failed")
     gathered = _gather_pairs(pairs, group)
     oi = torch.empty((b, k), dtype=torch.int32, device=dev)
     os_ = torch.empty((b, k), dtype=torch.float32, device=dev)
