@@ -14,9 +14,19 @@
 
 using namespace srb;
 
+namespace {
+struct RowStore {   // one row per stored entry, row_bytes each
+  uint8_t* base;
+  size_t row_bytes;
+  uint8_t* row(size_t r) const { return base + r * row_bytes; }
+};
+}  // namespace
+
 struct sr_cache {
   int device = 0, capacity = 0, cap_pad = 0, dim = 0, id_offset = 0, size = 0;
   __half* rows = nullptr;
+  // every store of row data: the fp16 rows, then an exact cache's fp32 rows; moving or compacting rows moves them in each
+  std::vector<RowStore> stores;
   uint8_t* valid = nullptr;
   void* ws = nullptr;
   size_t ws_bytes = 0;
@@ -61,41 +71,37 @@ double checked_max_norm(const float* x, size_t n, int dim) {
   }
   return best;
 }
+// Frees p and allocates it anew at `bytes`; false, with p null, when that fails
+template <typename T>
+bool regrow(T*& p, size_t bytes) {
+  if (p) cudaFree(p);
+  p = nullptr;
+  if (cudaMalloc(reinterpret_cast<void**>(&p), bytes) == cudaSuccess) return true;
+  p = nullptr;
+  return false;
+}
 // Grows the per-cache scratch.  Caller holds c->mu.  Buffers may still be referenced by work queued on the cache's
 // stream or on a caller's stream (sr_cache_topk_dev), so everything on the device drains before anything is freed.
 int ensure(sr_cache* c, int b, int k) {
   const int n = c->size > 0 ? c->size : 1;
   const size_t need = c->exact ? cache_topk_exact_workspace_bytes(b, n, c->dim, k) : cache_topk_workspace_bytes(b, n, c->dim, k);
   if (b > c->q_cap || b * k > c->res_cap || need > c->ws_bytes) cudaDeviceSynchronize();
+  const size_t nb = static_cast<size_t>(b);
   if (b > c->q_cap) {
-    if (c->d_q) cudaFree(c->d_q);
-    if (c->d_q32) cudaFree(c->d_q32);
-    c->d_q = nullptr; c->d_q32 = nullptr; c->q_cap = 0;
-    if (cudaMalloc(reinterpret_cast<void**>(&c->d_q), static_cast<size_t>(b) * c->dim * 2) != cudaSuccess) return -1;
-    if (cudaMalloc(reinterpret_cast<void**>(&c->d_q32), static_cast<size_t>(b) * c->dim * 4) != cudaSuccess) return -1;
-    if (c->exact) {
-      for (void* p : {static_cast<void*>(c->d_path), static_cast<void*>(c->d_band), static_cast<void*>(c->d_eps)})
-        if (p) cudaFree(p);
-      c->d_path = nullptr; c->d_band = nullptr; c->d_eps = nullptr;
-      if (cudaMalloc(reinterpret_cast<void**>(&c->d_path), static_cast<size_t>(b) * 4) != cudaSuccess ||
-          cudaMalloc(reinterpret_cast<void**>(&c->d_band), static_cast<size_t>(b) * 4) != cudaSuccess ||
-          cudaMalloc(reinterpret_cast<void**>(&c->d_eps), static_cast<size_t>(b) * 8) != cudaSuccess)
-        return -1;
-    }
+    c->q_cap = 0;
+    if (!regrow(c->d_q, nb * c->dim * 2) || !regrow(c->d_q32, nb * c->dim * 4) ||
+        (c->exact && (!regrow(c->d_path, nb * 4) || !regrow(c->d_band, nb * 4) || !regrow(c->d_eps, nb * 8))))
+      return -1;
     c->q_cap = b;
   }
   if (b * k > c->res_cap) {
-    if (c->d_idx) cudaFree(c->d_idx);
-    if (c->d_score) cudaFree(c->d_score);
-    c->d_idx = nullptr; c->d_score = nullptr; c->res_cap = 0;
-    if (cudaMalloc(reinterpret_cast<void**>(&c->d_idx), static_cast<size_t>(b) * k * 4) != cudaSuccess) return -1;
-    if (cudaMalloc(reinterpret_cast<void**>(&c->d_score), static_cast<size_t>(b) * k * 4) != cudaSuccess) return -1;
+    c->res_cap = 0;
+    if (!regrow(c->d_idx, nb * k * 4) || !regrow(c->d_score, nb * k * 4)) return -1;
     c->res_cap = b * k;
   }
   if (need > c->ws_bytes) {
-    if (c->ws) cudaFree(c->ws);
-    c->ws = nullptr; c->ws_bytes = 0;
-    if (cudaMalloc(&c->ws, need) != cudaSuccess) { c->ws = nullptr; c->ws_bytes = 0; return -1; }
+    c->ws_bytes = 0;
+    if (!regrow(c->ws, need)) return -1;
     c->ws_bytes = need;
   }
   return 0;
@@ -174,6 +180,8 @@ static int cache_create(int device, int capacity, int dim, int id_offset, bool e
   }
   cudaMemset(c->rows, 0, static_cast<size_t>(c->cap_pad) * dim * 2);
   cudaMemset(c->valid, 0, c->cap_pad);
+  c->stores.push_back({reinterpret_cast<uint8_t*>(c->rows), static_cast<size_t>(dim) * 2});
+  if (exact) c->stores.push_back({reinterpret_cast<uint8_t*>(c->rows32), static_cast<size_t>(dim) * 4});
   *out = c;
   return 0;
 }
@@ -200,51 +208,35 @@ int sr_cache_add(sr_cache* c, const float* rows, int n) {
   if (!c || !rows || n <= 0) return -1;
   std::lock_guard<std::mutex> lk(c->mu);
   if (c->size + n > c->capacity) return cfail("sr_cache_add: capacity exceeded");
+  const double norm = c->exact ? checked_max_norm(rows, static_cast<size_t>(n), c->dim) : 0;
+  if (norm < 0) return cfail("sr_cache_add: an exact cache takes finite components of magnitude <= 65504 only");
   cudaSetDevice(c->device);
-  if (c->exact) {
-    // the fp32 rows go up as they are and the fp16 copy is rounded from them on the device
-    const double norm = checked_max_norm(rows, static_cast<size_t>(n), c->dim);
-    if (norm < 0) return cfail("sr_cache_add: an exact cache takes finite components of magnitude <= 65504 only");
-    const size_t ne = static_cast<size_t>(n) * c->dim;
-    float* dst = c->rows32 + static_cast<size_t>(c->size) * c->dim;
-    bool ok = cudaMemcpyAsync(dst, rows, ne * 4, cudaMemcpyHostToDevice, c->stream) == cudaSuccess &&
-              srb::cast_rows_f16(c->stream, dst, ne, c->rows + static_cast<size_t>(c->size) * c->dim) == 0 &&
-              cudaMemsetAsync(c->valid + c->size, 1, n, c->stream) == cudaSuccess;
-    ok = cudaStreamSynchronize(c->stream) == cudaSuccess && ok;
-    if (!ok) return cfail("sr_cache_add: H2D failed");
-    c->rmax = std::max(c->rmax, norm);
-    const int first = c->size;
-    c->size += n;
-    return first;
-  }
-  // fp32 up in pieces of <= 64 MiB, rounded to fp16 (rn) on the device straight into the store
+  // fp32 up in pieces of <= 64 MiB, rounded to fp16 (rn) on the device straight into the store.  An exact cache keeps the
+  // fp32 rows as they are, so its pieces go up into rows32 and the fp16 copy is rounded from there; a default cache stages
+  // them.
   const size_t piece_rows = std::max<size_t>(1, (64u << 20) / (static_cast<size_t>(c->dim) * 4));
   float* stage = nullptr;
-  if (cudaMalloc(reinterpret_cast<void**>(&stage), std::min<size_t>(piece_rows, n) * c->dim * 4) != cudaSuccess)
+  if (!c->exact &&
+      cudaMalloc(reinterpret_cast<void**>(&stage), std::min<size_t>(piece_rows, n) * c->dim * 4) != cudaSuccess)
     return cfail("sr_cache_add: allocation failed");
   bool ok = true;
   for (size_t r0 = 0; ok && r0 < static_cast<size_t>(n); r0 += piece_rows) {
-    const size_t nr = std::min<size_t>(piece_rows, n - r0), ne = nr * c->dim;
-    ok = cudaMemcpyAsync(stage, rows + r0 * c->dim, ne * 4, cudaMemcpyHostToDevice, c->stream) == cudaSuccess &&
-         srb::cast_rows_f16(c->stream, stage, ne, c->rows + (static_cast<size_t>(c->size) + r0) * c->dim) == 0;
+    const size_t nr = std::min<size_t>(piece_rows, n - r0), ne = nr * c->dim, at = (c->size + r0) * c->dim;
+    float* up = c->exact ? c->rows32 + at : stage;
+    ok = cudaMemcpyAsync(up, rows + r0 * c->dim, ne * 4, cudaMemcpyHostToDevice, c->stream) == cudaSuccess &&
+         srb::cast_rows_f16(c->stream, up, ne, c->rows + at) == 0;
   }
   ok = ok && cudaMemsetAsync(c->valid + c->size, 1, n, c->stream) == cudaSuccess;
   ok = cudaStreamSynchronize(c->stream) == cudaSuccess && ok;
-  cudaFree(stage);
+  if (stage) cudaFree(stage);
   if (!ok) return cfail("sr_cache_add: H2D failed");
+  c->rmax = std::max(c->rmax, norm);
   const int first = c->size;
   c->size += n;
   return first;
 }
 
-int sr_cache_invalidate(sr_cache* c, int local_row) {
-  if (!c) return -1;
-  std::lock_guard<std::mutex> lk(c->mu);
-  if (local_row < 0 || local_row >= c->size) return -1;
-  cudaSetDevice(c->device);
-  const uint8_t z = 0;
-  return cudaMemcpy(c->valid + local_row, &z, 1, cudaMemcpyHostToDevice) == cudaSuccess ? 0 : -1;
-}
+int sr_cache_invalidate(sr_cache* c, int local_row) { return sr_cache_set_valid(c, local_row, 0); }
 
 // ---- lifecycle mirror of the reference's entries slice (pkg/cache/inmemory_cache_lifecycle.go): the Go backend keeps
 // entries[i] <-> device row i, so eviction (swap with the last entry, :296-303), TTL cleanup (stable compaction, :120-137)
@@ -264,13 +256,9 @@ int sr_cache_move(sr_cache* c, int dst_row, int src_row) {
   if (dst_row < 0 || src_row < 0 || dst_row >= c->size || src_row >= c->size) return -1;
   if (dst_row == src_row) return 0;
   cudaSetDevice(c->device);
-  const size_t rb = static_cast<size_t>(c->dim) * 2;
-  bool ok = cudaMemcpyAsync(c->rows + static_cast<size_t>(dst_row) * c->dim, c->rows + static_cast<size_t>(src_row) * c->dim, rb,
-                            cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
-  ok = ok && cudaMemcpyAsync(c->valid + dst_row, c->valid + src_row, 1, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
-  if (c->exact)
-    ok = ok && cudaMemcpyAsync(c->rows32 + static_cast<size_t>(dst_row) * c->dim, c->rows32 + static_cast<size_t>(src_row) * c->dim,
-                               rb * 2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+  bool ok = cudaMemcpyAsync(c->valid + dst_row, c->valid + src_row, 1, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+  for (const RowStore& s : c->stores)
+    ok = ok && cudaMemcpyAsync(s.row(dst_row), s.row(src_row), s.row_bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
   return (cudaStreamSynchronize(c->stream) == cudaSuccess && ok) ? 0 : -1;
 }
 
@@ -296,8 +284,8 @@ int sr_cache_compact(sr_cache* c, const uint8_t* keep, int n) {
   if (first_drop == n) return n;                       // nothing to remove
   std::vector<uint8_t> valid(static_cast<size_t>(n));
   if (cudaMemcpy(valid.data(), c->valid, n, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-  const size_t rb = static_cast<size_t>(c->dim) * 2;
-  const size_t unit = c->exact ? 2 * rb : rb;   // an exact cache moves its fp32 rows through the same scratch
+  size_t unit = 0;   // every store's runs go through the same scratch, sized for the widest store's rows
+  for (const RowStore& s : c->stores) unit = std::max(unit, s.row_bytes);
   const int scratch_rows = static_cast<int>(std::min<size_t>(static_cast<size_t>(n), std::max<size_t>(1, (64u << 20) / unit)));
   void* scratch = nullptr;
   if (cudaMalloc(&scratch, static_cast<size_t>(scratch_rows) * unit) != cudaSuccess)
@@ -308,13 +296,11 @@ int sr_cache_compact(sr_cache* c, const uint8_t* keep, int n) {
     if (!keep[r]) { ++r; continue; }
     int e = r;
     while (e < n && keep[e] && e - r < scratch_rows) ++e;   // run [r, e) of kept rows -> [w, w + e - r)
-    const size_t bytes = static_cast<size_t>(e - r) * rb;
-    ok = cudaMemcpyAsync(scratch, c->rows + static_cast<size_t>(r) * c->dim, bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess &&
-         cudaMemcpyAsync(c->rows + static_cast<size_t>(w) * c->dim, scratch, bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
-    if (c->exact)
-      ok = ok &&
-           cudaMemcpyAsync(scratch, c->rows32 + static_cast<size_t>(r) * c->dim, 2 * bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess &&
-           cudaMemcpyAsync(c->rows32 + static_cast<size_t>(w) * c->dim, scratch, 2 * bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+    for (const RowStore& s : c->stores) {
+      const size_t bytes = static_cast<size_t>(e - r) * s.row_bytes;
+      ok = ok && cudaMemcpyAsync(scratch, s.row(r), bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess &&
+           cudaMemcpyAsync(s.row(w), scratch, bytes, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+    }
     for (int i = r; i < e; ++i) valid[w + (i - r)] = valid[i];
     w += e - r;
     r = e;

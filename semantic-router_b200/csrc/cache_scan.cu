@@ -15,6 +15,8 @@
 
 #include <algorithm>
 #include <initializer_list>
+#include <mutex>
+#include <unordered_map>
 
 #include "common.cuh"
 #include "gemm.h"
@@ -30,23 +32,26 @@ struct Cand {
   float v;
   int i;
 };
-// A launch gets 48 KB of shared memory without opting in, the kernel's static shared memory included: select_stage2 and
-// merge_packed_kernel hold one Cand per warp for block_argmax besides their dynamic candidate arrays.
+// A launch gets 48 KB of shared memory without opting in, the kernel's static shared memory included.
 constexpr size_t kDefaultSmem = 48 * 1024;
-constexpr size_t kSelStaticSmem = sizeof(Cand) * (kSelThreads / 32);
 __device__ __forceinline__ bool better(float v, int i, float bv, int bi) {
   // larger score wins; equal score: lower (non-negative) index wins; index -1 = nothing
   if (i < 0) return false;
   if (bi < 0) return true;
   return v > bv || (v == bv && i < bi);
 }
-__device__ __forceinline__ Cand block_argmax(Cand c, Cand* red) {
+__device__ __forceinline__ Cand warp_argmax(Cand c) {   // every lane ends up with the winner
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, c.v, o);
     const int oi = __shfl_xor_sync(0xffffffffu, c.i, o);
     if (better(ov, oi, c.v, c.i)) { c.v = ov; c.i = oi; }
   }
+  return c;
+}
+__device__ __forceinline__ Cand block_argmax(Cand c) {   // every thread ends up with the winner
+  __shared__ Cand red[kSelThreads / 32];
+  c = warp_argmax(c);
   const int warp = threadIdx.x >> 5;
   __syncthreads();
   if (lane_id() == 0) red[warp] = c;
@@ -58,14 +63,35 @@ __device__ __forceinline__ Cand block_argmax(Cand c, Cand* red) {
   return b;
 }
 
-__device__ __forceinline__ Cand warp_argmax(Cand c) {   // every lane ends up with the winner
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, c.v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, c.i, o);
-    if (better(ov, oi, c.v, c.i)) { c.v = ov; c.i = oi; }
+// k rounds of argmax over the n entries (v[t], i[t]) of a shared-memory list, each winner removed from the list; out(r, b)
+// receives rank r's winner b (b.i -1: the list ran out).  warp_select: one warp, out called on lane 0; block_select: the
+// whole CTA, out called on thread 0, every round ending on a barrier.
+template <class Out>
+__device__ __forceinline__ void warp_select(float* v, int* i, int n, int k, Out out) {
+  const int lane = lane_id();
+  for (int r = 0; r < k; ++r) {
+    Cand c{-INFINITY, -1};
+    int where = -1;
+    for (int t = lane; t < n; t += 32)
+      if (better(v[t], i[t], c.v, c.i)) { c.v = v[t]; c.i = i[t]; where = t; }
+    const Cand b = warp_argmax(c);
+    if (where >= 0 && b.i >= 0 && c.i == b.i) i[where] = -1;   // indices are unique: exactly one owner
+    __syncwarp();
+    if (lane == 0) out(r, b);
   }
-  return c;
+}
+template <class Out>
+__device__ __forceinline__ void block_select(float* v, int* i, int n, int k, Out out) {
+  for (int r = 0; r < k; ++r) {
+    Cand c{-INFINITY, -1};
+    int where = -1;
+    for (int t = threadIdx.x; t < n; t += kSelThreads)
+      if (better(v[t], i[t], c.v, c.i)) { c.v = v[t]; c.i = i[t]; where = t; }
+    const Cand b = block_argmax(c);
+    if (where >= 0 && c.i == b.i && b.i >= 0) i[where] = -1;   // indices are unique: exactly one owner
+    if (threadIdx.x == 0) out(r, b);
+    __syncthreads();
+  }
 }
 
 // scores: [B, ld] fp32 for local rows [row0, row0 + n); out: cand_idx/cand_score [B, total_segments, k]
@@ -85,7 +111,7 @@ __device__ __forceinline__ void stage1_item(const float* __restrict__ scores, in
   constexpr int kWarps = kSelThreads / 32;
   __shared__ float lv[kWarps][kListCap];
   __shared__ int li[kWarps][kListCap];
-  __shared__ float wv[kWarps * 64];
+  __shared__ float wv[kWarps * 64];   // warp w's k winners at [w * k, (w + 1) * k): one list of kWarps * k for warp 0
   __shared__ int wi[kWarps * 64];
   const int warp = threadIdx.x >> 5, lane = lane_id();
   const int base = seg * kSegment + warp * (kSegment / kWarps);   // first local row of this warp's 1024 scores
@@ -122,17 +148,10 @@ __device__ __forceinline__ void stage1_item(const float* __restrict__ scores, in
     count += __popc(m);
   }
   __syncwarp();
+  float* mv = wv + warp * k;
+  int* mi = wi + warp * k;
   if (count <= kListCap) {
-    for (int r = 0; r < k; ++r) {
-      Cand c{-INFINITY, -1};
-      int where = -1;
-      for (int t = lane; t < count; t += 32)
-        if (better(lv[warp][t], li[warp][t], c.v, c.i)) { c.v = lv[warp][t]; c.i = li[warp][t]; where = t; }
-      const Cand b = warp_argmax(c);
-      if (where >= 0 && b.i >= 0 && c.i == b.i) li[warp][where] = -1;   // indices are unique: exactly one owner
-      __syncwarp();
-      if (lane == 0) { wv[warp * 64 + r] = b.i >= 0 ? b.v : -INFINITY; wi[warp * 64 + r] = b.i; }
-    }
+    warp_select(lv[warp], li[warp], count, k, [&](int r, Cand b) { mv[r] = b.i >= 0 ? b.v : -INFINITY; mi[r] = b.i; });
   } else {   // pathological ties: k passes over the registers
     uint32_t removed = 0;
     for (int r = 0; r < k; ++r) {
@@ -146,26 +165,14 @@ __device__ __forceinline__ void stage1_item(const float* __restrict__ scores, in
       }
       const Cand b = warp_argmax(c);
       if (b.i >= 0 && b.i == c.i) removed |= 1u << cj;
-      if (lane == 0) { wv[warp * 64 + r] = b.i >= 0 ? b.v : -INFINITY; wi[warp * 64 + r] = b.i; }
+      if (lane == 0) { mv[r] = b.i >= 0 ? b.v : -INFINITY; mi[r] = b.i; }
     }
   }
   __syncthreads();
   if (warp == 0) {
     int* oi = cand_idx + (static_cast<size_t>(q) * total_segments + seg0 + seg) * k;
     float* os = cand_score + (static_cast<size_t>(q) * total_segments + seg0 + seg) * k;
-    for (int r = 0; r < k; ++r) {
-      Cand c{-INFINITY, -1};
-      int where = -1;
-      for (int w = 0; w < kWarps; ++w)
-        for (int t = lane; t < k; t += 32) {
-          const int at = w * 64 + t;
-          if (better(wv[at], wi[at], c.v, c.i)) { c.v = wv[at]; c.i = wi[at]; where = at; }
-        }
-      const Cand b = warp_argmax(c);
-      if (where >= 0 && b.i >= 0 && c.i == b.i) wi[where] = -1;
-      __syncwarp();
-      if (lane == 0) { oi[r] = b.i; os[r] = b.i >= 0 ? b.v : -INFINITY; }
-    }
+    warp_select(wv, wi, kWarps * k, k, [&](int r, Cand b) { oi[r] = b.i; os[r] = b.i >= 0 ? b.v : -INFINITY; });
   }
 }
 
@@ -236,7 +243,6 @@ scores_small_kernel(const __half* __restrict__ queries, const __half* __restrict
 __device__ __forceinline__ void stage2_item(const int* __restrict__ cand_idx, const float* __restrict__ cand_score,
                                             int ncand, int k, int id_offset, int* __restrict__ out_idx,
                                             float* __restrict__ out_score, int q) {
-  __shared__ Cand red[kSelThreads / 32];
   extern __shared__ uint8_t dyn[];
   float* sv = reinterpret_cast<float*>(dyn);
   int* si = reinterpret_cast<int*>(sv + ncand);
@@ -245,19 +251,10 @@ __device__ __forceinline__ void stage2_item(const int* __restrict__ cand_idx, co
     si[c] = cand_idx[static_cast<size_t>(q) * ncand + c];
   }
   __syncthreads();
-  for (int r = 0; r < k; ++r) {   // each round ends on a barrier
-    Cand c{-INFINITY, -1};
-    int where = -1;
-    for (int j = threadIdx.x; j < ncand; j += kSelThreads)
-      if (better(sv[j], si[j], c.v, c.i)) { c.v = sv[j]; c.i = si[j]; where = j; }
-    const Cand b = block_argmax(c, red);
-    if (where >= 0 && c.i == b.i && b.i >= 0) si[where] = -1;  // unique local ids: exactly one owner
-    if (threadIdx.x == 0) {
-      out_idx[static_cast<size_t>(q) * k + r] = b.i >= 0 ? b.i + id_offset : -1;
-      out_score[static_cast<size_t>(q) * k + r] = b.i >= 0 ? b.v : -INFINITY;
-    }
-    __syncthreads();
-  }
+  block_select(sv, si, ncand, k, [&](int r, Cand b) {
+    out_idx[static_cast<size_t>(q) * k + r] = b.i >= 0 ? b.i + id_offset : -1;
+    out_score[static_cast<size_t>(q) * k + r] = b.i >= 0 ? b.v : -INFINITY;
+  });
 }
 
 // one CTA per query
@@ -284,11 +281,10 @@ __global__ void pack_pairs_kernel(const int* __restrict__ idx, const float* __re
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = make_int2(__float_as_int(score[i]), idx[i]);
 }
-// merge of G per-shard lists in the packed form: pairs [G][B][k]
+// merge of G per-shard lists in the packed form: pairs [G][B][k]; global ids are unique across shards
 __global__ void __launch_bounds__(kSelThreads)
 merge_packed_kernel(const int2* __restrict__ pairs, int G, int B, int k, int* __restrict__ out_idx,
                     float* __restrict__ out_score) {
-  __shared__ Cand red[kSelThreads / 32];
   extern __shared__ uint8_t dyn[];
   float* sv = reinterpret_cast<float*>(dyn);
   int* si = reinterpret_cast<int*>(sv + G * k);
@@ -300,30 +296,43 @@ merge_packed_kernel(const int2* __restrict__ pairs, int G, int B, int k, int* __
     si[c] = e.y;
   }
   __syncthreads();
-  for (int r = 0; r < k; ++r) {
-    Cand c{-INFINITY, -1};
-    int where = -1;
-    for (int j = threadIdx.x; j < G * k; j += kSelThreads)
-      if (better(sv[j], si[j], c.v, c.i)) { c.v = sv[j]; c.i = si[j]; where = j; }
-    const Cand b = block_argmax(c, red);
-    if (where >= 0 && c.i == b.i && b.i >= 0) si[where] = -1;   // global ids are unique across shards
-    if (threadIdx.x == 0) {
-      out_idx[static_cast<size_t>(q) * k + r] = b.i;
-      out_score[static_cast<size_t>(q) * k + r] = b.i >= 0 ? b.v : -INFINITY;
-    }
-    __syncthreads();
-  }
+  block_select(sv, si, G * k, k, [&](int r, Cand b) {
+    out_idx[static_cast<size_t>(q) * k + r] = b.i;
+    out_score[static_cast<size_t>(q) * k + r] = b.i >= 0 ? b.v : -INFINITY;
+  });
 }
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-int sm_count() {   // of the current device; the devices of one process are taken to be alike
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-      return 1;
+int sm_count() { return std::max(1, device_sms()); }   // a launch takes at least one CTA
+
+// static shared memory of a kernel, asked of the runtime once per kernel
+int static_smem(const void* kernel, size_t* bytes) {
+  static std::mutex mu;
+  static std::unordered_map<const void*, size_t> known;
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = known.find(kernel);
+  if (it == known.end()) {
+    cudaFuncAttributes a;
+    SRB_CUDA_CHECK(cudaFuncGetAttributes(&a, kernel));
+    it = known.emplace(kernel, a.sharedSizeBytes).first;
   }
-  return num_sms;
+  *bytes = it->second;
+  return 0;
+}
+
+// Launches kernel<<<grid, block, smem, stream>>>(args...), checks it and counts it.  A kernel whose static and smem
+// bytes of dynamic shared memory exceed 48 KB is opted in first (static shared memory alone never does).  Nothing here
+// synchronises or allocates, so the launches of a scan can be captured into a CUDA graph.
+template <typename... P, typename... A>
+int launch(void (*kernel)(P...), dim3 grid, int block, size_t smem, cudaStream_t stream, A... args) {
+  size_t fixed = 0;
+  if (smem > 0 && static_smem(reinterpret_cast<const void*>(kernel), &fixed)) return -1;
+  if (smem + fixed > kDefaultSmem)
+    SRB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  kernel<<<grid, block, smem, stream>>>(args...);
+  SRB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
+  return 0;
 }
 inline int chunk_rows(int B, int N) {
   // keep the score buffer <= 1 GiB; multiple of the stage-1 segment
@@ -332,6 +341,20 @@ inline int chunk_rows(int B, int N) {
   if (rows < static_cast<size_t>(kSegment)) rows = kSegment;
   const size_t need = align_up(static_cast<size_t>(N), kSegment);
   return static_cast<int>(rows < need ? rows : need);
+}
+
+// Workspace of the two-stage route, byte offsets: the score chunk [B, chunk_rows] at 0, then cand_idx and cand_score
+// [B, candidates]
+struct TwoStageLayout {
+  size_t cand_idx = 0, cand_score = 0, total = 0;
+};
+TwoStageLayout two_stage_layout(const CachePlan& p, int B) {
+  const size_t cands = align_up(static_cast<size_t>(B) * p.candidates * 4, 256);
+  TwoStageLayout L;
+  L.cand_idx = align_up(static_cast<size_t>(B) * p.chunk_rows * 4, 256);
+  L.cand_score = L.cand_idx + cands;
+  L.total = L.cand_score + cands;
+  return L;
 }
 
 }  // namespace
@@ -350,8 +373,7 @@ static bool plan_two_stage(CachePlan& p, int B, int N, int k) {
   p.candidates = p.segments * k;
   p.stage2_smem = static_cast<size_t>(p.candidates) * 8;
   if (p.stage2_smem > kStage2SmemMax) return false;
-  p.workspace_bytes = align_up(static_cast<size_t>(B) * p.chunk_rows * 4, 256) +
-                      2 * align_up(static_cast<size_t>(B) * p.candidates * 4, 256);
+  p.workspace_bytes = two_stage_layout(p, B).total;
   return true;
 }
 
@@ -389,12 +411,8 @@ int cache_topk(cudaStream_t stream, const __half* queries, int B, const __half* 
     return -1;
   }
   uint8_t* ws = static_cast<uint8_t*>(workspace);
-  if (plan.route == CACHE_EMPTY) {
-    select_stage2<<<B, kSelThreads, 0, stream>>>(nullptr, nullptr, 0, k, id_offset, out_idx, out_score);
-    SRB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
-    return 0;
-  }
+  if (plan.route == CACHE_EMPTY)
+    return launch(select_stage2, B, kSelThreads, 0, stream, nullptr, nullptr, 0, k, id_offset, out_idx, out_score);
   if (plan.route == CACHE_FUSED) {
     // Scores never leave the SM: the GEMM's epilogue keeps a running top-8 per (query, CTA) and only those short lists
     // are written (B x <= 148 x 8 pairs); no 1 GiB score chunks, no selection pass over them.
@@ -409,70 +427,49 @@ int cache_topk(cudaStream_t stream, const __half* queries, int B, const __half* 
     if (gemm_f16(stream, g)) return -1;
     if (lists <= 0 || lists > kFusedLists) { fprintf(stderr, "[srb200] cache_topk: %d lists\n", lists); return -1; }
     const int ncand = lists * kFusedK;
-    select_stage2<<<B, kSelThreads, static_cast<size_t>(ncand) * 8, stream>>>(l_idx, l_score, ncand, k, id_offset, out_idx, out_score);
-    SRB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
-    return 0;
+    return launch(select_stage2, B, kSelThreads, static_cast<size_t>(ncand) * 8, stream, l_idx, l_score, ncand, k,
+                  id_offset, out_idx, out_score);
   }
   const int chunk = plan.chunk_rows, segs = plan.segments;
+  const TwoStageLayout W = two_stage_layout(plan, B);
   float* scores = reinterpret_cast<float*>(ws);
-  int* cand_idx = reinterpret_cast<int*>(ws + align_up(static_cast<size_t>(B) * chunk * 4, 256));
-  float* cand_score = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(cand_idx) +
-                                               align_up(static_cast<size_t>(B) * plan.candidates * 4, 256));
+  int* cand_idx = reinterpret_cast<int*>(ws + W.cand_idx);
+  float* cand_score = reinterpret_cast<float*>(ws + W.cand_score);
   for (int row0 = 0; row0 < N; row0 += chunk) {
     const int n = (N - row0) < chunk ? (N - row0) : chunk;
     const int n_pad = static_cast<int>(align_up(n, 64));  // cache allocation is padded to 256 rows
     if (plan.route == CACHE_GEMV) {
       const int grid = sm_count() * 8;   // 8 CTAs x 8 warps per SM: enough loads in flight to cover the HBM latency
-      const size_t smem = static_cast<size_t>(B) * D * 4;
-      const __half* cw = cache + static_cast<size_t>(row0) * D;
-      switch (B) {
-        case 1: scores_small_kernel<1><<<grid, 256, smem, stream>>>(queries, cw, n, D, chunk, scores); break;
-        case 2: scores_small_kernel<2><<<grid, 256, smem, stream>>>(queries, cw, n, D, chunk, scores); break;
-        case 3: scores_small_kernel<3><<<grid, 256, smem, stream>>>(queries, cw, n, D, chunk, scores); break;
-        default: scores_small_kernel<4><<<grid, 256, smem, stream>>>(queries, cw, n, D, chunk, scores); break;
-      }
-      SRB_CUDA_CHECK(cudaGetLastError());
-      note_launch();
+      const auto gemv = B == 1 ? scores_small_kernel<1> : B == 2 ? scores_small_kernel<2>
+                      : B == 3 ? scores_small_kernel<3> : scores_small_kernel<4>;
+      if (launch(gemv, grid, 256, static_cast<size_t>(B) * D * 4, stream, queries, cache + static_cast<size_t>(row0) * D,
+                 n, D, chunk, scores))
+        return -1;
     } else {
       GemmDesc g;
       g.M = B; g.N = n_pad; g.K = D; g.A = queries; g.W = cache + static_cast<size_t>(row0) * D;
       g.out = scores; g.ldo = chunk; g.epi = EPI_RESID; g.resid = nullptr; g.ldr = chunk;
       if (gemm_f16(stream, g)) return -1;
     }
-    const dim3 grid((n + kSegment - 1) / kSegment, B);
-    select_stage1<<<grid, kSelThreads, 0, stream>>>(scores, chunk, n, row0, valid, k, row0 / kSegment, segs, cand_idx,
-                                                    cand_score);
-    SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
+    if (launch(select_stage1, dim3((n + kSegment - 1) / kSegment, B), kSelThreads, 0, stream, scores, chunk, n, row0,
+               valid, k, row0 / kSegment, segs, cand_idx, cand_score))
+      return -1;
   }
-  const size_t smem = plan.stage2_smem;
-  if (smem + kSelStaticSmem > kDefaultSmem)
-    SRB_CUDA_CHECK(cudaFuncSetAttribute(select_stage2, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  select_stage2<<<B, kSelThreads, smem, stream>>>(cand_idx, cand_score, plan.candidates, k, id_offset, out_idx, out_score);
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
-  return 0;
+  return launch(select_stage2, B, kSelThreads, plan.stage2_smem, stream, cand_idx, cand_score, plan.candidates, k,
+                id_offset, out_idx, out_score);
 }
 
 int cache_pack_pairs(cudaStream_t stream, const int* idx, const float* score, int n, void* pairs_out) {
   if (n <= 0) return 0;
-  pack_pairs_kernel<<<(n + 255) / 256, 256, 0, stream>>>(idx, score, n, static_cast<int2*>(pairs_out));
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
-  return 0;
+  return launch(pack_pairs_kernel, (n + 255) / 256, 256, 0, stream, idx, score, n, static_cast<int2*>(pairs_out));
 }
 
 int cache_merge_packed(cudaStream_t stream, const void* pairs, int G, int B, int k, int* out_idx, float* out_score) {
   if (B <= 0) return 0;
   const size_t smem = static_cast<size_t>(G) * k * 8;
   if (smem > kDefaultSmem) { fprintf(stderr, "[srb200] cache_merge_packed: G * k = %d too large\n", G * k); return -1; }
-  if (smem + kSelStaticSmem > kDefaultSmem)
-    SRB_CUDA_CHECK(cudaFuncSetAttribute(merge_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  merge_packed_kernel<<<B, kSelThreads, smem, stream>>>(static_cast<const int2*>(pairs), G, B, k, out_idx, out_score);
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
-  return 0;
+  return launch(merge_packed_kernel, B, kSelThreads, smem, stream, static_cast<const int2*>(pairs), G, B, k, out_idx,
+                out_score);
 }
 
 // ---- exact caches (sr_cache_create_exact): the scores of the reference's embeddingDotProduct on the fp32 rows and query
@@ -761,20 +758,14 @@ int cache_topk_exact(cudaStream_t stream, const float* queries32, __half* querie
   float* cand_score = reinterpret_cast<float*>(ws + L.cand_score);
   int* fb_count = reinterpret_cast<int*>(ws + L.fb_list);
   int* fb_list = fb_count + 1;
-  exact_query_f16_kernel<<<B, 256, 0, stream>>>(queries32, D, queries16);
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
-  if (cache_topk(stream, queries16, B, cache, valid, N, D, L.kc, 0, cand_idx, cand_score, ws, L.scan.workspace_bytes))
+  if (launch(exact_query_f16_kernel, B, 256, 0, stream, queries32, D, queries16) ||
+      cache_topk(stream, queries16, B, cache, valid, N, D, L.kc, 0, cand_idx, cand_score, ws, L.scan.workspace_bytes))
     return -1;
   SRB_CUDA_CHECK(cudaMemsetAsync(fb_count, 0, 4, stream));
-  const size_t qsmem = static_cast<size_t>(D) * 4;
-  auto band_kernel = sum_rule == 0 ? exact_band_kernel<0> : exact_band_kernel<1>;
-  if (qsmem > kDefaultSmem - 2048)
-    SRB_CUDA_CHECK(cudaFuncSetAttribute(band_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(qsmem)));
-  band_kernel<<<B, kExactCand, qsmem, stream>>>(queries32, cache32, D, rmax, cand_idx, cand_score, L.kc, k, id_offset,
-                                                out_idx, out_score, fb_list, fb_count, path, band, eps);
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
+  if (launch(sum_rule == 0 ? exact_band_kernel<0> : exact_band_kernel<1>, B, kExactCand, static_cast<size_t>(D) * 4,
+             stream, queries32, cache32, D, rmax, cand_idx, cand_score, L.kc, k, id_offset, out_idx, out_score, fb_list,
+             fb_count, path, band, eps))
+    return -1;
   if (N == 0) return 0;   // every query of an empty store is certified
   // Exhaustive exact scan of the fallback queries only: Go-order scores in chunks, then the two-stage selection of
   // cache_topk over them, then the results back to their query rows.  The number of fallback queries stays on the device
@@ -785,36 +776,25 @@ int cache_topk_exact(cudaStream_t stream, const float* queries32, __half* querie
   static const int stage1_grid = one_wave(select_stage1_counted, kSelThreads);
   const CachePlan& P = L.fallback;
   const int chunk = P.chunk_rows;
+  const TwoStageLayout W = two_stage_layout(P, B);
   float* scores = reinterpret_cast<float*>(ws);
-  int* sel_idx = reinterpret_cast<int*>(ws + align_up(static_cast<size_t>(B) * chunk * 4, 256));
-  float* sel_score = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sel_idx) +
-                                              align_up(static_cast<size_t>(B) * P.candidates * 4, 256));
+  int* sel_idx = reinterpret_cast<int*>(ws + W.cand_idx);
+  float* sel_score = reinterpret_cast<float*>(ws + W.cand_score);
   int* fb_idx = reinterpret_cast<int*>(ws + L.fb_idx);
   float* fb_score = reinterpret_cast<float*>(ws + L.fb_score);
-  auto scores_kernel = sum_rule == 0 ? exact_scores_kernel<0> : exact_scores_kernel<1>;
   for (int row0 = 0; row0 < N; row0 += chunk) {
     const int n = (N - row0) < chunk ? (N - row0) : chunk;
-    scores_kernel<<<scores_grid[sum_rule], 256, 0, stream>>>(queries32, fb_list, fb_count,
-                                                             cache32 + static_cast<size_t>(row0) * D, n, D, chunk, scores);
-    SRB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
-    select_stage1_counted<<<stage1_grid, kSelThreads, 0, stream>>>(scores, chunk, n, row0, valid, k, row0 / kSegment,
-                                                                   P.segments, sel_idx, sel_score, fb_count);
-    SRB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
+    if (launch(sum_rule == 0 ? exact_scores_kernel<0> : exact_scores_kernel<1>, scores_grid[sum_rule], 256, 0, stream,
+               queries32, fb_list, fb_count, cache32 + static_cast<size_t>(row0) * D, n, D, chunk, scores) ||
+        launch(select_stage1_counted, stage1_grid, kSelThreads, 0, stream, scores, chunk, n, row0, valid, k,
+               row0 / kSegment, P.segments, sel_idx, sel_score, fb_count))
+      return -1;
   }
-  const size_t smem = P.stage2_smem;
-  if (smem + kSelStaticSmem > kDefaultSmem)
-    SRB_CUDA_CHECK(cudaFuncSetAttribute(select_stage2_counted, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-  select_stage2_counted<<<sm_count(), kSelThreads, smem, stream>>>(sel_idx, sel_score, P.candidates, k, id_offset, fb_idx,
-                                                                   fb_score, fb_count);
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
-  exact_scatter_kernel<<<sm_count(), 64, 0, stream>>>(fb_list, fb_count, k, fb_idx, fb_score, out_idx, out_score);
-  SRB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
-  return 0;
+  if (launch(select_stage2_counted, sm_count(), kSelThreads, P.stage2_smem, stream, sel_idx, sel_score, P.candidates, k,
+             id_offset, fb_idx, fb_score, fb_count))
+    return -1;
+  return launch(exact_scatter_kernel, sm_count(), 64, 0, stream, fb_list, fb_count, k, fb_idx, fb_score, out_idx,
+                out_score);
 }
 
 }  // namespace srb

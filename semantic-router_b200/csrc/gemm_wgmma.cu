@@ -1080,8 +1080,8 @@ int gemm_cluster_size(int epi, int N, int K) {
   return share_a && ((N + BN - 1) / BN) % 2 == 0 && ((N + BNW - 1) / BNW) % 2 == 0 ? 2 : 1;
 }
 
-static int device_sms() {
-  static int num_sms = 0;  // all devices of one box are the same part
+int device_sms() {
+  static int num_sms = 0;
   if (!num_sms) {
     int dev = 0, n = 0;
     SRB_CUDA_CHECK(cudaGetDevice(&dev));

@@ -12,6 +12,9 @@ void note_launch(int n = 1);
 // SRB_PDL=1 turns programmatic dependent launch on for the GEMM kernels (default off)
 bool pdl_enabled();
 long long launches_total();
+// SMs of the current device (gemm_wgmma.cu), asked once: the devices of one process are taken to be alike.  -1 when
+// the runtime cannot tell.
+int device_sms();
 
 // Sequences one attention launch takes: they sit in gridDim.z, whose limit is 65 535; the attention launchers (here and in
 // precise.cu) run larger packs as slices of at most this many sequences.
